@@ -1,8 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the CHGNet hot path (E + F + sigma) on B200.
+"""bench.py — throughput of the CHGNet hot path (E + F + sigma) on H100.
 
-Contract (see task statement): ``python bench.py --gpus N --steps K --warmup W`` prints ONE
-JSON line.  A "step" is one pass of the hot path (forward + the force/stress reverse pass)
+``python bench.py --gpus N --steps K --warmup W`` prints ONE JSON line.  A "step" is one pass of the hot path (forward + the force/stress reverse pass)
 over one batch of synthetic CrystalGraphs.
 
 Workloads (SURVEY.md §8d, BASELINE.json `configs`):
@@ -23,6 +22,10 @@ roofline   AtomConv scatter-reduce kernel (chg_segment_sum over center-sorted me
 cpu_baseline / --impl reference
            the oracle port of the reference's torch CPU path (oracle/chgnet_oracle.py) on
            the host cores, on a bounded sample of the same workload
+
+--dump-outputs DIR  after the timed steps, writes what the timed path returned in its last step as DIR/<name>.npy
+           (c1..c4: energy, force, stress of the resident kernel path; c5: the loss terms and the flat parameter
+           gradient of the last fine-tuning step).  Inputs are seeded, so two builds can be compared output for output.
 
 Multi-GPU: one process per GPU (torchrun).  The global batch (N x the workload's batch) is assigned to
 ranks by `partition_graphs` (greedy LPT on edges + 2.5 x angles, chgnet_b200/batch.py); no device-path
@@ -73,7 +76,7 @@ L2_NOTE = "256 MiB buffer written, then 256 MiB read (clean lines), between time
 
 
 def bench_config(workload: str, desc: str, per_job: dict, world: int, task: str = "efs") -> dict:
-    """The `config` object, IDENTICAL in the product arm and in the reference arm (the driver compares them):
+    """The `config` object, IDENTICAL in the product arm and in the reference arm (the two lines are compared):
     the workload, the task, the whole-job sizes, the weights and how the L2 is treated between timed steps."""
     return {"workload": f"{workload}: {desc}", "task": task, "whole_job": per_job, "weights": "CHGNet 0.3.0",
             "l2": L2_NOTE, "parallelism": f"graph-sharded x{world} (LPT partition of the global batch), no inference collective"}
@@ -187,6 +190,7 @@ def run_train(args, rank: int, world: int, local_rank: int, light: bool = False)
     tg_dev = trainer._targets(lab, batch.atoms_per_graph, dev)
 
     ar_events: list = []
+    last_grad: list = [None]
 
     def step_resident():
         engine = model._get_engine()  # re-packs the weights the previous Adam step changed
@@ -201,6 +205,7 @@ def run_train(args, rank: int, world: int, local_rank: int, light: bool = False)
         trainer.step_count += 1
         K.adam_step(trainer.flat, fg, trainer.exp_avg, trainer.exp_avg_sq, trainer.lr, 0.9, 0.999, 1e-8, 0.0, trainer.step_count)
         trainer.refresh_packed_weights()
+        last_grad[0] = fg
         return report_
 
     n_steps = min(args.steps, 5) if light else args.steps
@@ -240,6 +245,9 @@ def run_train(args, rank: int, world: int, local_rank: int, light: bool = False)
                       "steps": n_steps, "workload": f"c5: {desc}", "per_gpu": c}
     if light:
         return collective
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"flat_grad": last_grad[0],
+                                         **{f"loss_{k}": np.float64(v) for k, v in rep_last.items() if np.isscalar(v)}})
 
     # end to end: Trainer.train_step from host graphs + host labels, report read back every step
     targets = lab
@@ -317,6 +325,15 @@ def run_train(args, rank: int, world: int, local_rank: int, light: bool = False)
         "last_report": rep_last, "breakdown": breakdown, "kernel_shares": shares}), flush=True)
     if world > 1:
         dist.barrier()
+
+
+def dump_outputs(dirname: str, arrays: dict) -> None:
+    """--dump-outputs: one .npy per array (float32 / float64), written by rank 0 only."""
+    os.makedirs(dirname, exist_ok=True)
+    for name, v in arrays.items():
+        a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        np.save(os.path.join(dirname, f"{name}.npy"), a)
 
 
 def counts(graphs):
@@ -400,7 +417,7 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"  # H100 SXM data sheet
 
 
 # ------------------------------------------------------------------------------------------
@@ -488,8 +505,8 @@ def run_reference(args, rank: int, world: int) -> None:
 
 # ------------------------------------------------------------------------------------------
 class L2Flush:
-    """Evicts everything of ours from the 126 MB L2 between timed iterations: writes a 256 MiB
-    buffer (the rule of the task statement), then streams a second 256 MiB buffer through with a
+    """Evicts everything of ours from the 50 MB L2 between timed iterations: writes a 256 MiB
+    buffer, then streams a second 256 MiB buffer through with a
     read so that the cache is left holding CLEAN lines — otherwise the timed kernel also pays
     for the write-back of the flush buffer's dirty lines."""
 
@@ -595,11 +612,12 @@ def infer_leg(model, graphs, dev, local_rank: int, world: int, steps: int, warmu
     launches0 = K.launches
     elapsed_ms = 0.0
     t_wall0 = time.perf_counter()
+    last = None
     for _ in range(steps):
         flush()
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
-        step_resident()
+        last = step_resident()
         e.record()
         e.synchronize()
         elapsed_ms += s.elapsed_time(e)
@@ -629,7 +647,8 @@ def infer_leg(model, graphs, dev, local_rank: int, world: int, steps: int, warmu
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return {"ms_per_step": float(t[0].item()) / steps, "e2e_ms_per_step": float(t[1].item()) / steps, "launches": int(launches),
-            "clocks": clocks, "wall_ms": wall_ms, "h2d": h2d, "d2h": d2h, "preds": preds, "batch": batch}
+            "clocks": clocks, "wall_ms": wall_ms, "h2d": h2d, "d2h": d2h, "preds": preds, "batch": batch,
+            "last": dict(zip(("energy", "force", "stress"), last))}
 
 
 def md_leg(model, dev, steps: int = 20) -> dict:
@@ -680,11 +699,7 @@ def scatter_roofline(K, batch, workload: str, dev) -> dict:
     peaks, peak_kind = measured_peaks()
     sc_ms, sc_bytes = time_scatter_kernel(K, batch, width=128)
     achieved = sc_bytes / (sc_ms * 1e-3) / 1e9
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "scatter_traffic.json")
-    if os.path.exists(tpath):  # dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu capture
-        with open(tpath) as f:
-            traffic = json.load(f).get(workload + "_w128", {}).get("dram_bytes_per_launch")
+    traffic = None  # measured DRAM bytes per launch: not available without a hardware-counter profiler
     ms64, b64 = time_scatter_kernel(K, batch, width=64)
     return {"kernel": "segment_sum_kernel<128> (AtomConv scatter-reduce of the reverse pass: dE/dpre rows -> atoms)", "bound": "hbm",
             "achieved": round(achieved, 1), "peak": peaks["hbm_gbs"], "peak_kind": f"{peak_kind} copy bandwidth",
@@ -744,7 +759,7 @@ def run_ours(args, rank: int, world: int, local_rank: int) -> None:
     engine = model._get_engine()
     K = engine.K
 
-    if args.scatter_only:  # ncu capture target: only the AtomConv scatter-reduce launches
+    if args.scatter_only:  # profiler target: only the AtomConv scatter-reduce launches
         batch = build_batch(graphs, dev, with_reverse=True)
         ms, nbytes = time_scatter_kernel(K, batch, n_iter=5)
         print(json.dumps({"scatter_only": True, "us_per_launch": ms * 1e3, "algorithmic_bytes": nbytes}))
@@ -753,6 +768,8 @@ def run_ours(args, rank: int, world: int, local_rank: int) -> None:
     leg = infer_leg(model, graphs, dev, local_rank, world, args.steps, args.warmup, replay=args.graph_replay)
     batch = leg["batch"]
     ms_per_step, e2e_ms_per_step = leg["ms_per_step"], leg["e2e_ms_per_step"]
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, leg["last"])
 
     # ---------------- the same resident step replayed as ONE CUDA graph (NativeForward.replay) ----------------
     graph_replay = None
@@ -825,10 +842,10 @@ def run_ours(args, rank: int, world: int, local_rank: int) -> None:
         us = fa["ms"] / fa["calls"] * 1e3
         nb = (268 + 512) * c["directed_edges"] + 512 * c["atoms"]
         roofline["fused_forward_atom_conv"] = {
-            "kernel": "gated_ws_fwd_kernel<ATOM> + seg_stitch_kernel (message + aggregation, tcgen05)", "us_per_launch": round(us, 2),
+            "kernel": "gated_ws_fwd_kernel<ATOM> + seg_stitch_kernel (message + aggregation, wgmma)", "us_per_launch": round(us, 2),
             "compulsory_bytes": nb, "bytes_formula": "(268 + 512 saved p) * E_d + 512 * N",
             "achieved": round(nb / (us * 1e-6) / 1e9, 1), "frac": round(nb / (us * 1e-6) / 1e9 / peaks["hbm_gbs"], 4),
-            "note": "latency-bound (gathers + MUFU), not bandwidth-bound: see profiles/ for tensor-pipe % and DRAM bytes"}
+            "note": "compulsory bytes over kernel time; the kernel also waits on gathers and MUFU, so this is not a bandwidth bound"}
 
     # ---------------- the 10,000-atom cell (BASELINE configs[3]) as an extra key ----------------
     c4 = None
@@ -913,7 +930,7 @@ def run_ours(args, rank: int, world: int, local_rank: int) -> None:
                   "vs": f"oracle port (fp32 torch CPU = the reference's arithmetic) on {len(sample)} graph(s) of this run",
                   "tolerance": {"e": 1e-4, "f": 1e-3, "s": 1e-3},
                   "ok": bool(worst("e") < 1e-4 and worst("f") < 1e-3 and worst("s") < 1e-3)}
-        # the realistic incumbent (SURVEY.md §8d): the reference's torch ops on the SAME B200 (stock PyTorch CUDA)
+        # the realistic incumbent (SURVEY.md §8d): the reference's torch ops on the SAME GPU (stock PyTorch CUDA)
         if args.workload != "c4":
             try:
                 for _ in range(2):
@@ -926,7 +943,7 @@ def run_ours(args, rank: int, world: int, local_rank: int) -> None:
                 dtc = (time.perf_counter() - t0) / 3
                 torch_cuda = {"value": c["graphs"] / dtc, "unit": "structures/s", "ms_per_step": dtc * 1e3,
                               "what": "oracle port = the reference's torch ops and per-graph batching loop, stock PyTorch "
-                                      "CUDA on the same B200, fp32, host graphs in / numpy out, this rank's share (compare with e2e / n_gpus)"}
+                                      "CUDA on the same GPU, fp32, host graphs in / numpy out, this rank's share (compare with e2e / n_gpus)"}
             except Exception as exc:  # reported, never fatal for the bench line
                 torch_cuda = {"unavailable": repr(exc)[:200]}
 
@@ -966,7 +983,9 @@ def main() -> None:
     ap.add_argument("--no-collective", action="store_true", help="N > 1: skip the c5 all-reduce leg")
     ap.add_argument("--no-md", action="store_true", help="skip the MD sub-leg of the c4 extra leg")
     ap.add_argument("--graph-replay", action="store_true", help="kernel-path leg: replay one captured CUDA graph of chg_forward per step")
-    ap.add_argument("--scatter-only", action="store_true", help="run only the AtomConv scatter kernel timing (ncu target)")
+    ap.add_argument("--scatter-only", action="store_true", help="run only the AtomConv scatter kernel timing")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the timed path's outputs of its last step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))

@@ -1,4 +1,4 @@
-"""chgnet_b200 — B200-native hot path for CHGNet (forward + force/stress backward)."""
+"""chgnet_b200 — H100-native hot path for CHGNet (forward + force/stress backward)."""
 from __future__ import annotations
 
 from typing import Literal

@@ -119,7 +119,7 @@ class CudaKernels:
         current device is (``CHGNet.load(use_device='cuda:1')`` in a process sitting on cuda:0)."""
         self.lib = load_library()
         if not torch.cuda.is_available():
-            raise ChgnetB200Error("chgnet_b200 needs a CUDA device (B200 / sm_100a); none is visible")
+            raise ChgnetB200Error("chgnet_b200 needs a CUDA device (H100 / sm_90a); none is visible")
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if dev.type != "cuda":
             raise ChgnetB200Error(f"chgnet_b200 kernels run on CUDA devices only (got {dev})")
@@ -144,9 +144,9 @@ class CudaKernels:
                 raise ChgnetB200Error("kernel arguments must be contiguous CUDA tensors")
 
     def set_option(self, name: str, value: int) -> None:
-        """A/B switches (include/chgnet_b200.h): 'linear_impl' 0 FFMA | 1 tcgen05 | 2 tcgen05+TMA rows |
-        3 warp-specialised tcgen05 + TMA tensor maps (default),
-        'gated_impl' 3 fused warp-specialised tcgen05 message + aggregation (default) | 0 FFMA 4x8 | 1 tcgen05 | 2 FFMA 8x8."""
+        """A/B switches (include/chgnet_b200.h): 'linear_impl' 0 FFMA | 1 wgmma | 2 wgmma (as 1) |
+        3 warp-specialised wgmma + TMA tensor maps (default),
+        'gated_impl' 3 fused warp-specialised wgmma message + aggregation (default) | 0 FFMA 4x8 | 1 wgmma | 2 FFMA 8x8."""
         if self.lib.chg_set_option(name.encode(), int(value)) != 0:
             raise ChgnetB200Error(self.lib.chg_last_error().decode())
 

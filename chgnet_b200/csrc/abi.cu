@@ -24,10 +24,10 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 int sm_count() {  // of the CURRENT device (cached per device ordinal)
   static std::atomic<int> cache[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;  // B200
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;  // H100 SXM
   int n = cache[dev].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -37,9 +37,9 @@ int sm_count() {  // of the CURRENT device (cached per device ordinal)
 namespace chg {
 namespace {
 // implementation switches.  Defaults follow the measured A/B (profiles/): the dense feature-mixing GEMM runs on
-// the warp-specialised tcgen05 kernel (linear_impl 3); the AtomConv / BondConv message + aggregation runs as the
-// fused warp-specialised tcgen05 kernel of gated_ws.cu (gated_impl 3) wherever the engine calls the fused entry
-// points; gated_impl 0..2 select the older unfused kernels (FFMA 4x8 / tcgen05 / FFMA 8x8) for A/B runs.
+// the warp-specialised wgmma kernel (linear_impl 3); the AtomConv / BondConv message + aggregation runs as the
+// fused warp-specialised wgmma kernel of gated_ws.cu (gated_impl 3) wherever the engine calls the fused entry
+// points; gated_impl 0..2 select the older unfused kernels (FFMA 4x8 / wgmma / FFMA 8x8) for A/B runs.
 std::atomic<int> g_linear_impl{-1}, g_gated_impl{-1}, g_wgrad_impl{-1}, g_ws_min_rows{-1}, g_segsum_unroll{-1}, g_segsum_s{-1};
 int env_default(const char* name, int dflt) {
   const char* e = getenv(name);

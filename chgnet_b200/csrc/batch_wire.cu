@@ -70,8 +70,8 @@ using namespace chg;
 
 // Pinned staging memory for the packers.  write_combined != 0: cudaHostAllocWriteCombined - the packer's worker threads
 // only WRITE it (streaming stores, no cache lines left dirty in many cores' caches), and the copy engine reads it at
-// full PCIe rate: on the B200 hosts of this pool a 19 MiB buffer freshly written by 8 threads copies at 54 GB/s from
-// write-combined memory and at 8 GB/s from ordinary pinned memory (profiles/SUMMARY_r2.md).  Never read it on the CPU.
+// full PCIe rate (on the earlier Blackwell build's hosts a 19 MiB buffer freshly written by 8 threads copied at 54 GB/s
+// from write-combined memory and at 8 GB/s from ordinary pinned memory).  Never read it on the CPU.
 extern "C" int chg_host_alloc(int64_t bytes, int32_t write_combined, void** out) {
   CHG_CHECK_ARG(bytes > 0 && out != nullptr, "bad size or null pointer");
   CHG_CUDA(cudaHostAlloc(out, (size_t)bytes, write_combined ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
@@ -247,7 +247,7 @@ extern "C" int chg_pack_batch_wire(int32_t n_graphs, const int64_t* counts, cons
     if (Ed > 0) {
       CHG_CUDA(cudaMemcpyAsync(img_dev, img_host, (size_t)Ed * 3, cudaMemcpyHostToDevice, stream));
       const int64_t n_img = Ed * 3;
-      expand_image_kernel<<<(unsigned)std::min<int64_t>((n_img + 255) / 256, 4 * 148), 256, 0, stream>>>(img_dev, fbuf_dev + n_flt, n_img);
+      expand_image_kernel<<<(unsigned)std::min<int64_t>((n_img + 255) / 256, 4 * sm_count()), 256, 0, stream>>>(img_dev, fbuf_dev + n_flt, n_img);
       CHG_LAUNCH_CHECK("chg_pack_batch_wire (expand_image)");
     }
   }
@@ -262,7 +262,7 @@ extern "C" int chg_pack_batch_wire(int32_t n_graphs, const int64_t* counts, cons
     int32_t* dev_center = ibuf_dev + 2 * N;
     int32_t* dev_d2u = dev_center + 2 * Ed;
     int32_t* dev_di = ibuf_dev + n_int_1;
-    derive_angle_columns_kernel<<<(unsigned)std::min<int64_t>((A + 255) / 256, 4 * 148), 256, 0, stream>>>(
+    derive_angle_columns_kernel<<<(unsigned)std::min<int64_t>((A + 255) / 256, 4 * sm_count()), 256, 0, stream>>>(
         dev_center, dev_d2u, dev_di, dev_di + A, dev_di + 2 * A, dev_di + 3 * A, dev_di + 4 * A, (int32_t)A);
     CHG_LAUNCH_CHECK("chg_pack_batch_wire (derive_angle_columns)");
   }

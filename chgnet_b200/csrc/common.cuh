@@ -1,4 +1,4 @@
-// Shared device/host helpers for the chgnet_b200 kernels (sm_100a).
+// Shared device/host helpers for the chgnet_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,7 +11,7 @@ namespace chg {
 void set_error(const char* fmt, ...);
 void count_launch();
 int sm_count();
-int linear_impl();  // 1 = tcgen05, 0 = FFMA
+int linear_impl();  // 0 = FFMA, 1..3 = tensor cores (wgmma)
 int gated_impl();
 int segsum_unroll();   // 4 or 8 input rows in flight per lane-group of chg_segment_sum
 int segsum_force_s();  // 0 = heuristic

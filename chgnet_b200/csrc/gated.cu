@@ -4,7 +4,7 @@
 // 238-249 (BondConv message), 348-360 (AngleUpdate), GatedMLP in
 // chgnet/model/functions.py:168-183.
 //
-// B200 design (DESIGN.md §3): the first Linear of every GatedMLP is split by input
+// Design (DESIGN.md §3): the first Linear of every GatedMLP is split by input
 // block and evaluated per ATOM / per BOND / per ANGLE by chg_linear (tensor cores); the
 // kernels here gather the 128-wide pre-activation rows of each edge/angle (3 for AtomConv,
 // 4 for BondConv / AngleUpdate), add them, run the two 64x64 second layers, and fuse
@@ -12,7 +12,7 @@
 //
 // This file is the FFMA implementation (64-row tiles in shared memory, register-tiled
 // GEMM; measured shared-memory-bandwidth bound, profiles/SUMMARY_r01.md).  gated_tc.cu
-// is the tcgen05 implementation of the same entry points; CHG_GATED_IMPL=ffma selects
+// is the tensor-core (wgmma) implementation of the same entry points; CHG_GATED_IMPL=ffma selects
 // this one.  One persistent CTA per resident slot; weights stay in shared memory.
 //
 // Thread map: 256 threads = 16 (ty) x 16 (tx); a thread owns rows ty*4..+3 and, in
@@ -369,7 +369,7 @@ __global__ void __launch_bounds__(NTHR, 2) gated_bwd_kernel(const BwdArgs a) {
 // gate) so that a thread's 8 rows x 8 columns share their A operand: (8 + 8) floats per 64 FMAs
 // = 1 byte per FMA.  The accumulators go back through the shared tile, and the epilogue runs in
 // the 16-lane-per-row layout (LayerNorm by shuffles, coalesced stores) as before.
-// Measured (B200, c4): 3-20 % SLOWER than the 4x8 kernels above — the extra tile round trip,
+// Measured on the earlier Blackwell build (c4): 3-20 % SLOWER than the 4x8 kernels above — the extra tile round trip,
 // two more block barriers and the lower occupancy of the reverse kernel cost more than the
 // operand traffic saves; the default stays on the 4x8 kernels.
 // =====================================================================================
@@ -782,7 +782,7 @@ extern "C" int chg_atom_conv_bwd(const float* pcn, const float* pe, const float*
   CHG_CHECK_ARG(pcn && pe && wag && center && nbr && d2u && save_p && g_agg && w2 && g_pre && g_w, "null pointer");
   BwdArgs a{pcn, pe, wag, center, nbr, d2u, n_edges, nullptr, save_p, g_agg, w2, ln, g_pre, g_w, nullptr, g_p, g_ln};
   const bool train = g_p != nullptr || g_ln != nullptr;
-  if (gated_impl() == 3 && !train && n_edges >= ws_min_rows()) return atom_conv_bwd_ws(a, as_stream(stream));  // warp-specialised tcgen05 (default)
+  if (gated_impl() == 3 && !train && n_edges >= ws_min_rows()) return atom_conv_bwd_ws(a, as_stream(stream));  // warp-specialised wgmma (default)
   if (gated_impl() == 1 && !train) return atom_conv_bwd_tc(a, as_stream(stream));
   if (gated_impl() == 2 && !train) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
     static int slots = 0;
@@ -817,7 +817,7 @@ extern "C" int chg_bond_conv_bwd(const float* save_pre, const float* save_p, con
   BwdArgs a{nullptr, nullptr, wbg, ang_i, ang_j, nullptr, n_angles, save_pre, save_p, g_agg, w2, ln,
             g_pre, gw_i, gw_j, g_p, g_ln};
   const bool train = g_p != nullptr || g_ln != nullptr;
-  if (gated_impl() == 3 && !train && n_angles >= ws_min_rows()) return bond_conv_bwd_ws(a, as_stream(stream));  // warp-specialised tcgen05 (default)
+  if (gated_impl() == 3 && !train && n_angles >= ws_min_rows()) return bond_conv_bwd_ws(a, as_stream(stream));  // warp-specialised wgmma (default)
   if (gated_impl() == 1 && !train) return bond_conv_bwd_tc(a, as_stream(stream));
   if (gated_impl() == 2 && !train) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
     static int slots = 0;

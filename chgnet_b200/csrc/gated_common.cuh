@@ -1,4 +1,4 @@
-// Shared pieces of the gated-MLP kernels (FFMA: gated.cu, tcgen05: gated_tc.cu).
+// Shared pieces of the gated-MLP kernels (FFMA: gated.cu, wgmma: gated_tc.cu).
 #pragma once
 #include "common.cuh"
 
@@ -8,7 +8,7 @@ namespace gated {
 constexpr int HS = 132;    // smem stride of a 128-wide row
 constexpr float LN_EPS = 1e-5f;
 }  // namespace gated
-// below this many rows the warp-specialised tcgen05 kernels hand the call to the FFMA kernels (launch-bound regime);
+// below this many rows the warp-specialised tensor-core kernels hand the call to the FFMA kernels (launch-bound regime);
 // chg_set_option("ws_min_rows", n) / env CHG_WS_MIN_ROWS, default 4096 (abi.cu)
 int ws_min_rows();
 namespace gated {
@@ -149,17 +149,17 @@ inline int resident_ctas(KernelT kernel, int smem_bytes) {
 
 #endif
 
-// entry points of the tcgen05 implementation (gated_tc.cu)
+// entry points of the unfused tensor-core implementation (gated_tc.cu)
 int atom_conv_fwd_tc(const FwdArgs& a, cudaStream_t stream);
 int bond_conv_fwd_tc(const FwdArgs& a, cudaStream_t stream);
 int atom_conv_bwd_tc(const BwdArgs& a, cudaStream_t stream);
 int bond_conv_bwd_tc(const BwdArgs& a, cudaStream_t stream);
 
-// warp-specialised tcgen05 reverse kernels (gated_ws.cu): same outputs as gated_bwd_kernel<MODE, false>
+// warp-specialised wgmma reverse kernels (gated_ws.cu): same outputs as gated_bwd_kernel<MODE, false>
 int atom_conv_bwd_ws(const BwdArgs& a, cudaStream_t stream);
 int bond_conv_bwd_ws(const BwdArgs& a, cudaStream_t stream);
 
-// warp-specialised tcgen05 message + aggregation kernels (gated_ws.cu); `parts` = strip partials workspace
+// warp-specialised wgmma message + aggregation kernels (gated_ws.cu); `parts` = strip partials workspace
 int atom_conv_fused_ws(const float* pcn, const float* pe, const float* wag, const int32_t* center, const int32_t* nbr,
                        const int32_t* d2u, const int32_t* ptr_c, int n_edges, int n_atoms, const float* w2t, const float* b2,
                        const float* ln, float* agg, float* save_p, float* parts, cudaStream_t stream);

@@ -1,20 +1,20 @@
-// AtomConv / BondConv message kernels on tcgen05 (sm_100a): forward and reverse.
+// AtomConv / BondConv message kernels on the Hopper tensor cores (wgmma, sm_90a): forward and reverse.
 //
 // Same entry points, arguments and arithmetic as the FFMA kernels in gated.cu; the two
 // 64x64 second-layer products of the GatedMLP (and their transposes in the reverse) run on
-// the tensor cores as 3xTF32 (tc.cuh) with accumulators in tensor memory:
+// the tensor cores as 3xTF32 (tc.cuh) with accumulators in registers:
 //
 //   (a) cooperative phase, 16 lanes x float4 per 64-wide half-row (coalesced): gather + add
 //       the pre-activation rows, SiLU, write the 128-row tile to shared memory
-//   (b) thread t of the warpgroup reads ITS row, splits hi/lo, tcgen05.st -> A operand in
-//       TMEM (lane t); one elected thread issues 2 x 8 x 3 tcgen05.mma.kind::tf32 against the
+//   (b) each warp reads the A fragments of its rows from the tile, splits hi/lo, and the
+//       warpgroup issues 8 x 3 wgmma.mma_async m64n64k8 per (64-row block, half) against the
 //       weight images resident in shared memory (core half, then gate half)
-//   (c) tcgen05.ld of the accumulator row -> shared memory
+//   (c) the accumulator fragments overwrite the rows they were computed from
 //   (d) cooperative epilogue in the same 16-lane layout as the FFMA kernel: bias, LayerNorm
 //       (shfl reductions), SiLU x sigmoid, bond-weight smoothing, coalesced stores
 //
 // One persistent CTA per SM = two warpgroups on alternating 128-row tiles (one group's
-// gathers / epilogue overlap the other's MMAs).  TMEM: 2 x (64 hi + 64 lo + 128 D) columns.
+// gathers / epilogue overlap the other's MMAs).
 // Shared memory: 4 weight images (64 KB) + 2 x [128][132] fp32 tiles (132 KB).
 #include "gated_common.cuh"
 #include "tc.cuh"
@@ -50,85 +50,24 @@ __device__ __forceinline__ void build_image(uint8_t* hi, uint8_t* lo, const floa
   }
 }
 
-struct WgCtx {
-  int wg, t, warp, bar_id;
-  uint32_t lane_sel, a_hi, a_lo, d_acc, img_addr;
-  uint64_t* bar;
-  uint32_t phase;
-};
-
-// stage row t [0:64 | 64:128] x (Bc | Bg) -> D[0:64 | 64:128]; returns with both products complete
-__device__ __forceinline__ void tile_blockdiag_mma(const float* stage, WgCtx& c) {
-  const uint32_t idesc = tc::idesc_tf32(128, 64);
+// stage row r [0:64 | 64:128] x (Bc | Bg) -> the same row of the stage [0:64 | 64:128], all 128 threads of the
+// warpgroup; each warp only reads and rewrites its own 16-row slices, so no barrier is needed in between
+__device__ __forceinline__ void tile_blockdiag_mma(float* stage, uint32_t img_addr) {
 #pragma unroll 1
   for (int half = 0; half < 2; ++half) {
+    const uint32_t bhi = img_addr + half * 2 * IMG, blo = bhi + IMG;
+#pragma unroll 1
+    for (int mb = 0; mb < 2; ++mb) {
+      float* rows = stage + mb * 64 * HS + half * 64;
+      float d[32];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t hi[16], lo[16];
+      for (int i = 0; i < 32; ++i) d[i] = 0.f;
+      tc::wg_gemm_k64<64>(d, [&](int r, int k) { return rows[r * HS + k]; }, bhi, blo, 2048);
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 v = lds4(stage + c.t * HS + half * 64 + g * 16 + q * 4);
-        tc::split_tf32(v.x, hi[q * 4 + 0], lo[q * 4 + 0]);
-        tc::split_tf32(v.y, hi[q * 4 + 1], lo[q * 4 + 1]);
-        tc::split_tf32(v.z, hi[q * 4 + 2], lo[q * 4 + 2]);
-        tc::split_tf32(v.w, hi[q * 4 + 3], lo[q * 4 + 3]);
-      }
-      tc::tmem_st16(c.a_hi + c.lane_sel + g * 16, hi);
-      tc::tmem_st16(c.a_lo + c.lane_sel + g * 16, lo);
+      for (int i = 0; i < 32; i += 2)
+        *reinterpret_cast<float2*>(rows + tc::frag_row(i) * HS + tc::frag_col(i)) = make_float2(d[i], d[i + 1]);
     }
-    tc::tmem_st_wait();
-    tc::fence_before_sync();
-    tc::wg_barrier(c.bar_id, 128);
-    if (c.t == 0) {
-      tc::fence_after_sync();
-      const uint32_t bhi = c.img_addr + half * 2 * IMG, blo = bhi + IMG;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint64_t bh = tc::smem_desc_kmajor(bhi + j * 256, 128, 2048);
-        const uint64_t bl = tc::smem_desc_kmajor(blo + j * 256, 128, 2048);
-        tc::mma_tf32_ts(c.d_acc + half * 64, c.a_hi + j * 8, bh, idesc, j > 0 ? 1u : 0u);
-        tc::mma_tf32_ts(c.d_acc + half * 64, c.a_lo + j * 8, bh, idesc, 1u);
-        tc::mma_tf32_ts(c.d_acc + half * 64, c.a_hi + j * 8, bl, idesc, 1u);
-      }
-      tc::mma_commit(c.bar);
-    }
-    tc::mbar_wait(c.bar, c.phase);
-    c.phase ^= 1;
-    tc::fence_after_sync();
   }
-}
-
-// accumulator row t -> stage row t (128 floats)
-__device__ __forceinline__ void acc_to_stage(float* stage, const WgCtx& c) {
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    uint32_t v[16];
-    tc::tmem_ld16(c.d_acc + c.lane_sel + g * 16, v);
-    tc::tmem_ld_wait();
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      sts4(stage + c.t * HS + g * 16 + q * 4,
-           make_float4(__uint_as_float(v[q * 4 + 0]), __uint_as_float(v[q * 4 + 1]), __uint_as_float(v[q * 4 + 2]),
-                       __uint_as_float(v[q * 4 + 3])));
-  }
-  tc::fence_before_sync();
-}
-
-__device__ __forceinline__ WgCtx setup_ctx(uint32_t tmem_base, uint64_t* bars, const uint8_t* s_img) {
-  WgCtx c;
-  const int tid = threadIdx.x;
-  c.wg = tid >> 7;
-  c.t = tid & 127;
-  c.warp = tid >> 5;
-  c.bar_id = 1 + c.wg;
-  c.lane_sel = (uint32_t)((c.warp & 3) * 32) << 16;
-  c.a_hi = tmem_base + c.wg * 256;
-  c.a_lo = c.a_hi + 64;
-  c.d_acc = c.a_hi + 128;
-  c.img_addr = tc::smem_u32(s_img);
-  c.bar = &bars[c.wg];
-  c.phase = 0;
-  return c;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -138,8 +77,6 @@ __global__ void __launch_bounds__(NTHR, 1) gated_fwd_tc_kernel(const FwdArgs a) 
   uint8_t* s_img = smem_raw + SmemLayout::IMG_OFF;
   float* s_b2 = reinterpret_cast<float*>(smem_raw + SmemLayout::B2_OFF);
   float* s_ln = reinterpret_cast<float*>(smem_raw + SmemLayout::LN_OFF);
-  __shared__ __align__(8) uint64_t s_bar[2];
-  __shared__ uint32_t s_tmem;
 
   const int tid = threadIdx.x;
   const bool use_ln = a.ln != nullptr;
@@ -147,33 +84,26 @@ __global__ void __launch_bounds__(NTHR, 1) gated_fwd_tc_kernel(const FwdArgs a) 
   build_image(s_img + 2 * IMG, s_img + 3 * IMG, a.w2t, 128, 64, tid);  // gate
   if (tid < 128) s_b2[tid] = a.b2[tid];
   if (use_ln) s_ln[tid] = a.ln[tid];
-  if (tid == 0) {
-    tc::mbar_init(&s_bar[0], 1);
-    tc::mbar_init(&s_bar[1], 1);
-    tc::mbar_fence_init();
-  }
-  if ((tid >> 5) == 0) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
 
-  WgCtx c = setup_ctx(s_tmem, s_bar, s_img);
-  float* stage = reinterpret_cast<float*>(smem_raw + SmemLayout::STAGE_OFF) + c.wg * STAGE_FLOATS;
-  int* s_idx = reinterpret_cast<int*>(smem_raw + SmemLayout::IDX_OFF) + c.wg * 3 * TMT;
-  const int tx = c.t & 15, ty = c.t >> 4;  // 16 lanes per row, 8 row groups
+  const int wg = tid >> 7, t = tid & 127, bar_id = 1 + wg;
+  const uint32_t img_addr = tc::smem_u32(s_img);
+  float* stage = reinterpret_cast<float*>(smem_raw + SmemLayout::STAGE_OFF) + wg * STAGE_FLOATS;
+  int* s_idx = reinterpret_cast<int*>(smem_raw + SmemLayout::IDX_OFF) + wg * 3 * TMT;
+  const int tx = t & 15, ty = t >> 4;  // 16 lanes per row, 8 row groups
   const int c0 = tx * 4;
 
   const int n_tiles = (a.n_rows + TMT - 1) / TMT;
-  for (int tile = blockIdx.x * 2 + c.wg; tile < n_tiles; tile += gridDim.x * 2) {
+  for (int tile = blockIdx.x * 2 + wg; tile < n_tiles; tile += gridDim.x * 2) {
     const int base = tile * TMT;
     {
-      const int r = min(base + c.t, a.n_rows - 1);
-      s_idx[c.t] = a.idx0[r];
-      s_idx[TMT + c.t] = a.idx1[r];
-      s_idx[2 * TMT + c.t] = a.idx2[r];
+      const int r = min(base + t, a.n_rows - 1);
+      s_idx[t] = a.idx0[r];
+      s_idx[TMT + t] = a.idx1[r];
+      s_idx[2 * TMT + t] = a.idx2[r];
     }
-    tc::wg_barrier(c.bar_id, 128);
+    tc::wg_barrier(bar_id, 128);
 
     // (a) gather + add the pre-activation rows, SiLU -> stage
 #pragma unroll 1
@@ -198,12 +128,11 @@ __global__ void __launch_bounds__(NTHR, 1) gated_fwd_tc_kernel(const FwdArgs a) 
              make_float4(silu_f(acc[i][4]), silu_f(acc[i][5]), silu_f(acc[i][6]), silu_f(acc[i][7])));
       }
     }
-    tc::wg_barrier(c.bar_id, 128);
+    tc::wg_barrier(bar_id, 128);
 
     // (b) second layer on the tensor cores, (c) accumulators back to shared memory
-    tile_blockdiag_mma(stage, c);
-    acc_to_stage(stage, c);
-    tc::wg_barrier(c.bar_id, 128);
+    tile_blockdiag_mma(stage, img_addr);
+    tc::wg_barrier(bar_id, 128);
 
     // (d) epilogue: + b2 -> LayerNorm -> silu * sigmoid -> smoothing -> store
     float4 g1, b1, g2, b2v;
@@ -249,12 +178,8 @@ __global__ void __launch_bounds__(NTHR, 1) gated_fwd_tc_kernel(const FwdArgs a) 
         if (valid) stg4(a.out + (size_t)g * 64 + c0, o);
       }
     }
-    tc::wg_barrier(c.bar_id, 128);  // stage / s_idx are free for the next tile
+    tc::wg_barrier(bar_id, 128);  // stage / s_idx are free for the next tile
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if ((tid >> 5) == 0) tc::tmem_dealloc(s_tmem, 512);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -263,8 +188,6 @@ __global__ void __launch_bounds__(NTHR, 1) gated_bwd_tc_kernel(const BwdArgs a) 
   extern __shared__ __align__(128) uint8_t smem_raw[];
   uint8_t* s_img = smem_raw + SmemLayout::IMG_OFF;
   float* s_ln = reinterpret_cast<float*>(smem_raw + SmemLayout::LN_OFF);
-  __shared__ __align__(8) uint64_t s_bar[2];
-  __shared__ uint32_t s_tmem;
 
   const int tid = threadIdx.x;
   const bool use_ln = a.ln != nullptr;
@@ -272,33 +195,26 @@ __global__ void __launch_bounds__(NTHR, 1) gated_bwd_tc_kernel(const BwdArgs a) 
   build_image(s_img, s_img + IMG, a.w2, 64, 0, tid);
   build_image(s_img + 2 * IMG, s_img + 3 * IMG, a.w2 + 64 * 64, 64, 0, tid);
   if (use_ln) s_ln[tid] = a.ln[tid];
-  if (tid == 0) {
-    tc::mbar_init(&s_bar[0], 1);
-    tc::mbar_init(&s_bar[1], 1);
-    tc::mbar_fence_init();
-  }
-  if ((tid >> 5) == 0) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
 
-  WgCtx c = setup_ctx(s_tmem, s_bar, s_img);
-  float* stage = reinterpret_cast<float*>(smem_raw + SmemLayout::STAGE_OFF) + c.wg * STAGE_FLOATS;
-  int* s_idx = reinterpret_cast<int*>(smem_raw + SmemLayout::IDX_OFF) + c.wg * 3 * TMT;
-  const int tx = c.t & 15, ty = c.t >> 4;
+  const int wg = tid >> 7, t = tid & 127, bar_id = 1 + wg;
+  const uint32_t img_addr = tc::smem_u32(s_img);
+  float* stage = reinterpret_cast<float*>(smem_raw + SmemLayout::STAGE_OFF) + wg * STAGE_FLOATS;
+  int* s_idx = reinterpret_cast<int*>(smem_raw + SmemLayout::IDX_OFF) + wg * 3 * TMT;
+  const int tx = t & 15, ty = t >> 4;
   const int c0 = tx * 4;
 
   const int n_tiles = (a.n_rows + TMT - 1) / TMT;
-  for (int tile = blockIdx.x * 2 + c.wg; tile < n_tiles; tile += gridDim.x * 2) {
+  for (int tile = blockIdx.x * 2 + wg; tile < n_tiles; tile += gridDim.x * 2) {
     const int base = tile * TMT;
     {
-      const int r = min(base + c.t, a.n_rows - 1);
-      s_idx[c.t] = a.idx0[r];
-      s_idx[TMT + c.t] = a.idx1[r];
-      if (MODE == ATOM) s_idx[2 * TMT + c.t] = a.idx2[r];
+      const int r = min(base + t, a.n_rows - 1);
+      s_idx[t] = a.idx0[r];
+      s_idx[TMT + t] = a.idx1[r];
+      if (MODE == ATOM) s_idx[2 * TMT + t] = a.idx2[r];
     }
-    tc::wg_barrier(c.bar_id, 128);
+    tc::wg_barrier(bar_id, 128);
 
     // (a) recompute the gate from saved p, bond-weight gradients, LayerNorm reverse -> g_p -> stage
     float4 g1, g2, b1, b2v;
@@ -391,12 +307,11 @@ __global__ void __launch_bounds__(NTHR, 1) gated_bwd_tc_kernel(const BwdArgs a) 
         sts4(stage + row * HS + 64 + c0, make_float4(gy2[0], gy2[1], gy2[2], gy2[3]));
       }
     }
-    tc::wg_barrier(c.bar_id, 128);
+    tc::wg_barrier(bar_id, 128);
 
     // (b) g_h = g_p . W2 on the tensor cores, (c) back to shared memory
-    tile_blockdiag_mma(stage, c);
-    acc_to_stage(stage, c);
-    tc::wg_barrier(c.bar_id, 128);
+    tile_blockdiag_mma(stage, img_addr);
+    tc::wg_barrier(bar_id, 128);
 
     // (d) g_pre = g_h * silu'(pre)
 #pragma unroll 1
@@ -434,12 +349,8 @@ __global__ void __launch_bounds__(NTHR, 1) gated_bwd_tc_kernel(const BwdArgs a) 
         }
       }
     }
-    tc::wg_barrier(c.bar_id, 128);
+    tc::wg_barrier(bar_id, 128);
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if ((tid >> 5) == 0) tc::tmem_dealloc(s_tmem, 512);
 }
 
 template <typename KernelT, typename ArgsT>

@@ -1,33 +1,30 @@
-// AtomConv / BondConv message + aggregation as ONE warp-specialised tcgen05 kernel (sm_100a).
+// AtomConv / BondConv message + aggregation as ONE warp-specialised wgmma kernel (sm_90a).
 //
 //   agg[s] = sum_{rows r of segment s} GatedMLP(pre_r) * w_r          (reference layers.py:113-126, 238-254)
 //
 // with pre_r = the gather-add of 3 (AtomConv) / 4 (BondConv) first-layer rows (DESIGN.md §3.1), the two
-// 64x64 second-layer products on the tensor cores (3xTF32, accumulators in tensor memory), LayerNorm +
+// 64x64 second-layer products on the tensor cores (3xTF32, accumulators in registers), LayerNorm +
 // SiLU x sigmoid in the epilogue, and the segmented reduction over the centre-sorted (bond-i-sorted) rows done
 // inside the CTA: the [rows, 64] message never goes to HBM.
 //
-// One persistent CTA per SM, 17 warps (544 threads, <= 96 registers each), three roles connected by mbarriers:
+// One persistent CTA per SM, 16 warps (512 threads), two roles connected by mbarriers:
 //
 //   warps 8-11  producer of the CORE half, warps 12-15 producer of the GATE half of every 128-row tile (two
-//               independent groups, so one gathers while the other converts): 16 lanes x float4 per 64-float
-//               half-row (coalesced) gather + add the first-layer rows, SiLU, store the [128 x 64] half-tile to
-//               shared memory (16-byte chunks XOR-swizzled by row), group barrier, then thread t reads ITS row
-//               (conflict-free), splits hi / lo and tcgen05.st's it into the group's A stage of tensor memory;
-//               BondConv also writes save_pre
-//   warp 16     MMA: one lane issues 8 k-steps x 3 split terms of tcgen05.mma.kind::tf32 (M=128, N=64) per
-//               half into one of two D stages, tcgen05.commit -> mbarriers
-//   warps 0-3   epilogue of the CORE half, warps 4-7 of the GATE half: thread t owns (half of) row t: two
-//               tcgen05.ld sweeps (shifted one-pass mean / variance, then normalise: LayerNorm is in-thread, no
-//               shuffles), SiLU (core) / sigmoid (gate) -> two [128 x 64] tiles in shared memory; then each of the
-//               8 warps reduces a 16-row strip (core x gate x bond weights, the weights read coalesced) over runs
-//               of equal segment id: complete segments are stored, strip-boundary partials go to `parts`
+//               independent groups): 16 lanes x float4 per 64-float half-row (coalesced) gather + add the
+//               first-layer rows, SiLU, store the [128 x 64] half-tile to shared memory (16-byte chunks
+//               XOR-swizzled by row); BondConv also writes save_pre
+//   warps 0-7   two consumer warpgroups, tile rows 0-63 / 64-127: each warp reads its A fragments from both
+//               half-tiles (conflict-free), the warpgroup issues 8 k-steps x 3 split terms of wgmma m64n64k8
+//               per half; the epilogue runs on the accumulator fragments (a row's 64 values sit in one lane
+//               quad: LayerNorm by quad shuffles), SiLU (core) x sigmoid (gate) -> one [128 x 64] tile in
+//               shared memory; then each of the 8 warps reduces a 16-row strip (x bond weights, read
+//               coalesced) over runs of equal segment id: complete segments are stored, strip-boundary
+//               partials go to `parts`
 //
 // A tiny second kernel (seg_stitch) adds the strip partials of every segment that spans strips, in strip
 // order (deterministic, no atomics), and zeroes empty segments.
 //
-// TMEM: 2 x (64 hi + 64 lo) A + 2 x 128 D = 512 columns.  Shared memory: 4 weight images (64 KB) + 2 half-tiles
-// (64 KB) + the core / gate output tiles (64 KB) + indices.
+// Shared memory: 4 weight images (64 KB) + 2 half-tiles (64 KB) + the output tile (32 KB) + indices.
 #include "gated_common.cuh"
 #include "tc.cuh"
 
@@ -35,27 +32,17 @@ namespace chg {
 namespace gated {
 namespace {
 
-constexpr int WS_THREADS = 544;  // 17 warps: 8 epilogue, 8 producer, 1 MMA
+constexpr int WS_THREADS = 512;  // 8 consumer warps (two warpgroups), 8 producer warps
 constexpr int TR = 128;          // rows per tile
 constexpr int HALF_BYTES = TR * 64 * 4;
 constexpr int IMG_BYTES = 64 * 64 * 4;
 constexpr int STRIP = 16;        // rows per reduction strip (one half-warp)
-#ifndef CHG_WS_REGSPLIT
-// 1: setmaxnreg in the forward kernel - 20 warps launched with 96 registers, then 144 for the producer warps (24 instead of 12
-// independent 16-byte gathers in flight per thread), 72 for the epilogue warps, 40 for the MMA warp's warpgroup (3 of its 4 warps
-// exist only to donate registers; the pool of a CTA is what it was launched with).  Measured on B200 (c3): AtomConv 1.53 -> 1.47 ms,
-// BondConv 1.55 -> 1.51 ms per step, i.e. the gathers' memory-level parallelism is NOT what bounds the kernel: left off.
-#define CHG_WS_REGSPLIT 0
-#endif
-constexpr int PB = CHG_WS_REGSPLIT ? 8 : 4;  // rows gathered per producer batch (x 3-4 loads each in flight)
-// register pool of the CTA = what it was launched with: 20 warps x 96; after the reallocation 8 x 72 + 8 x 144 + 4 x 40 = 1888 <= 1920
-constexpr int WS_FWD_THREADS = CHG_WS_REGSPLIT ? 640 : WS_THREADS;
 
 struct WsSmem {
   static constexpr int IMG_OFF = 0;                          // Bc_hi, Bc_lo, Bg_hi, Bg_lo
   static constexpr int HS_OFF = 4 * IMG_BYTES;               // 2 x [128][64] fp32, swizzled (core | gate producer)
-  static constexpr int O_OFF = HS_OFF + 2 * HALF_BYTES;      // 2 x [128][64] fp32, swizzled: silu(core), sigmoid(gate)
-  static constexpr int GIDX_OFF = O_OFF + 2 * HALF_BYTES;    // 2 groups x 3 x 128 int
+  static constexpr int O_OFF = HS_OFF + 2 * HALF_BYTES;      // [128][64] fp32, swizzled: silu(core) * sigmoid(gate)
+  static constexpr int GIDX_OFF = O_OFF + HALF_BYTES;        // 2 groups x 3 x 128 int
   static constexpr int EIDX_OFF = GIDX_OFF + 2 * 3 * TR * 4;  // 4 x 128 int: segment id, weight row, segment begin / end
   static constexpr int B2_OFF = EIDX_OFF + 4 * TR * 4;       // 128 floats
   static constexpr int LN_OFF = B2_OFF + 128 * 4;            // 256 floats
@@ -64,7 +51,6 @@ struct WsSmem {
 
 struct WsBars {
   uint64_t a_full[2], a_empty[2];
-  uint64_t d_full[2], d_empty[2];
 };
 
 struct FusedArgs {
@@ -86,9 +72,6 @@ struct FusedArgs {
   float* save_p;        // [rows][128] or null
 };
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
 // pull one 128-byte line towards L2 (no register, no dependency): issued one tile ahead of the gathers that read it
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // byte offset of 16-byte chunk c (0..15) of row r in a swizzled [128][64] fp32 tile
@@ -107,67 +90,46 @@ __device__ __forceinline__ void build_image_ws(uint8_t* hi, uint8_t* lo, const f
   }
 }
 
-// ---- epilogue helper: one 64-wide half of row t out of tensor memory ----------------------------------------
-// p = acc + b2; y = LN(p) (or p); CORE: out = silu(y);  GATE: out = sigmoid(y); out -> row t of the swizzled tile.
-// LayerNorm statistics in one sweep, shifted by the row's first element (no cancellation for |mean| >> std).
-template <bool GATE>
-__device__ __forceinline__ void epilogue_half(uint32_t d_addr, const float* s_b2, const float* s_gamma, const float* s_beta,
-                                              bool use_ln, uint8_t* s_tile, int t, float* save_row) {
-  float mean = 0.f, rstd = 1.f;
-  if (use_ln) {
-    float s1 = 0.f, s2 = 0.f, s1b = 0.f, s2b = 0.f, x0 = 0.f;
+// ---- epilogue helpers on m64n64 accumulator fragments -----------------------------------------------------
+// sum over the lane quad that holds one accumulator row
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+// in place: d (+ b2) -> saved p (optional) -> LayerNorm (optional, per row over the quad; two-pass statistics)
+__device__ __forceinline__ void bias_ln_frag(float (&d)[32], const float* s_b2, const float* s_gamma, const float* s_beta,
+                                             bool use_ln, float* save_rows, int row0, int n_rows) {
 #pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      uint32_t v[32];
-      tc::tmem_ld32(d_addr + g * 32, v);
-      tc::tmem_ld_wait();
-      if (g == 0) x0 = __uint_as_float(v[0]) + s_b2[0];
+  for (int i = 0; i < 32; ++i) d[i] += s_b2[tc::frag_col(i)];
+  if (save_rows != nullptr) {
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 b = lds4(s_b2 + g * 32 + q * 4);  // broadcast
-        const float d0 = __uint_as_float(v[q * 4]) + b.x - x0, d1 = __uint_as_float(v[q * 4 + 1]) + b.y - x0;
-        const float d2 = __uint_as_float(v[q * 4 + 2]) + b.z - x0, d3 = __uint_as_float(v[q * 4 + 3]) + b.w - x0;
-        s1 += d0 + d1;
-        s1b += d2 + d3;
-        s2 = fmaf(d0, d0, fmaf(d1, d1, s2));
-        s2b = fmaf(d2, d2, fmaf(d3, d3, s2b));
-      }
+    for (int i = 0; i < 32; i += 2) {
+      const int g = row0 + tc::frag_row(i);
+      if (g < n_rows) *reinterpret_cast<float2*>(save_rows + (size_t)g * 128 + tc::frag_col(i)) = make_float2(d[i], d[i + 1]);
     }
-    const float m1 = (s1 + s1b) * (1.f / 64.f);
-    mean = x0 + m1;
-    rstd = 1.f / sqrtf(fmaxf((s2 + s2b) * (1.f / 64.f) - m1 * m1, 0.f) + LN_EPS);
   }
+  if (!use_ln) return;
 #pragma unroll
-  for (int g = 0; g < 2; ++g) {
-    uint32_t v[32];
-    tc::tmem_ld32(d_addr + g * 32, v);
-    tc::tmem_ld_wait();
+  for (int h = 0; h < 2; ++h) {  // h = 0: row frag_row(0), h = 1: row frag_row(0) + 8
+    float s1 = 0.f;
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 b = lds4(s_b2 + g * 32 + q * 4);
-      float4 p = make_float4(__uint_as_float(v[q * 4]) + b.x, __uint_as_float(v[q * 4 + 1]) + b.y,
-                             __uint_as_float(v[q * 4 + 2]) + b.z, __uint_as_float(v[q * 4 + 3]) + b.w);
-      if (save_row != nullptr) stg4(save_row + g * 32 + q * 4, p);
-      if (use_ln) {
-        const float4 ga = lds4(s_gamma + g * 32 + q * 4), be = lds4(s_beta + g * 32 + q * 4);
-        p.x = fmaf((p.x - mean) * rstd, ga.x, be.x);
-        p.y = fmaf((p.y - mean) * rstd, ga.y, be.y);
-        p.z = fmaf((p.z - mean) * rstd, ga.z, be.z);
-        p.w = fmaf((p.w - mean) * rstd, ga.w, be.w);
-      }
-      float4 o;
-      if (GATE) {
-        o = make_float4(sigmoid_f(p.x), sigmoid_f(p.y), sigmoid_f(p.z), sigmoid_f(p.w));
-      } else {
-        o = make_float4(silu_f(p.x), silu_f(p.y), silu_f(p.z), silu_f(p.w));
-      }
-      *reinterpret_cast<float4*>(s_tile + swz(t, g * 8 + q)) = o;
-    }
+    for (int i = 0; i < 32; ++i)
+      if (((i >> 1) & 1) == h) s1 += d[i];
+    const float mean = quad_sum(s1) * (1.f / 64.f);
+    float s2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      if (((i >> 1) & 1) == h) s2 = fmaf(d[i] - mean, d[i] - mean, s2);
+    const float rstd = 1.f / sqrtf(quad_sum(s2) * (1.f / 64.f) + LN_EPS);
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      if (((i >> 1) & 1) == h) d[i] = fmaf((d[i] - mean) * rstd, s_gamma[tc::frag_col(i)], s_beta[tc::frag_col(i)]);
   }
 }
 
 template <int MODE>
-__global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const FusedArgs a) {
+__global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_fwd_kernel(const FusedArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* s_img = smem_raw + WsSmem::IMG_OFF;
   uint8_t* s_hs = smem_raw + WsSmem::HS_OFF;
@@ -177,13 +139,12 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
   float* s_b2 = reinterpret_cast<float*>(smem_raw + WsSmem::B2_OFF);
   float* s_ln = reinterpret_cast<float*>(smem_raw + WsSmem::LN_OFF);
   __shared__ __align__(8) WsBars bars;
-  __shared__ uint32_t s_tmem;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const bool use_ln = a.ln != nullptr;
   const int n_tiles = (a.n_rows + TR - 1) / TR;
 
-  // ---- one-time setup: weight images, bias / LayerNorm rows, barriers, tensor memory ------------------------
+  // ---- one-time setup: weight images, bias / LayerNorm rows, barriers ------------------------------------------
   build_image_ws(s_img, s_img + IMG_BYTES, a.w2t, 128, 0, tid);                     // core: (n=c, kk=k) = w2t[k][c]
   build_image_ws(s_img + 2 * IMG_BYTES, s_img + 3 * IMG_BYTES, a.w2t, 128, 64, tid);  // gate
   if (tid < 128) s_b2[tid] = a.b2[tid];
@@ -191,36 +152,22 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
       tc::mbar_init(&bars.a_full[i], 128);
-      tc::mbar_init(&bars.a_empty[i], 1);
-      tc::mbar_init(&bars.d_full[i], 1);
-      tc::mbar_init(&bars.d_empty[i], 256);
+      tc::mbar_init(&bars.a_empty[i], 256);
     }
     tc::mbar_fence_init();
   }
-  if (warp == 16) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = s_tmem;
-  // TMEM columns: A stage h (h = 0 core, 1 gate) at h*128 (hi) / h*128 + 64 (lo); D stage s at 256 + s*128
-  // (core 0..63 | gate 64..127)
 
-  if (warp >= 8 && warp < 16) {
-    // ============================ producer groups (gather -> SiLU -> A operand) ============================
-#if CHG_WS_REGSPLIT
-    // the gathers are what the kernel waits for: take registers from the epilogue warps (which give up 24 each) so that a
-    // producer thread keeps 24 instead of 12 independent 16-byte loads in flight
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 144;");
-#endif
+  if (warp >= 8) {
+    // ============================ producer groups (gather -> SiLU -> half-tile) ============================
     const int half = (warp - 8) >> 2;            // 0: core columns, 1: gate columns
-    const int gt = tid - 256 - half * 128;       // 0..127 inside the group; also this thread's tile row / TMEM lane
+    const int gt = tid - 256 - half * 128;       // 0..127 inside the group
     const int tx = gt & 15, ty = gt >> 4;        // 16 lanes per row, 8 rows per pass
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
     int* gi = s_gidx + half * 3 * TR;
     uint8_t* stage = s_hs + half * HALF_BYTES;
     const int col = half * 64 + tx * 4;
-    const uint32_t a_hi = tmem_base + half * 128 + lane_sel, a_lo = a_hi + 64;
+    constexpr int PB = 4;  // rows gathered per batch (x 3-4 loads each in flight)
     int tl = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
       const int base = tile * TR;
@@ -230,7 +177,7 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
         gi[TR + gt] = a.idx1[r];
         gi[2 * TR + gt] = a.idx2[r];
       }
-      tc::wg_barrier(1 + half, 128);  // indices visible; every thread of the group is done with the previous half-tile
+      tc::wg_barrier(1 + half, 128);  // indices visible
       {
         // the rows of the NEXT tile that stream from HBM (p_b: per-bond products for AtomConv; p_c: per-angle products for
         // BondConv): prefetch this group's half (2 lines of 128 B per row) towards L2 while this tile is gathered
@@ -254,6 +201,7 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
           v[i] = ldg4(s0) + ldg4(s1) + ldg4(s2);
           if (MODE == BOND) v[i] = v[i] + ldg4(a.p_c + (size_t)min(base + row, a.n_rows - 1) * 128 + col);
         }
+        if (b == 0) tc::mbar_wait(&bars.a_empty[half], (tl & 1) ^ 1);  // the consumers have read the previous half-tile
 #pragma unroll
         for (int i = 0; i < PB; ++i) {
           const int row = ty + 8 * (b * PB + i);
@@ -262,80 +210,25 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
               make_float4(silu_f(v[i].x), silu_f(v[i].y), silu_f(v[i].z), silu_f(v[i].w));
         }
       }
-      tc::wg_barrier(1 + half, 128);  // the half-tile is complete in shared memory
-      tc::mbar_wait(&bars.a_empty[half], (tl & 1) ^ 1);  // the MMAs of the previous tile have read this A stage
-      tc::fence_after_sync();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 v = *reinterpret_cast<const float4*>(stage + swz(gt, g * 4 + q));
-          tc::split_tf32(v.x, hi[q * 4 + 0], lo[q * 4 + 0]);
-          tc::split_tf32(v.y, hi[q * 4 + 1], lo[q * 4 + 1]);
-          tc::split_tf32(v.z, hi[q * 4 + 2], lo[q * 4 + 2]);
-          tc::split_tf32(v.w, hi[q * 4 + 3], lo[q * 4 + 3]);
-        }
-        tc::tmem_st16(a_hi + g * 16, hi);
-        tc::tmem_st16(a_lo + g * 16, lo);
-      }
-      tc::tmem_st_wait();
-      tc::fence_before_sync();
-      mbar_arrive(&bars.a_full[half]);
+      tc::wg_barrier(1 + half, 128);  // every thread of the group is done with the indices of this tile
+      tc::mbar_arrive(&bars.a_full[half]);
     }
-  } else if (warp >= 16) {
-    // ============================ MMA issuer (warp 16; warps 17-19 only donate registers) ============================
-#if CHG_WS_REGSPLIT
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-#endif
-    if (warp == 16 && lane == 0) {
-      const uint32_t idesc = tc::idesc_tf32(128, 64);
-      const uint32_t img = tc::smem_u32(s_img);
-      int tl = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
-        const int ds = tl & 1;
-#pragma unroll 1
-        for (int half = 0; half < 2; ++half) {
-          tc::mbar_wait(&bars.a_full[half], tl & 1);
-          if (half == 0) tc::mbar_wait(&bars.d_empty[ds], ((tl >> 1) & 1) ^ 1);
-          tc::fence_after_sync();
-          const uint32_t d_acc = tmem_base + 256 + ds * 128 + half * 64;
-          const uint32_t a_hi = tmem_base + half * 128, a_lo = a_hi + 64;
-          const uint32_t bhi = img + half * 2 * IMG_BYTES, blo = bhi + IMG_BYTES;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint64_t bh = tc::smem_desc_kmajor(bhi + j * 256, 128, 2048);
-            const uint64_t bl = tc::smem_desc_kmajor(blo + j * 256, 128, 2048);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bh, idesc, j > 0 ? 1u : 0u);
-            tc::mma_tf32_ts(d_acc, a_lo + j * 8, bh, idesc, 1u);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bl, idesc, 1u);
-          }
-          tc::mma_commit(&bars.a_empty[half]);  // A stage reusable once these MMAs have read it
-          if (half == 1) tc::mma_commit(&bars.d_full[ds]);
-        }
-      }
-    }
-  } else if (warp < 8) {
-    // ============================ epilogue: warps 0-3 core half, warps 4-7 gate half ============================
-#if CHG_WS_REGSPLIT
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-#endif
-    const int eh = warp >> 2;        // 0: core, 1: gate
-    const int t = tid & 127;         // tile row == TMEM lane
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
+  } else {
+    // ============================ consumers: warps 0-3 rows 0-63, warps 4-7 rows 64-127 ============================
+    const int cw = warp >> 2;
+    const int t = tid & 127;         // index-row duty: warps 0-3 segment rows, warps 4-7 weight rows
+    const int row0 = cw * 64;
     int* s_seg = s_eidx;             // segment id of every tile row
     int* s_wrow = s_eidx + TR;       // row of the bond weight (ATOM: d2u; BOND: slot j - slot i is the segment id)
     int* s_sa = s_eidx + 2 * TR;     // ptr[seg], ptr[seg + 1] of every tile row
     int* s_sb = s_eidx + 3 * TR;
-    uint8_t* s_o1 = s_o;
-    uint8_t* s_o2 = s_o + HALF_BYTES;
+    const uint32_t img = tc::smem_u32(s_img);
     int tl = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
       const int base = tile * TR;
-      const int ds = tl & 1;
       {
         const int r = min(base + t, a.n_rows - 1);
-        if (eh == 0) {
+        if (cw == 0) {
           const int seg = a.idx0[r];
           s_seg[t] = seg;
           s_sa[t] = __ldg(a.ptr + seg);
@@ -343,21 +236,31 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
         } else {
           const int wr = MODE == BOND ? a.idx1[r] : a.idx2[r];
           s_wrow[t] = wr;
-          prefetch_l2(a.wgt + (size_t)wr * 64);  // the bond-weight row the strip reduction reads after the sweeps
+          prefetch_l2(a.wgt + (size_t)wr * 64);  // the bond-weight row the strip reduction reads after the products
           prefetch_l2(a.wgt + (size_t)wr * 64 + 32);
         }
       }
-      tc::mbar_wait(&bars.d_full[ds], (tl >> 1) & 1);
-      tc::fence_after_sync();
-      const uint32_t d_acc = tmem_base + 256 + ds * 128 + eh * 64 + lane_sel;
-      float* save_row = (a.save_p != nullptr && base + t < a.n_rows) ? a.save_p + (size_t)(base + t) * 128 + eh * 64 : nullptr;
-      if (eh == 0) {
-        epilogue_half<false>(d_acc, s_b2, s_ln, s_ln + 64, use_ln, s_o1, t, save_row);
-      } else {
-        epilogue_half<true>(d_acc, s_b2 + 64, s_ln + 128, s_ln + 192, use_ln, s_o2, t, save_row);
+      float dc[32], dg[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dc[i] = dg[i] = 0.f;
+      tc::mbar_wait(&bars.a_full[0], tl & 1);
+      tc::wg_gemm_k64<64>(dc, [&](int r, int k) { return *reinterpret_cast<const float*>(s_hs + swz(row0 + r, k >> 2) + (k & 3) * 4); },
+                          img, img + IMG_BYTES, 2048);
+      tc::mbar_arrive(&bars.a_empty[0]);
+      tc::mbar_wait(&bars.a_full[1], tl & 1);
+      tc::wg_gemm_k64<64>(dg, [&](int r, int k) { return *reinterpret_cast<const float*>(s_hs + HALF_BYTES + swz(row0 + r, k >> 2) + (k & 3) * 4); },
+                          img + 2 * IMG_BYTES, img + 3 * IMG_BYTES, 2048);
+      tc::mbar_arrive(&bars.a_empty[1]);
+      // epilogue: p = acc + b2 (saved), LayerNorm, silu(core) * sigmoid(gate) -> output tile
+      float* save = a.save_p != nullptr ? a.save_p + (size_t)base * 128 : nullptr;
+      bias_ln_frag(dc, s_b2, s_ln, s_ln + 64, use_ln, save, row0, a.n_rows - base);
+      bias_ln_frag(dg, s_b2 + 64, s_ln + 128, s_ln + 192, use_ln, save != nullptr ? save + 64 : nullptr, row0, a.n_rows - base);
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int r = row0 + tc::frag_row(i), c = tc::frag_col(i);
+        *reinterpret_cast<float2*>(s_o + swz(r, c >> 2) + (c & 3) * 4) =
+            make_float2(silu_f(dc[i]) * sigmoid_f(dg[i]), silu_f(dc[i + 1]) * sigmoid_f(dg[i + 1]));
       }
-      tc::fence_before_sync();
-      mbar_arrive(&bars.d_empty[ds]);  // the accumulator stage can be overwritten
       tc::wg_barrier(3, 256);
 
       // ---- segmented reduction: warp w owns the 16-row strip w, lane l the columns 2l, 2l+1 ----------------
@@ -378,8 +281,8 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
         }
         float2 acc = make_float2(0.f, 0.f);
         int cur_row = warp * STRIP;  // first row of the current run
-        auto emit = [&](int row0, const float2& v) {
-          const int seg = s_seg[row0], sa = s_sa[row0], sb = s_sb[row0];
+        auto emit = [&](int row0_, const float2& v) {
+          const int seg = s_seg[row0_], sa = s_sa[row0_], sb = s_sb[row0_];
           float* dst;
           if (sa >= strip_lo && sb <= strip_hi) {
             dst = a.out + (size_t)seg * 64;  // the whole segment lies in this strip
@@ -397,22 +300,16 @@ __global__ void __launch_bounds__(WS_FWD_THREADS, 1) gated_ws_fwd_kernel(const F
               cur_row = rr;
               acc = make_float2(0.f, 0.f);
             }
-            const int off = swz(rr, lane >> 1) + (lane & 1) * 8;
-            const float2 c = *reinterpret_cast<const float2*>(s_o1 + off);
-            const float2 g = *reinterpret_cast<const float2*>(s_o2 + off);
-            acc.x = fmaf(c.x * g.x, w[i].x, acc.x);
-            acc.y = fmaf(c.y * g.y, w[i].y, acc.y);
+            const float2 o = *reinterpret_cast<const float2*>(s_o + swz(rr, lane >> 1) + (lane & 1) * 8);
+            acc.x = fmaf(o.x, w[i].x, acc.x);
+            acc.y = fmaf(o.y, w[i].y, acc.y);
           }
         }
         emit(cur_row, acc);
       }
-      tc::wg_barrier(3, 256);  // the output tiles and the index rows are free for the next tile
+      tc::wg_barrier(3, 256);  // the output tile and the index rows are free for the next tile
     }
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 16) tc::tmem_dealloc(tmem_base, 512);
 }
 
 // out[s] for every segment that spans more than one strip (sum of its strip partials, in strip order) and for
@@ -444,7 +341,7 @@ int launch_fused(const FusedArgs& a, cudaStream_t stream) {
       attr_set = true;
     }
     const int n_tiles = (a.n_rows + TR - 1) / TR;
-    gated_ws_fwd_kernel<MODE><<<min(n_tiles, sm_count()), WS_FWD_THREADS, WsSmem::TOTAL, stream>>>(a);
+    gated_ws_fwd_kernel<MODE><<<min(n_tiles, sm_count()), WS_THREADS, WsSmem::TOTAL, stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
       set_error("gated_ws_fwd_kernel: launch failed: %s", cudaGetErrorString(e));
@@ -493,7 +390,7 @@ extern "C" int chg_atom_conv_fused(const float* pcn, const float* pe, const floa
   if (n_atoms == 0) return CHG_OK;
   CHG_CHECK_ARG(ptr_c && agg, "null pointer");
   CHG_CHECK_ARG(n_edges == 0 || (pcn && pe && wag && center && nbr && d2u && w2t && b2 && work), "null pointer");
-  // tiny inputs (a few tiles) are launch-bound: the persistent tcgen05 kernel's fixed cost (weight images, TMEM) loses there
+  // tiny inputs (a few tiles) are launch-bound: the persistent tensor-core kernel's fixed cost (weight images) loses there
   if (gated_impl() == 3 && n_edges >= ws_min_rows())
     return gated::atom_conv_fused_ws(pcn, pe, wag, center, nbr, d2u, ptr_c, n_edges, n_atoms, w2t, b2, ln, agg, save_p, work,
                                      as_stream(stream));
@@ -522,17 +419,15 @@ extern "C" int chg_bond_conv_fused(const float* pij, const float* px, const floa
 
 // =====================================================================================================================
 // Reverse of the AtomConv / BondConv message (same entry points and arithmetic as gated_bwd_kernel<MODE, false> in
-// gated.cu; reference: autograd of layers.py:113-121, 238-249): warp-specialised tcgen05 version.
+// gated.cu; reference: autograd of layers.py:113-121, 238-249): warp-specialised wgmma version.
 //
 //   warps 0-7   P  16 lanes x float4 per 64-wide half-row: saved p -> LayerNorm statistics (shuffles) -> gates,
 //                  bond-weight gradients (stored), LayerNorm reverse -> g_p tile in shared memory (two swizzled
-//                  halves); group barrier; then thread t converts ITS half-row (t < 128: core, else gate) hi / lo into
-//                  the A operand in tensor memory
-//   warp 16     M  one lane: g_h = g_p . W2 per half (8 k-steps x 3 split terms of tcgen05.mma.kind::tf32 each)
-//   warps 8-15  F  thread t reads its half-row of the accumulator (tcgen05.ld) into a shared-memory tile; group
-//                  barrier; then 16 lanes x float4 per half-row: g_pre = g_h * silu'(pre), pre recomputed from the
-//                  first-layer rows (AtomConv) or read from save_pre (BondConv), coalesced stores
-// TMEM: A (64 hi + 64 lo) x 2 halves = 256 columns, D 2 stages x 128 = 256 columns.
+//                  halves)
+//   warps 8-15  F  two warpgroups, tile rows 0-63 / 64-127: g_h = g_p . W2 per half (A fragments read from the g_p
+//                  tile, 8 k-steps x 3 split terms of wgmma m64n64k8), accumulator fragments -> g_h tile in shared
+//                  memory; group barrier; then 16 lanes x float4 per half-row: g_pre = g_h * silu'(pre), pre
+//                  recomputed from the first-layer rows (AtomConv) or read from save_pre (BondConv), coalesced stores
 // =====================================================================================================================
 namespace chg {
 namespace gated {
@@ -550,7 +445,6 @@ struct WsBwdSmem {
 
 struct WsBwdBars {
   uint64_t a_full, a_empty;
-  uint64_t d_full[2], d_empty[2];
 };
 
 template <int MODE>
@@ -563,9 +457,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
   int* s_fidx = reinterpret_cast<int*>(smem_raw + WsBwdSmem::FIDX_OFF);
   float* s_ln = reinterpret_cast<float*>(smem_raw + WsBwdSmem::LN_OFF);
   __shared__ __align__(8) WsBwdBars bars;
-  __shared__ uint32_t s_tmem;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const bool use_ln = a.ln != nullptr;
   const int n_tiles = (a.n_rows + TR - 1) / TR;
 
@@ -575,28 +468,17 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
   if (tid < 256) s_ln[tid] = use_ln ? a.ln[tid] : 0.f;
   if (tid == 0) {
     tc::mbar_init(&bars.a_full, 256);
-    tc::mbar_init(&bars.a_empty, 1);
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&bars.d_full[i], 1);
-      tc::mbar_init(&bars.d_empty[i], 256);
-    }
+    tc::mbar_init(&bars.a_empty, 256);
     tc::mbar_fence_init();
   }
-  if (warp == 16) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = s_tmem;
-  // TMEM columns: A half h at h*128 (hi) / h*128 + 64 (lo); D stage s at 256 + s*128 (core 0..63 | gate 64..127)
 
   if (warp < 8) {
     // ============================ P: saved p -> g_p -> A operand ============================
     const int t = tid;                   // 0..255
     const int tx = t & 15, ty = t >> 4;  // 16 lanes per row, 16 rows per pass
     const int c0 = tx * 4;
-    const int crow = t & 127, chalf = t >> 7;  // conversion: this thread's tile row and half
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
     int tl = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
       const int base = tile * TR;
@@ -606,7 +488,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         s_pidx[TR + t] = a.idx1[r];
         if (MODE == ATOM) s_pidx[2 * TR + t] = a.idx2[r];
       }
-      tc::wg_barrier(1, 256);  // indices visible; every thread has converted the previous tile
+      tc::wg_barrier(1, 256);  // indices visible
       {
         const int nt = tile + gridDim.x;  // next tile of this CTA: its saved p rows stream from HBM (4 lines of 128 B per row)
         if (nt < n_tiles) {
@@ -623,6 +505,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         g2 = lds4(s_ln + 128 + c0);
         b2v = lds4(s_ln + 192 + c0);
       }
+      tc::mbar_wait(&bars.a_empty, (tl & 1) ^ 1);  // the MMAs of the previous tile have read the g_p tile
 #pragma unroll 2
       for (int pass = 0; pass < 8; ++pass) {
         const int row = pass * 16 + ty;
@@ -708,69 +591,20 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         *reinterpret_cast<float4*>(s_t1 + swz(row, tx)) = make_float4(gy1[0], gy1[1], gy1[2], gy1[3]);
         *reinterpret_cast<float4*>(s_t1 + HALF_BYTES + swz(row, tx)) = make_float4(gy2[0], gy2[1], gy2[2], gy2[3]);
       }
-      tc::wg_barrier(1, 256);  // the g_p tile is complete
-      tc::mbar_wait(&bars.a_empty, (tl & 1) ^ 1);  // the MMAs of the previous tile have read the A operand
-      tc::fence_after_sync();
-      const uint8_t* src = s_t1 + chalf * HALF_BYTES;
-      const uint32_t a_hi = tmem_base + chalf * 128 + lane_sel, a_lo = a_hi + 64;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 v = *reinterpret_cast<const float4*>(src + swz(crow, g * 4 + q));
-          tc::split_tf32(v.x, hi[q * 4 + 0], lo[q * 4 + 0]);
-          tc::split_tf32(v.y, hi[q * 4 + 1], lo[q * 4 + 1]);
-          tc::split_tf32(v.z, hi[q * 4 + 2], lo[q * 4 + 2]);
-          tc::split_tf32(v.w, hi[q * 4 + 3], lo[q * 4 + 3]);
-        }
-        tc::tmem_st16(a_hi + g * 16, hi);
-        tc::tmem_st16(a_lo + g * 16, lo);
-      }
-      tc::tmem_st_wait();
-      tc::fence_before_sync();
-      mbar_arrive(&bars.a_full);
+      tc::wg_barrier(1, 256);  // every thread is done with the indices of this tile
+      tc::mbar_arrive(&bars.a_full);
     }
-  } else if (warp == 16) {
-    // ============================ M: g_h = g_p . W2 ============================
-    if (lane == 0) {
-      const uint32_t idesc = tc::idesc_tf32(128, 64);
-      const uint32_t img = tc::smem_u32(s_img);
-      int tl = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
-        const int ds = tl & 1;
-        tc::mbar_wait(&bars.a_full, tl & 1);
-        tc::mbar_wait(&bars.d_empty[ds], ((tl >> 1) & 1) ^ 1);
-        tc::fence_after_sync();
-#pragma unroll 1
-        for (int half = 0; half < 2; ++half) {
-          const uint32_t d_acc = tmem_base + 256 + ds * 128 + half * 64;
-          const uint32_t a_hi = tmem_base + half * 128, a_lo = a_hi + 64;
-          const uint32_t bhi = img + half * 2 * IMG_BYTES, blo = bhi + IMG_BYTES;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint64_t bh = tc::smem_desc_kmajor(bhi + j * 256, 128, 2048);
-            const uint64_t bl = tc::smem_desc_kmajor(blo + j * 256, 128, 2048);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bh, idesc, j > 0 ? 1u : 0u);
-            tc::mma_tf32_ts(d_acc, a_lo + j * 8, bh, idesc, 1u);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bl, idesc, 1u);
-          }
-        }
-        tc::mma_commit(&bars.a_empty);
-        tc::mma_commit(&bars.d_full[ds]);
-      }
-    }
-  } else if (warp < 16) {
-    // ============================ F: g_h -> g_pre = g_h * silu'(pre) ============================
+  } else {
+    // ============================ F: g_h = g_p . W2, then g_pre = g_h * silu'(pre) ============================
     const int t = tid - 256;             // 0..255
     const int tx = t & 15, ty = t >> 4;
     const int c0 = tx * 4;
     const int crow = t & 127, chalf = t >> 7;
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
+    const int row0 = ((warp - 8) >> 2) * 64;  // this warpgroup's rows of the products
+    const uint32_t img = tc::smem_u32(s_img);
     int tl = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
       const int base = tile * TR;
-      const int ds = tl & 1;
       if (MODE == ATOM && t < TR) {
         const int r = min(base + t, a.n_rows - 1);
         s_fidx[t] = a.idx0[r];
@@ -784,25 +618,23 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         prefetch_l2(row);
         prefetch_l2(row + 32);
       }
-      tc::mbar_wait(&bars.d_full[ds], (tl >> 1) & 1);
-      tc::fence_after_sync();
-      {
-        const uint32_t d_acc = tmem_base + 256 + ds * 128 + chalf * 64 + lane_sel;
-        uint8_t* dst = s_t2 + chalf * HALF_BYTES;
+      tc::mbar_wait(&bars.a_full, tl & 1);
+#pragma unroll 1
+      for (int half = 0; half < 2; ++half) {
+        float d[32];
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          uint32_t v[32];
-          tc::tmem_ld32(d_acc + g * 32, v);
-          tc::tmem_ld_wait();
+        for (int i = 0; i < 32; ++i) d[i] = 0.f;
+        const uint8_t* src = s_t1 + half * HALF_BYTES;
+        tc::wg_gemm_k64<64>(d, [&](int r, int k) { return *reinterpret_cast<const float*>(src + swz(row0 + r, k >> 2) + (k & 3) * 4); },
+                            img + half * 2 * IMG_BYTES, img + (half * 2 + 1) * IMG_BYTES, 2048);
+        uint8_t* dst = s_t2 + half * HALF_BYTES;
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(dst + swz(crow, g * 8 + q)) =
-                make_float4(__uint_as_float(v[q * 4]), __uint_as_float(v[q * 4 + 1]), __uint_as_float(v[q * 4 + 2]),
-                            __uint_as_float(v[q * 4 + 3]));
+        for (int i = 0; i < 32; i += 2) {
+          const int r = row0 + tc::frag_row(i), c = tc::frag_col(i);
+          *reinterpret_cast<float2*>(dst + swz(r, c >> 2) + (c & 3) * 4) = make_float2(d[i], d[i + 1]);
         }
       }
-      tc::fence_before_sync();
-      mbar_arrive(&bars.d_empty[ds]);
+      tc::mbar_arrive(&bars.a_empty);
       tc::wg_barrier(2, 256);  // the g_h tile (and the index rows) are complete
 #pragma unroll 2
       for (int pass = 0; pass < 8; ++pass) {
@@ -832,10 +664,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
       tc::wg_barrier(2, 256);  // the g_h tile can be overwritten
     }
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 16) tc::tmem_dealloc(tmem_base, 512);
 }
 
 template <int MODE>

@@ -1,22 +1,16 @@
-// chg_linear on the 5th-generation tensor cores (tcgen05, sm_100a), 3xTF32.
+// chg_linear on the Hopper tensor cores (wgmma, sm_90a), 3xTF32.
 //
 //   y[yr] = x[xr] @ wt (+ bias) (+ residual[yr])        x rows of k floats, wt [k][n_out]
 //
 // One persistent CTA per SM, two warpgroups working on alternating 128-row tiles so that one
-// group's loads / epilogue overlap the other group's MMAs.  Thread t of a warpgroup owns row t
-// of its tile end to end:
-//   global rows (64-float chunks, coalesced) -> shared staging -> thread t reads ITS row ->
-//   hi/lo TF32 split -> tcgen05.st into the warpgroup's A region of tensor memory (lane t,
-//   K along columns)
-//   one elected thread: 8 k-steps x 3 split terms of tcgen05.mma.kind::tf32 (A from TMEM,
-//   B = the [NT x k] weight panel, resident in shared memory as hi and lo images in the
-//   K-major no-swizzle canonical layout), tcgen05.commit -> mbarrier
-//   tcgen05.ld of the fp32 accumulator row -> shared staging -> + bias/residual -> coalesced
-//   global rows (thread-per-row 16-byte global accesses are transaction-bound: 8x the L1<->L2
-//   transactions of the staged version)
-// No operand ever passes through the LSU/shared-memory crossbar as an FFMA operand, which is
-// what bounds the FFMA version (profiles/SUMMARY_r01.md).  TMEM: 2 x (64 hi + 64 lo + 128 D)
-// = 512 columns.
+// group's loads / epilogue overlap the other group's MMAs.  Per 64-column chunk of k:
+//   global rows (64-float chunks, coalesced, with the optional row gather) -> shared staging ->
+//   each warp reads its m16 x k8 A fragments from the staging rows, splits them hi / lo ->
+//   wgmma.mma_async m64 x NT x k8 (two 64-row blocks, 8 k-steps x 3 split terms; B = the
+//   [NT x k] weight panel, resident in shared memory as hi and lo images in the K-major
+//   no-swizzle layout), accumulators in registers across the k chunks
+// Epilogue: accumulator fragments -> shared staging (32 columns at a time) -> + bias/residual ->
+// coalesced global rows (with the optional row scatter).
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -25,7 +19,7 @@ namespace {
 
 constexpr int NTHR = 256;
 
-constexpr int IN_LD = 68;   // staging stride (floats) of a 64-float input chunk row
+constexpr int IN_LD = 68;   // staging stride (floats) of a 64-float input chunk row: conflict-free fragment reads
 constexpr int OUT_LD = 36;  // staging stride of a 32-float output chunk row
 constexpr int STAGE_FLOATS = 128 * IN_LD;
 
@@ -38,11 +32,9 @@ linear_tc_kernel(const float* __restrict__ x, const int32_t* __restrict__ x_rows
   uint8_t* s_bhi = smem_raw;
   uint8_t* s_blo = smem_raw + (size_t)NT * k * 4;
   float* s_stage_all = reinterpret_cast<float*>(smem_raw + (size_t)2 * NT * k * 4);
-  __shared__ __align__(8) uint64_t s_bar[2];
-  __shared__ uint32_t s_tmem;
   __shared__ int s_yrow[2][128];
 
-  const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, warp = tid >> 5;
+  const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
   const int col_base = blockIdx.y * NT;
   float* stage = s_stage_all + wg * STAGE_FLOATS;
 
@@ -76,108 +68,56 @@ linear_tc_kernel(const float* __restrict__ x, const int32_t* __restrict__ x_rows
       }
     }
   }
-  if (tid == 0) {
-    tc::mbar_init(&s_bar[0], 1);
-    tc::mbar_init(&s_bar[1], 1);
-    tc::mbar_fence_init();
-  }
-  if (warp == 0) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
 
-  const uint32_t tmem_base = s_tmem;
-  const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-  const uint32_t a_hi = tmem_base + wg * 256, a_lo = a_hi + 64, d_acc = a_hi + 128;
-  const uint32_t idesc = tc::idesc_tf32(128, NT);
   const uint32_t bhi_addr = tc::smem_u32(s_bhi), blo_addr = tc::smem_u32(s_blo);
   const uint32_t sbo = (uint32_t)(k / 4) * 128;
   const int bar_id = 1 + wg;
-  uint32_t phase = 0;
 
   const int n_tiles = (m + 127) / 128;
   const int c4_in = t & 15, row0_in = t >> 4;
-  // software pipeline: the 16 row-chunk loads of the NEXT tile are issued right after this
-  // tile's MMAs, so their latency hides behind the MMA wait and the epilogue
-  float4 pre[16];
-  auto issue_loads = [&](int tile_, int kc_) {
-#pragma unroll
-    for (int q = 0; q < 16; ++q) {
-      const int r = min(tile_ * 128 + row0_in + q * 8, m - 1);
-      const int xr = x_rows != nullptr ? __ldg(x_rows + r) : r;
-      pre[q] = ldg4(x + (size_t)xr * k + kc_ + c4_in * 4);
-    }
-  };
-  int tile = blockIdx.x * 2 + wg;
-  if (tile < n_tiles) issue_loads(tile, 0);
-  for (; tile < n_tiles; tile += gridDim.x * 2) {
+  for (int tile = blockIdx.x * 2 + wg; tile < n_tiles; tile += gridDim.x * 2) {
     const int base = tile * 128;
     {
       const int r = min(base + t, m - 1);
       s_yrow[wg][t] = (base + t < m) ? (y_rows != nullptr ? __ldg(y_rows + r) : r) : -1;
     }
+    float acc[2][NT / 2];
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc[mb][i] = 0.f;
 
     for (int kc = 0; kc < k; kc += 64) {
+      float4 v[16];
 #pragma unroll
-      for (int q = 0; q < 16; ++q) sts4(stage + (row0_in + q * 8) * IN_LD + c4_in * 4, pre[q]);
+      for (int q = 0; q < 16; ++q) {
+        const int r = min(base + row0_in + q * 8, m - 1);
+        const int xr = x_rows != nullptr ? __ldg(x_rows + r) : r;
+        v[q] = ldg4(x + (size_t)xr * k + kc + c4_in * 4);
+      }
+#pragma unroll
+      for (int q = 0; q < 16; ++q) sts4(stage + (row0_in + q * 8) * IN_LD + c4_in * 4, v[q]);
       tc::wg_barrier(bar_id, 128);
-      // thread t: its own row -> hi/lo split -> tensor memory (lane t)
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 v = lds4(stage + t * IN_LD + g * 16 + q * 4);
-          tc::split_tf32(v.x, hi[q * 4 + 0], lo[q * 4 + 0]);
-          tc::split_tf32(v.y, hi[q * 4 + 1], lo[q * 4 + 1]);
-          tc::split_tf32(v.z, hi[q * 4 + 2], lo[q * 4 + 2]);
-          tc::split_tf32(v.w, hi[q * 4 + 3], lo[q * 4 + 3]);
-        }
-        tc::tmem_st16(a_hi + lane_sel + g * 16, hi);
-        tc::tmem_st16(a_lo + lane_sel + g * 16, lo);
+      for (int mb = 0; mb < 2; ++mb) {
+        const float* a_rows = stage + mb * 64 * IN_LD;
+        tc::wg_gemm_k64<NT>(acc[mb], [&](int r, int kk) { return a_rows[r * IN_LD + kk]; }, bhi_addr + kc * 32,
+                            blo_addr + kc * 32, sbo);
       }
-      tc::tmem_st_wait();
-      tc::fence_before_sync();
-      tc::wg_barrier(bar_id, 128);
-      if (t == 0) {
-        tc::fence_after_sync();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t koff = (uint32_t)((kc + 8 * j) / 4) * 128;
-          const uint64_t bh = tc::smem_desc_kmajor(bhi_addr + koff, 128, sbo);
-          const uint64_t bl = tc::smem_desc_kmajor(blo_addr + koff, 128, sbo);
-          tc::mma_tf32_ts(d_acc, a_hi + j * 8, bh, idesc, (kc > 0 || j > 0) ? 1u : 0u);
-          tc::mma_tf32_ts(d_acc, a_lo + j * 8, bh, idesc, 1u);
-          tc::mma_tf32_ts(d_acc, a_hi + j * 8, bl, idesc, 1u);
-        }
-        tc::mma_commit(&s_bar[wg]);
-      }
-      {  // prefetch: next K chunk of this tile, or the first chunk of this warpgroup's next tile
-        const bool more_k = kc + 64 < k;
-        const int nt = more_k ? tile : tile + (int)gridDim.x * 2;
-        if (nt < n_tiles) issue_loads(nt, more_k ? kc + 64 : 0);
-      }
-      tc::mbar_wait(&s_bar[wg], phase);
-      phase ^= 1;
-      tc::fence_after_sync();
+      tc::wg_barrier(bar_id, 128);  // the staging rows may be overwritten
     }
 
-    // accumulator row -> staging (32 columns at a time) -> coalesced global rows
-#pragma unroll 1
-    for (int c = 0; c < NT; c += 32) {
-      uint32_t v[16], w[16];
-      tc::tmem_ld16(d_acc + lane_sel + c, v);
-      tc::tmem_ld16(d_acc + lane_sel + c + 16, w);
-      tc::tmem_ld_wait();
+    // accumulator fragments -> staging (32 columns at a time) -> coalesced global rows
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        sts4(stage + t * OUT_LD + q * 4, make_float4(__uint_as_float(v[q * 4 + 0]), __uint_as_float(v[q * 4 + 1]),
-                                                     __uint_as_float(v[q * 4 + 2]), __uint_as_float(v[q * 4 + 3])));
-        sts4(stage + t * OUT_LD + 16 + q * 4,
-             make_float4(__uint_as_float(w[q * 4 + 0]), __uint_as_float(w[q * 4 + 1]), __uint_as_float(w[q * 4 + 2]),
-                         __uint_as_float(w[q * 4 + 3])));
-      }
+    for (int c = 0; c < NT; c += 32) {
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = c / 2; i < c / 2 + 16; i += 2)
+          *reinterpret_cast<float2*>(stage + (mb * 64 + tc::frag_row(i)) * OUT_LD + tc::frag_col(i) - c) =
+              make_float2(acc[mb][i], acc[mb][i + 1]);
       tc::wg_barrier(bar_id, 128);
       {
         const int c4 = t & 7, row0 = t >> 3;
@@ -202,12 +142,7 @@ linear_tc_kernel(const float* __restrict__ x, const int32_t* __restrict__ x_rows
       }
       tc::wg_barrier(bar_id, 128);
     }
-    tc::fence_before_sync();  // accumulator reads ordered before the next tile's MMAs
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 512);
 }
 
 template <int NT>

@@ -1,19 +1,17 @@
-// chg_linear, warp-specialised tcgen05 pipeline fed by 2-D TMA tensor maps (k in {64,128},
+// chg_linear, warp-specialised wgmma pipeline fed by 2-D TMA tensor maps (k in {64,128},
 // no row gather/scatter):   y = x @ wt (+ bias) (+ residual)
 //
-//   warp 0      producer   one lane issues cp.async.bulk.tensor.2d loads (128B swizzle) of the
+//   warp 8      producer   one lane issues cp.async.bulk.tensor.2d loads (128B swizzle) of the
 //                          next [128 rows x 64 cols] chunk into a 2-stage shared-memory ring
 //                          (and of the residual tile into the output stage)
-//   warps 2-5   converter  thread t reads ITS row from the swizzled stage (conflict-free),
-//                          splits hi/lo (3xTF32) and tcgen05.st's it into one of two A stages
-//                          in tensor memory
-//   warp 1      MMA        one lane issues 8 k-steps x 3 split terms of tcgen05.mma.kind::tf32
-//                          per chunk into one of two D stages in tensor memory, tcgen05.commit
-//   warps 6-9   epilogue   tcgen05.ld of the accumulator row, + bias / residual, swizzled store
-//                          to the output stage, one lane issues the TMA tensor store
+//   warps 0-7   consumers  two warpgroups, rows 0-63 / 64-127 of every tile: each warp reads its
+//                          m16 x k8 A fragments from the swizzled stage (conflict-free), splits
+//                          them hi/lo (3xTF32) and the warpgroup issues 8 k-steps x 3 split terms
+//                          of wgmma.mma_async m64 x NT x k8 per chunk against the weight panel
+//                          images (accumulators in registers); then + bias / residual, swizzled
+//                          store to the output stage, one lane issues the TMA tensor store
 // Every hand-off is an mbarrier (full/empty per ring slot); nothing on the critical path is a
-// synchronous global access, so HBM stays busy while the tensor pipe works on the previous tile.
-// TMEM: 2 x (64 hi + 64 lo) A + 2 x 128 D = 512 columns.
+// synchronous global access, so HBM stays busy while the tensor cores work on the current chunk.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -22,21 +20,17 @@
 namespace chg {
 namespace {
 
-constexpr int NTHR = 320;
+constexpr int NTHR = 288;
+constexpr int PRODUCER_WARP = 8;
 constexpr int S_IN = 2;                 // input ring depth (chunks of 128 rows x 64 floats)
 constexpr int PANEL = 128 * 128;        // bytes of one 128-row x 32-float swizzled panel
 constexpr int IN_STAGE = 2 * PANEL;     // 64 columns = 2 panels
 
 struct Bars {
   uint64_t in_full[S_IN], in_empty[S_IN];
-  uint64_t a_full[2], a_empty[2];
-  uint64_t d_full[2], d_empty[2];
   uint64_t res_full, out_empty;
 };
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
@@ -51,6 +45,8 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int
 }
 // byte offset of 16-byte chunk `c` of row `r` inside a 128B-swizzled panel
 __device__ __forceinline__ int swz(int r, int c) { return r * 128 + ((c ^ (r & 7)) << 4); }
+// byte offset of element (r, col) of a tile stored as consecutive 32-column swizzled panels
+__device__ __forceinline__ int panel_offset(int r, int col) { return (col >> 5) * PANEL + swz(r, (col & 31) >> 2) + (col & 3) * 4; }
 
 template <int NT>
 __global__ void __launch_bounds__(NTHR, 1)
@@ -64,7 +60,6 @@ linear_ws_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   uint8_t* s_bhi = s_out + (NT / 32) * PANEL;
   uint8_t* s_blo = s_bhi + (size_t)NT * k * 4;
   __shared__ __align__(8) Bars bars;
-  __shared__ uint32_t s_tmem;
   __shared__ __align__(16) float s_bias[NT];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -72,7 +67,7 @@ linear_ws_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   const int n_tiles = (m + 127) / 128;
   const int k_chunks = k / 64;
 
-  // ---- one-time setup: weight images, bias, barriers, tensor memory --------------------------
+  // ---- one-time setup: weight images, bias, barriers ------------------------------------------
   {
     const int n4 = NT / 4, total4 = n4 * k;
     for (int i4 = tid; i4 < total4; i4 += NTHR) {
@@ -92,27 +87,16 @@ linear_ws_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   if (tid == 0) {
     for (int i = 0; i < S_IN; ++i) {
       tc::mbar_init(&bars.in_full[i], 1);
-      tc::mbar_init(&bars.in_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&bars.a_full[i], 1);
-      tc::mbar_init(&bars.a_empty[i], 1);
-      tc::mbar_init(&bars.d_full[i], 1);
-      tc::mbar_init(&bars.d_empty[i], 1);
+      tc::mbar_init(&bars.in_empty[i], 256);
     }
     tc::mbar_init(&bars.res_full, 1);
     tc::mbar_init(&bars.out_empty, 1);
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc(&s_tmem, 512);
   tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = s_tmem;
-  // TMEM columns: A stage s at s*128 (hi) / s*128+64 (lo); D stage s at 256 + s*128
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ================= producer =================
     if (lane == 0) {
       int it = 0, tile_it = 0;
@@ -133,122 +117,52 @@ linear_ws_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = tc::idesc_tf32(128, NT);
-      const uint32_t bhi_addr = tc::smem_u32(s_bhi), blo_addr = tc::smem_u32(s_blo);
-      const uint32_t sbo = (uint32_t)(k / 4) * 128;
-      int it = 0, tile_it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_it) {
-        const int ds = tile_it & 1;
-        tc::mbar_wait(&bars.d_empty[ds], ((tile_it >> 1) & 1) ^ 1);
-        tc::fence_after_sync();
-        const uint32_t d_acc = tmem_base + 256 + ds * 128;
-        for (int kc = 0; kc < k_chunks; ++kc, ++it) {
-          const int as = it & 1;
-          tc::mbar_wait(&bars.a_full[as], (it >> 1) & 1);
-          tc::fence_after_sync();
-          const uint32_t a_hi = tmem_base + as * 128, a_lo = a_hi + 64;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint32_t koff = (uint32_t)((kc * 64 + 8 * j) / 4) * 128;
-            const uint64_t bh = tc::smem_desc_kmajor(bhi_addr + koff, 128, sbo);
-            const uint64_t bl = tc::smem_desc_kmajor(blo_addr + koff, 128, sbo);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bh, idesc, (kc > 0 || j > 0) ? 1u : 0u);
-            tc::mma_tf32_ts(d_acc, a_lo + j * 8, bh, idesc, 1u);
-            tc::mma_tf32_ts(d_acc, a_hi + j * 8, bl, idesc, 1u);
-          }
-          tc::mma_commit(&bars.a_empty[as]);  // A stage reusable once these MMAs have read it
-        }
-        tc::mma_commit(&bars.d_full[ds]);
-      }
-    }
-  } else if (warp < 6) {
-    // ================= converter warpgroup (warps 2..5) =================
-    const int r = (warp & 3) * 32 + lane;  // TMEM lane == tile row
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    const int t = tid - 64;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      for (int kc = 0; kc < k_chunks; ++kc, ++it) {
-        const int s = it % S_IN, as = it & 1;
-        tc::mbar_wait(&bars.in_full[s], (it / S_IN) & 1);
-        tc::mbar_wait(&bars.a_empty[as], ((it >> 1) & 1) ^ 1);
-        tc::fence_after_sync();
-        const uint8_t* stage = s_in + s * IN_STAGE;
-        const uint32_t a_hi = tmem_base + as * 128, a_lo = a_hi + 64;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {  // 16 columns: panel g/2, chunks (g%2)*4 .. +3
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 v =
-                *reinterpret_cast<const float4*>(stage + (g >> 1) * PANEL + swz(r, (g & 1) * 4 + q));
-            tc::split_tf32(v.x, hi[q * 4 + 0], lo[q * 4 + 0]);
-            tc::split_tf32(v.y, hi[q * 4 + 1], lo[q * 4 + 1]);
-            tc::split_tf32(v.z, hi[q * 4 + 2], lo[q * 4 + 2]);
-            tc::split_tf32(v.w, hi[q * 4 + 3], lo[q * 4 + 3]);
-          }
-          tc::tmem_st16(a_hi + lane_sel + g * 16, hi);
-          tc::tmem_st16(a_lo + lane_sel + g * 16, lo);
-        }
-        tc::tmem_st_wait();
-        tc::fence_before_sync();
-        tc::wg_barrier(1, 128);
-        if (t == 0) {
-          mbar_arrive(&bars.a_full[as]);
-          mbar_arrive(&bars.in_empty[s]);
-        }
-      }
-    }
   } else {
-    // ================= epilogue warpgroup (warps 6..9) =================
-    const int r = (warp & 3) * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    const int t = tid - 192;
-    int tile_it = 0;
+    // ================= consumer warpgroups (warps 0..3: rows 0..63, warps 4..7: rows 64..127) =================
+    const int t = tid;            // 0..255
+    const int row0 = (warp >> 2) * 64;
+    const uint32_t bhi_addr = tc::smem_u32(s_bhi), blo_addr = tc::smem_u32(s_blo);
+    const uint32_t sbo = (uint32_t)(k / 4) * 128;
+    int it = 0, tile_it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_it) {
       const int base = tile * 128;
-      const int ds = tile_it & 1;
-      tc::mbar_wait(&bars.d_full[ds], (tile_it >> 1) & 1);
-      tc::fence_after_sync();
-      if (has_residual) tc::mbar_wait(&bars.res_full, tile_it & 1);
-      tc::wg_barrier(2, 128);  // the previous tile's TMA store has finished reading the output stage
-      const uint32_t d_acc = tmem_base + 256 + ds * 128;
-#pragma unroll 1
-      for (int c = 0; c < NT; c += 16) {
-        uint32_t v[16];
-        tc::tmem_ld16(d_acc + lane_sel + c, v);
-        tc::tmem_ld_wait();
+      float acc[NT / 2];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float4 o = make_float4(__uint_as_float(v[q * 4 + 0]), __uint_as_float(v[q * 4 + 1]),
-                                 __uint_as_float(v[q * 4 + 2]), __uint_as_float(v[q * 4 + 3]));
-          o = o + lds4(s_bias + c + q * 4);
-          float4* dst = reinterpret_cast<float4*>(s_out + (c >> 5) * PANEL + swz(r, ((c & 31) >> 2) + q));
-          if (has_residual) o = o + *dst;
-          *dst = o;
-        }
+      for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+      for (int kc = 0; kc < k_chunks; ++kc, ++it) {
+        const int s = it % S_IN;
+        tc::mbar_wait(&bars.in_full[s], (it / S_IN) & 1);
+        const uint8_t* stage = s_in + s * IN_STAGE;
+        tc::wg_gemm_k64<NT>(acc, [&](int r, int kk) { return *reinterpret_cast<const float*>(stage + panel_offset(row0 + r, kk)); },
+                            bhi_addr + kc * 2048, blo_addr + kc * 2048, sbo);
+        tc::mbar_arrive(&bars.in_empty[s]);
       }
-      tc::fence_before_sync();
+      if (has_residual) tc::mbar_wait(&bars.res_full, tile_it & 1);
+      tc::wg_barrier(2, 256);  // the previous tile's TMA store has finished reading the output stage
+#pragma unroll
+      for (int i = 0; i < NT / 2; i += 2) {
+        const int r = row0 + tc::frag_row(i), col = tc::frag_col(i);
+        float2* dst = reinterpret_cast<float2*>(s_out + panel_offset(r, col));
+        float2 o = make_float2(acc[i] + s_bias[col], acc[i + 1] + s_bias[col + 1]);
+        if (has_residual) {
+          const float2 res = *dst;
+          o.x += res.x;
+          o.y += res.y;
+        }
+        *dst = o;
+      }
       tc::fence_async_smem();
-      tc::wg_barrier(2, 128);
+      tc::wg_barrier(2, 256);
       if (t == 0) {
-        mbar_arrive(&bars.d_empty[ds]);
 #pragma unroll
         for (int p = 0; p < NT / 32; ++p) tma_store_2d(&map_y, col_base + p * 32, base, s_out + p * PANEL);
         tc::bulk_commit();
         tc::bulk_wait_read<0>();
-        mbar_arrive(&bars.out_empty);
+        tc::mbar_arrive(&bars.out_empty);
       }
     }
     if (t == 0) tc::bulk_wait_all<0>();
   }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 512);
 }
 
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

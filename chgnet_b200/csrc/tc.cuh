@@ -1,10 +1,15 @@
-// tcgen05 / TMEM / mbarrier primitives for sm_100a (inline PTX; no CUTLASS dependency).
+// Hopper tensor-core / mbarrier / bulk-copy primitives for sm_90a (inline PTX; no CUTLASS dependency).
 //
 // Precision: the model needs fp32-level products (DESIGN.md §4), so every GEMM is issued as
 // a 3xTF32 split:  a = a_hi + a_lo with a_hi = a with its 13 low mantissa bits cleared
 // (exactly a TF32 number) and a_lo = a - a_hi (exact in fp32), likewise b;
 //   a.b ~= a_hi.b_hi + a_lo.b_hi + a_hi.b_lo          (error ~2^-21 relative)
-// accumulated in fp32 in tensor memory.
+// accumulated in fp32 in the registers of the issuing warpgroup (wgmma.mma_async, m64nNk8).
+//
+// Operand layouts: B (and A in the shared-memory form) are K-major no-swizzle images of 8-row x
+// 16-byte core matrices (kmajor_offset); A in the register form is the m16n8k8 tf32 fragment per
+// warp.  Accumulator fragment of a m64nN product, warp w of the warpgroup, lane l (g = l / 4,
+// c = l % 4):  d[4j + 0 / 1] = D[16w + g][8j + 2c + 0 / 1],  d[4j + 2 / 3] = D[16w + g + 8][8j + 2c + 0 / 1].
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,21 +19,7 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// ---- TMEM allocation (one warp, .sync.aligned) ------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---- fences ---------------------------------------------------------------------------------
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// generic-proxy writes to shared memory -> visible to the async proxy (tensor core operand reads)
+// generic-proxy writes to shared memory -> visible to the async proxy (tensor core operand reads, TMA stores)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- mbarrier -------------------------------------------------------------------------------
@@ -36,6 +27,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 // bounded spin: a lost arrive traps instead of hanging the GPU
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
@@ -52,83 +46,61 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
   __trap();
 }
-// arrive on `bar` when all tcgen05.mma issued so far by this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
 
-// ---- descriptors ----------------------------------------------------------------------------
-// K-major operand, no swizzle ("interleave"): 8-row x 16-byte core matrices stored as 128
-// contiguous bytes; lbo = byte distance between the two core matrices one MMA consumes along K,
-// sbo = byte distance between 8-row groups.  (cute: ((8,m),(T,2)):((1T,SBO),(1,LBO)))
+// ---- wgmma ----------------------------------------------------------------------------------
+// shared-memory matrix descriptor, K-major, no swizzle: lbo = byte distance between the two core
+// matrices one k8 step consumes along K, sbo = byte distance between 8-row groups
+// (cute: ((8,m),(T,2)):((1T,SBO),(1,LBO)))
 __device__ __forceinline__ uint64_t smem_desc_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // base_offset 0, lbo_mode 0, layout_type 0 = SWIZZLE_NONE
+  return d;  // base_offset 0, layout_type 0 = no swizzle
 }
-// instruction descriptor: D fp32, A/B tf32, both K-major, M x N
-__host__ __device__ constexpr uint32_t idesc_tf32(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-
-// D[tmem] (+)= A[tmem] . B[smem]^T ; one thread issues
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// D[tmem] (+)= A[smem] . B[smem]^T ; both operands K-major in shared memory; one thread issues
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
+// D[64 x N] += A . B^T, one warpgroup; A from registers (tf32 fragment), B from shared memory
+__device__ __forceinline__ void wgmma_tf32_m64n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "{%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc)
       : "memory");
 }
-
-// ---- TMEM <-> registers (warp w touches lanes 32*(w%4) .. +31; thread i = lane i) --------------
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_tf32_m64n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "{%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc)
       : "memory");
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_tf32_ss_m64n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc) {
+  if constexpr (N == 64) wgmma_tf32_m64n64(d, a, b_desc);
+  else wgmma_tf32_m64n128(d, a, b_desc);
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---- 3xTF32 split -----------------------------------------------------------------------------
 __device__ __forceinline__ void split_tf32(float a, uint32_t& hi, uint32_t& lo) {
@@ -141,6 +113,43 @@ __host__ __device__ constexpr uint32_t kmajor_offset(int row, int k, int K) {
   return (uint32_t)((row >> 3) * (K / 4) * 128 + (k >> 2) * 128 + (row & 7) * 16 + (k & 3) * 4);
 }
 
+// d[64 x N] += A[64 x 64] . B^T as 3xTF32 on one warpgroup (all 128 threads call it).
+// A: fp32, element (r, k) of this warpgroup's 64-row block read from shared memory as a_at(r, k);
+// B: hi / lo images (byte addresses of the slice's first k) of N rows x K, sbo = byte stride of 8 rows.
+// Returns with the products complete (A may be overwritten).
+template <int N, class AFn>
+__device__ __forceinline__ void wg_gemm_k64(float (&d)[N / 2], AFn a_at, uint32_t bhi, uint32_t blo, uint32_t sbo) {
+  const int lane = threadIdx.x & 31;
+  const int r = 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2), c = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = (h * 4 + j) * 8 + c;
+      split_tf32(a_at(r, k), ahi[j][0], alo[j][0]);
+      split_tf32(a_at(r + 8, k), ahi[j][1], alo[j][1]);
+      split_tf32(a_at(r, k + 4), ahi[j][2], alo[j][2]);
+      split_tf32(a_at(r + 8, k + 4), ahi[j][3], alo[j][3]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t koff = (uint32_t)(h * 4 + j) * 256;
+      const uint64_t bh = smem_desc_kmajor(bhi + koff, 128, sbo), bl = smem_desc_kmajor(blo + koff, 128, sbo);
+      wgmma_tf32<N>(d, ahi[j], bh);
+      wgmma_tf32<N>(d, alo[j], bh);
+      wgmma_tf32<N>(d, ahi[j], bl);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+  }
+}
+
+// this thread's accumulator element i of a m64nN fragment: (row, col) inside the 64 x N block
+__device__ __forceinline__ int frag_row(int i) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + ((i >> 1) & 1) * 8; }
+__device__ __forceinline__ int frag_col(int i) { return (i >> 2) * 8 + 2 * (threadIdx.x & 3) + (i & 1); }
+
 // named barrier for one warpgroup (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void wg_barrier(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -149,25 +158,12 @@ __device__ __forceinline__ void wg_barrier(int id, int nthreads) {
 }  // namespace tc
 }  // namespace chg
 
-// ---- TMA-style bulk copies (cp.async.bulk, no tensor map: 1-D, 16-byte granular) -----------------
+// ---- TMA completion and bulk-group bookkeeping -------------------------------------------------
 namespace chg {
 namespace tc {
 // one thread: this phase of `bar` completes after `bytes` more bytes have landed (plus 1 arrival)
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-// global -> shared, completion signalled on `bar` (bytes % 16 == 0, both addresses 16-byte aligned)
-__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-// shared -> global, tracked by the issuing thread's bulk async-group
-__device__ __forceinline__ void bulk_store(void* gmem_dst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(smem_u32(smem_src)),
-               "r"(bytes)
-               : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // wait until at most N of this thread's bulk groups still READ their shared-memory source

@@ -488,13 +488,13 @@ void wgrad_reduce_launch(const float* partial, const float* cs_partial, int n_ch
 int wgrad_tc(const float* x, const float* x2, int ldx, const int32_t* x_rows, int x_silu, const float* g, int ldg,
              const int32_t* g_rows, int m, int n_out, float* out, int ldo, float* colsum, float* workspace, int max_chunks,
              cudaStream_t stream);  // wgrad_tc.cu: returns 1 when it does not take the call
-int wgrad_impl();  // abi.cu: 1 = tcgen05 (default), 0 = FFMA
+int wgrad_impl();  // abi.cu: 1 = tensor cores (wgmma, default), 0 = FFMA
 }  // namespace chg
 
 using namespace chg;
 
 extern "C" int64_t chg_wgrad_workspace_floats(int32_t n_out) {
-  // chunks(n) * (64 n + n) with chunks(n) <= min(WG_MAX_CHUNKS, 2 * 256 / n * SMs): largest at n = 256 on 148+ SMs
+  // chunks(n) * (64 n + n) with chunks(n) <= min(WG_MAX_CHUNKS, 2 * 256 / n * SMs): largest at n = 256
   const int64_t chunks = std::min<int64_t>(WG_MAX_CHUNKS, (int64_t)sm_count() * 2 * std::max(1, 256 / n_out));
   return chunks * (64 * (int64_t)n_out + n_out);
 }

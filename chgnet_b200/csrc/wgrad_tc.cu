@@ -1,4 +1,4 @@
-// chg_wgrad on the tensor cores (sm_100a):  out[64][n] = act(X[xr])^T . G[gr]   (reduction over the m rows)
+// chg_wgrad on the Hopper tensor cores (wgmma, sm_90a):  out[64][n] = act(X[xr])^T . G[gr]   (reduction over the m rows)
 //
 // The weight gradients of the training step (reference trainer.py:409 loss.backward(): dL/dW of every dense layer) are
 // true GEMMs with the ROWS as the contraction dimension: [64 x m] . [m x n], m up to the number of angles (4e5 per GPU in
@@ -7,10 +7,10 @@
 //   D[j][i] (+)= sum_k G[k][c0 + j] * act(X)[k][i]          A = G^T block (M = 128 columns of G, zero rows when the
 //                                                            block is 64 wide), B = act(X)^T (N = 64), K = rows
 //
-// as 3xTF32 tcgen05.mma.kind::tf32 (M=128, N=64, K=8) with BOTH operands in shared memory: every 32-row stage is
-// transposed into the no-swizzle K-major operand images (hi and lo parts) by the 8 warps - lane <-> column, four rows
-// per 16-byte store, conflict-free - while the MMAs of the previous stage run (two stages, one mbarrier each).
-// Accumulator: 64 TMEM columns.  Each CTA owns a contiguous range of rows and one 128-column block and writes a
+// as 3xTF32 wgmma.mma_async m64n64k8 with BOTH operands in shared memory (warpgroup w takes the 64 columns 64w.. of
+// the G block): every 32-row stage is transposed into the no-swizzle K-major operand images (hi and lo parts) by the
+// 8 warps - lane <-> column, four rows per 16-byte store, conflict-free - while the MMAs of the previous stage run
+// (two stages; wgmma.wait_group 1 before a stage is rewritten).  Accumulator: 32 registers per thread.  Each CTA owns a contiguous range of rows and one 128-column block and writes a
 // partial [64][n] tile; the fp64 second pass of train.cu (wgrad_reduce_kernel) sums the partials in fixed order.
 #include "common.cuh"
 #include "tc.cuh"
@@ -41,8 +41,6 @@ wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ x2, int l
   uint8_t* s_stage = smem_raw;
   int* s_xi = reinterpret_cast<int*>(smem_raw + 2 * STAGE);  // [2][WT_K] row of X
   int* s_gi = s_xi + 2 * WT_K;                               // [2][WT_K] row of G
-  __shared__ __align__(8) uint64_t s_free[2];
-  __shared__ uint32_t s_tmem;
   __shared__ float s_cs[8][128];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -56,20 +54,14 @@ wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ x2, int l
   if (n_block < 128) {
     for (int i = tid * 4; i < 2 * STAGE / 4; i += WT_THREADS * 4) sts4(reinterpret_cast<float*>(s_stage) + i, make_float4(0.f, 0.f, 0.f, 0.f));
   }
-  if (tid == 0) {
-    tc::mbar_init(&s_free[0], 1);
-    tc::mbar_init(&s_free[1], 1);
-    tc::mbar_fence_init();
-  }
-  if (warp == 0) tc::tmem_alloc(&s_tmem, 64);
-  tc::fence_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t d_tmem = s_tmem;
+  const int wg = warp >> 2;
+  const bool wg_live = wg == 0 || n_block > 64;  // a 64-wide block leaves the second warpgroup's rows of A zero
+  float d[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) d[i] = 0.f;
 
   float cs[4] = {0.f, 0.f, 0.f, 0.f};  // column sums of G for this lane's columns lane + 32 c
-  const uint32_t idesc = tc::idesc_tf32(128, 64);
   int it = 0;
   for (int step = s_beg; step < s_end; ++step, ++it) {
     const int st = it & 1;
@@ -77,8 +69,8 @@ wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ x2, int l
     uint8_t* a_lo = a_hi + A_IMG;
     uint8_t* b_hi = a_lo + A_IMG;
     uint8_t* b_lo = b_hi + B_IMG;
-    // the MMAs that read this stage two iterations ago have completed
-    if (it >= 2) tc::mbar_wait(&s_free[st], ((it >> 1) - 1) & 1);
+    // the MMAs that read this stage two iterations ago have completed (both warpgroups: the barrier below)
+    tc::wgmma_wait<1>();
     const int base = step * WT_K;
     if (tid < WT_K) {
       const int row = min(base + tid, m - 1);
@@ -132,44 +124,30 @@ wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ x2, int l
     }
     tc::fence_async_smem();  // generic-proxy writes -> visible to the tensor core's operand reads
     __syncthreads();
-    if (tid == 0) {
-      tc::fence_after_sync();
-      const uint32_t ah = tc::smem_u32(a_hi), al = tc::smem_u32(a_lo), bh = tc::smem_u32(b_hi), bl = tc::smem_u32(b_lo);
+    if (wg_live) {
+      // this warpgroup's 64 rows of the G^T image (8192 bytes per 64 rows of a 32-wide K-major image)
+      const uint32_t ah = tc::smem_u32(a_hi) + wg * 8192, al = tc::smem_u32(a_lo) + wg * 8192;
+      const uint32_t bh = tc::smem_u32(b_hi), bl = tc::smem_u32(b_lo);
       const uint32_t sbo = (WT_K / 4) * 128;
+      tc::wgmma_fence();
 #pragma unroll
       for (int j = 0; j < WT_K / 8; ++j) {
         const uint64_t dah = tc::smem_desc_kmajor(ah + j * 256, 128, sbo), dal = tc::smem_desc_kmajor(al + j * 256, 128, sbo);
         const uint64_t dbh = tc::smem_desc_kmajor(bh + j * 256, 128, sbo), dbl = tc::smem_desc_kmajor(bl + j * 256, 128, sbo);
-        tc::mma_tf32_ss(d_tmem, dah, dbh, idesc, (it > 0 || j > 0) ? 1u : 0u);
-        tc::mma_tf32_ss(d_tmem, dal, dbh, idesc, 1u);
-        tc::mma_tf32_ss(d_tmem, dah, dbl, idesc, 1u);
+        tc::wgmma_tf32_ss_m64n64(d, dah, dbh);
+        tc::wgmma_tf32_ss_m64n64(d, dal, dbh);
+        tc::wgmma_tf32_ss_m64n64(d, dah, dbl);
       }
-      tc::mma_commit(&s_free[st]);
+      tc::wgmma_commit();
     }
   }
-  // ---- wait for the last MMAs of both stages, then accumulator -> partial tile ------------------------------------
-  if (it >= 1) tc::mbar_wait(&s_free[(it - 1) & 1], ((it - 1) >> 1) & 1);
-  if (it >= 2) tc::mbar_wait(&s_free[it & 1], ((it - 2) >> 1) & 1);
-  tc::fence_after_sync();
+  // ---- wait for the last MMAs, then accumulator fragments -> partial tile: out[i][j], i = feature of X, j = column of G
+  tc::wgmma_wait<0>();
   float* dst = partial + (size_t)blockIdx.x * 64 * n;
-  if (warp < 4) {
-    const int j = warp * 32 + lane;  // TMEM lane = column of G inside the block
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      uint32_t v[16];
-      if (it > 0) {
-        tc::tmem_ld16(d_tmem + lane_sel + c * 16, v);
-        tc::tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) v[q] = 0u;
-      }
-      if (j < n_block) {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) dst[(size_t)(c * 16 + q) * n + col_base + j] = __uint_as_float(v[q]);  // out[i][j], coalesced in j
-      }
-    }
+  for (int q = 0; q < 32; ++q) {
+    const int j = wg * 64 + tc::frag_row(q);
+    if (j < n_block) dst[(size_t)tc::frag_col(q) * n + col_base + j] = d[q];
   }
   if (cs_partial != nullptr) {
 #pragma unroll
@@ -182,9 +160,6 @@ wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ x2, int l
       cs_partial[(size_t)blockIdx.x * n + col_base + tid] = t;
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(d_tmem, 64);
 }
 
 }  // namespace
@@ -226,7 +201,7 @@ int wgrad_tc(const float* x, const float* x2, int ldx, const int32_t* x_rows, in
   {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
-      set_error("chg_wgrad (tcgen05): launch failed: %s", cudaGetErrorString(e));
+      set_error("chg_wgrad (wgmma): launch failed: %s", cudaGetErrorString(e));
       return CHG_ERR_CUDA;
     }
     count_launch();
@@ -234,7 +209,7 @@ int wgrad_tc(const float* x, const float* x2, int ldx, const int32_t* x_rows, in
   wgrad_reduce_launch(partial, cs_partial, n_chunks, n_out, out, ldo, colsum, stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
-    set_error("chg_wgrad (tcgen05): reduce launch failed: %s", cudaGetErrorString(e));
+    set_error("chg_wgrad (wgmma): reduce launch failed: %s", cudaGetErrorString(e));
     return CHG_ERR_CUDA;
   }
   count_launch();

@@ -76,7 +76,7 @@ class Atoms:
 
 
 class CHGNetCalculator(_Base):
-    """CHGNet calculator (reference dynamics.py:58-181) on the B200 kernel path."""
+    """CHGNet calculator (reference dynamics.py:58-181) on the H100 kernel path."""
 
     implemented_properties = ("energy", "forces", "stress", "magmoms", "energies")
 

@@ -1,4 +1,4 @@
-"""``CHGNet`` — drop-in model API over the B200 kernel engine.
+"""``CHGNet`` — drop-in model API over the H100 kernel engine.
 
 Mirrors the public surface of the reference class (reference
 chgnet/model/model.py:35-745): constructor keywords, ``forward`` (330-387),
@@ -306,7 +306,7 @@ class StaticGraphEvaluator:
 
 
 class CHGNet(nn.Module):
-    """Crystal Hamiltonian Graph neural Network — B200 kernel path."""
+    """Crystal Hamiltonian Graph neural Network — H100 kernel path."""
 
     def __init__(
         self,
@@ -415,7 +415,7 @@ class CHGNet(nn.Module):
         dev = self.device
         if dev.type != "cuda":
             raise RuntimeError(
-                "chgnet_b200.CHGNet has no CPU path: move the model to a CUDA device (B200) first "
+                "chgnet_b200.CHGNet has no CPU path: move the model to a CUDA device (H100) first "
                 f"(parameters are on {dev})")
         sd = self.state_dict()
         key = (str(dev), tuple(int(v._version) for v in sd.values()), tuple(v.data_ptr() for v in sd.values()))
@@ -433,7 +433,7 @@ class CHGNet(nn.Module):
         dev = self.device
         if dev.type != "cuda":
             raise RuntimeError(
-                "chgnet_b200.CHGNet has no CPU path: move the model to a CUDA device (B200) first "
+                "chgnet_b200.CHGNet has no CPU path: move the model to a CUDA device (H100) first "
                 f"(parameters are on {dev})")
         sd = self.state_dict()
         key = (str(dev), tuple(int(v._version) for v in sd.values()), tuple(v.data_ptr() for v in sd.values()))

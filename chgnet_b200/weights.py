@@ -6,7 +6,7 @@ source of truth; this module only produces re-arranged *views/copies* of them
 per-atom / per-bond / per-angle column blocks).  Call again after a parameter
 update.
 
-First-layer split (the algebraic core of the B200 design, DESIGN.md §3):
+First-layer split (the algebraic core of the H100 design, DESIGN.md §3):
 ``W1 [x_c | e_u | x_n] = W1[:, 0:64] x_c + W1[:, 64:128] e_u + W1[:, 128:192] x_n``
 so the 192->128 (AtomConv, reference layers.py:113-117) and 256->128 (BondConv /
 AngleUpdate, layers.py:238-244, 348-355) products are computed once per ATOM and

@@ -1,5 +1,5 @@
 /*
- * chgnet_b200.h — C ABI of the B200-native CHGNet hot path (libchgnet_b200.so).
+ * chgnet_b200.h — C ABI of the H100-native CHGNet hot path (libchgnet_b200.so).
  *
  * The reference (CederGroupHub/chgnet) has NO native interface for this path:
  * it is pure PyTorch (SURVEY.md §2b).  This header is therefore the boundary a
@@ -45,15 +45,15 @@ int chg_abi_version(void);
 /* number of kernel launches issued by this library since load (host counter) */
 int64_t chg_launch_count(void);
 /* implementation switches for A/B measurements (same results, same ABI):
- *   "linear_impl": 0 FFMA, 1 tcgen05 register-staged, 2 tcgen05 + TMA row copies,
- *                  3 warp-specialised tcgen05 fed by 2-D TMA tensor maps (default; calls with
+ *   "linear_impl": 0 FFMA, 1 wgmma register-staged, 2 wgmma + TMA row copies,
+ *                  3 warp-specialised wgmma fed by 2-D TMA tensor maps (default; calls with
  *                    row indirection or k = 256 use 1)
- *   "gated_impl" : 3 fused warp-specialised tcgen05 message + aggregation (default; chg_*_conv_fused),
- *                  0 FFMA 4x8 tiles, 1 tcgen05 (un-pipelined), 2 FFMA 8x8 tiles (all unfused; with 3 the
+ *   "gated_impl" : 3 fused warp-specialised wgmma message + aggregation (default; chg_*_conv_fused),
+ *                  0 FFMA 4x8 tiles, 1 wgmma (un-pipelined), 2 FFMA 8x8 tiles (all unfused; with 3 the
  *                  unfused entry points chg_*_conv_fwd / _bwd run the FFMA 4x8 kernels)
  *   "ws_min_rows": calls with fewer rows than this (default 4096) run the FFMA kernels even with gated_impl 3
- *                  (launch-bound regime: the persistent tcgen05 kernels' fixed cost loses on a few tiles)
- *   "wgrad_impl" : 1 tcgen05 3xTF32 for reductions over >= 4096 rows (default; csrc/wgrad_tc.cu), 0 FFMA
+ *                  (launch-bound regime: the persistent wgmma kernels' fixed cost loses on a few tiles)
+ *   "wgrad_impl" : 1 wgmma 3xTF32 for reductions over >= 4096 rows (default; csrc/wgrad_tc.cu), 0 FFMA
  *   "segsum_unroll": 4 (default) or 8 input rows in flight per lane-group of chg_segment_sum (identical results)
  *   "segsum_s"   : 0 (default: chosen from the mean segment length) or 1 / 2 / 4 / 8 lane-groups per output row
  * (env CHG_LINEAR_IMPL / CHG_GATED_IMPL = 0..3, CHG_WGRAD_IMPL = 0..1, CHG_WS_MIN_ROWS, CHG_SEGSUM_UNROLL, CHG_SEGSUM_S set
@@ -146,7 +146,7 @@ int chg_segment_sum(const float* data, int32_t width, const int32_t* perm,
  * agg[s] = sum over the rows r of segment s of  G(pre_r) * w_r,  rows sorted by segment:
  *   AtomConv: rows = directed edges sorted by centre, segment = centre atom (ptr_c [N+1]), w = wag[d2u];
  *   BondConv: rows = angles sorted by bond slot i, segment = slot i (ptr_i [Es+1]), w = wbg[i] * wbg[j].
- * One warp-specialised tcgen05 kernel (csrc/gated_ws.cu): gather + add of the first-layer rows, the two 64x64
+ * One warp-specialised wgmma kernel (csrc/gated_ws.cu): gather + add of the first-layer rows, the two 64x64
  * second-layer products as 3xTF32 on the tensor cores, LayerNorm / SiLU x sigmoid, and the segmented sum inside the
  * CTA (the [rows][64] message never reaches HBM), followed by a small stitch kernel for segments that span
  * 16-row strips (fixed order: deterministic).  save_p / save_pre [rows][128] may be NULL (no reverse pass).

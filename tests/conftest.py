@@ -11,17 +11,17 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
     """`-m gpu` tests need a CUDA device: on a CPU-only host they are skipped, not failed (a plain
-    `pytest tests/` stays green here; the driver runs them on the B200 box)."""
+    `pytest tests/` stays green on a machine without a GPU)."""
     import torch
 
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="no CUDA device visible (GPU tests run on the B200 box)")
+    skip = pytest.mark.skip(reason="no CUDA device visible")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

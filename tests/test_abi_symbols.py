@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports exactly the symbols
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports exactly the symbols
 declared in include/chgnet_b200.h (no compute calls without a GPU)."""
 import os
 import re
@@ -71,12 +71,12 @@ def test_product_fails_loudly_without_cuda():
         model([])
 
 
-def test_sass_is_sm100a():
+def test_sass_is_sm90a():
     so = os.path.join(ROOT, "chgnet_b200", "libchgnet_b200.so")
     import subprocess
 
     out = subprocess.run(["cuobjdump", "-lelf", so], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
 
 
 def test_product_never_imports_oracle():

@@ -38,17 +38,18 @@ def recorded(weights030):
     return _record(weights030, graphs, need_grad=True, need_magmom=True, need_atom_fea=True, need_crystal_fea=True)
 
 
+# ids are the stable names of the implementation slots (option values); on sm_90a every tensor-core slot is a wgmma kernel
 @pytest.mark.parametrize("linear_impl,gated_impl", [(3, 3), (3, 0), (1, 0), (0, 1), (2, 2)],
                          ids=["defaults: linear=tcgen05-ws,gated=fused-tcgen05-ws", "linear=tcgen05-ws,gated=ffma4x8",
                               "linear=tcgen05,gated=ffma4x8", "linear=ffma,gated=tcgen05", "linear=tcgen05+tma,gated=ffma8x8"])
 def test_every_kernel_matches_its_spec(recorded, linear_impl, gated_impl):
-    """Both implementations of every entry point (tcgen05 3xTF32 and FFMA) against the spec."""
+    """Both implementations of every entry point (wgmma 3xTF32 and FFMA) against the spec."""
     from chgnet_b200._lib import CudaKernels
 
     K = CudaKernels()
     K.set_option("linear_impl", linear_impl)
     K.set_option("gated_impl", gated_impl)
-    K.set_option("ws_min_rows", 0)  # the recorded graphs are small: run the tcgen05 kernels on them anyway
+    K.set_option("ws_min_rows", 0)  # the recorded graphs are small: run the tensor-core kernels on them anyway
     try:
         seen = {}
         for name, snap, outs in recorded:
@@ -132,6 +133,7 @@ def test_loss_terms_and_adam_match_torch():
         assert float((p - ref.detach()).abs().max()) < 2e-6
 
 
+# ids are the stable names of the implementation slots (option values); on sm_90a every tensor-core slot is a wgmma kernel
 @pytest.mark.parametrize("impl", [3, 2, 1, 0], ids=["tcgen05-ws", "tcgen05+tma", "tcgen05", "ffma"])
 def test_linear_large_ragged_calls(impl):
     """chg_linear at the sizes where the tensor-core kernels are dispatched (m >= 4096): ragged
@@ -222,6 +224,7 @@ def test_bad_arguments_are_reported():
         K.linear(torch.zeros(4, 64), torch.zeros(64, 64), None, None, torch.zeros(4, 64))  # CPU tensors
 
 
+# ids are the stable names of the implementation slots (option values); on sm_90a every tensor-core slot is a wgmma kernel
 @pytest.mark.parametrize("wgrad_impl", [1, 0], ids=["tcgen05", "ffma"])
 def test_wgrad_large_reduction_matches_fp64(wgrad_impl):
     """chg_wgrad at the sizes where the tensor-core kernel (csrc/wgrad_tc.cu, 3xTF32) takes over (>= 4096 rows): plain,

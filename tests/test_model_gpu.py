@@ -47,6 +47,7 @@ def test_limno2_known_answers(model, limno2_graph, golden):
     print({k: f"{_maxabs(out[k], golden[f'limno2.oracle64.{k}']):.2e}" for k in TOL})
 
 
+# ids are the stable names of the implementation slots (option values); on sm_90a every tensor-core slot is a wgmma kernel
 @pytest.mark.parametrize("linear_impl,gated_impl", [(1, 1), (0, 0), (3, 3)], ids=["all-tcgen05", "all-ffma", "defaults"])
 def test_limno2_parity_for_every_implementation(model, limno2_graph, golden, linear_impl, gated_impl):
     from chgnet_b200._lib import CudaKernels
@@ -54,7 +55,7 @@ def test_limno2_parity_for_every_implementation(model, limno2_graph, golden, lin
     K = CudaKernels()
     K.set_option("linear_impl", linear_impl)
     K.set_option("gated_impl", gated_impl)
-    K.set_option("ws_min_rows", 0)  # 8-atom cell: force the tcgen05 kernels where gated_impl asks for them
+    K.set_option("ws_min_rows", 0)  # 8-atom cell: force the tensor-core kernels where gated_impl asks for them
     try:
         out = model.predict_graph(limno2_graph)
         for k, tol in TOL.items():
