@@ -61,6 +61,10 @@ SIGNATURES: dict[str, list] = {
     "chg_angle_update_tan": [P, P, P, P, P, P, P, I, P, P, P, P, P],
     "chg_angle_update_bwd2": [P, P, P, P, I, P, P, P, P],
     "chg_readout_bwd2": [P, P, I, P, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P],
+    # Hessian-vector products
+    "chg_bond_basis_hvp": [P, P, P, I, P, P, I, F, F, I, P, P, P, P, P, P],
+    "chg_angle_basis_hvp": [P, P, P, P, I, P, I, P, P, P, P],
+    "chg_edge_tangent_bwd": [P, P, P, P, P, P, P, P, P, P, I, P, P],
 }
 
 _lib = None
@@ -329,6 +333,22 @@ class CudaKernels:
         self._chk(rhat, drhat, ang_di, ang_dj, freq, w, lam_a0, g_freq)
         self._call("chg_angle_basis_bwd2", _p(rhat), _p(drhat), _p(ang_di), _p(ang_dj), ang_di.shape[0], _p(freq),
                    freq.shape[0], _p(w), _p(lam_a0), _p(g_freq))
+
+    def bond_basis_hvp(self, dist, ddist, u2d, freq_ag, freq_bg, rc_ag, rc_bg, p, w3, lam_e0, lam_wag, lam_wbg, g_dist):
+        self._chk(dist, ddist, u2d, freq_ag, freq_bg, w3, lam_e0, lam_wag, lam_wbg, g_dist)
+        self._call("chg_bond_basis_hvp", _p(dist), _p(ddist), _p(u2d), u2d.shape[0], _p(freq_ag), _p(freq_bg),
+                   freq_ag.shape[0], float(rc_ag), float(rc_bg), int(p), _p(w3), _p(lam_e0), _p(lam_wag), _p(lam_wbg),
+                   _p(g_dist))
+
+    def angle_basis_hvp(self, rhat, drhat, ang_di, ang_dj, freq, w, lam_a0, g_rhat):
+        self._chk(rhat, drhat, ang_di, ang_dj, freq, w, lam_a0, g_rhat)
+        self._call("chg_angle_basis_hvp", _p(rhat), _p(drhat), _p(ang_di), _p(ang_dj), ang_di.shape[0], _p(freq),
+                   freq.shape[0], _p(w), _p(lam_a0), _p(g_rhat))
+
+    def edge_tangent_bwd(self, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, force):
+        self._chk(dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, force)
+        self._call("chg_edge_tangent_bwd", _p(dist), _p(rhat), _p(ddist), _p(drhat), _p(lam_dist), _p(lam_rhat), _p(d2u),
+                   _p(u2d), _p(center), _p(nbr), center.shape[0], _p(force))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

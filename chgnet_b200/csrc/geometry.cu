@@ -483,14 +483,45 @@ bond_basis_tangent_kernel(const float* __restrict__ dist, const float* __restric
   }
 }
 
-// g_freq += d/dfreq < lam, (dB/dd ddist) W >
+// d^2 envelope / dd^2 (basis.py:184-205 differentiated twice)
+__device__ __forceinline__ float envelope_d2(float d, float rc, int p) {
+  const float x = d / rc;
+  if (p == 0 || !(x < 1.f)) return 0.f;
+  const float pf = (float)p;
+  const float a = -(pf + 1.f) * (pf + 2.f) * 0.5f, b = pf * (pf + 2.f), c = -pf * (pf + 1.f) * 0.5f;
+  float xpm1 = 1.f;  // x^(p-1)
+  for (int i = 0; i < p - 1; ++i) xpm1 *= x;
+  float t0 = 0.f;  // a p (p-1) x^(p-2)
+  if (p >= 2) {
+    float xpm2 = 1.f;
+    for (int i = 0; i < p - 2; ++i) xpm2 *= x;
+    t0 = a * pf * (pf - 1.f) * xpm2;
+  }
+  return (t0 + xpm1 * (b * (pf + 1.f) * pf + x * c * (pf + 2.f) * (pf + 1.f))) / (rc * rc);
+}
+
+// d^2 basis / dd^2 of the basis function of frequency f:  raw'' env + 2 raw' env' + raw env''
+__device__ __forceinline__ float rbf_d2(float d, float f, float rc, int p) {
+  const Envelope e = envelope(d, rc, p);
+  const float nrm = sqrtf(2.f / rc), k = f / rc;
+  float sn, cs;
+  sincosf(f * (d / rc), &sn, &cs);
+  const float raw = nrm * sn / d;
+  const float draw = nrm * (k * cs / d - sn / (d * d));
+  const float d2raw = nrm * (-k * k * sn / d - 2.f * k * cs / (d * d) + 2.f * sn / (d * d * d));
+  return d2raw * e.env + 2.f * draw * e.denv + raw * envelope_d2(d, rc, p);
+}
+
+// kGeom = false: g_freq += d/dfreq < lam, (dB/dd ddist) W >          (force / stress loss)
+// kGeom = true : g_dist[u] += < lam W^T, d^2B/dd^2 > ddist             (Hessian-vector product)
+template <bool kGeom>
 __global__ void __launch_bounds__(256)
 bond_basis_bwd2_kernel(const float* __restrict__ dist, const float* __restrict__ ddist,
                        const int32_t* __restrict__ u2d, int n_bonds, const float* __restrict__ freq_ag,
                        const float* __restrict__ freq_bg, int R, float rc_ag, float rc_bg, int p,
                        const float* __restrict__ w3, const float* __restrict__ lam_e0,
                        const float* __restrict__ lam_wag, const float* __restrict__ lam_wbg,
-                       double* __restrict__ g_freq) {
+                       double* __restrict__ g_freq, float* __restrict__ g_dist) {
   extern __shared__ __align__(16) float s_w[];  // [3][64][R]
   for (int i = threadIdx.x; i < 3 * R * 64; i += blockDim.x) s_w[i] = w3[i];
   __syncthreads();
@@ -516,7 +547,16 @@ bond_basis_bwd2_kernel(const float* __restrict__ dist, const float* __restrict__
       gb_bg = fmaf(__shfl_sync(0xffffffffu, c0, n), s_w[(128 + n) * R + kl], gb_bg);
       gb_bg = fmaf(__shfl_sync(0xffffffffu, c1, n), s_w[(128 + n + 32) * R + kl], gb_bg);
     }
-    if (lane < R) {
+    if constexpr (kGeom) {
+      float src = 0.f;
+      if (lane < R) {
+        src = gb_ag * rbf_d2(d, f_ag, rc_ag, p);
+        const Envelope eb = envelope(d, rc_bg, p);
+        if (eb.env != 0.f || eb.denv != 0.f || !(d == d)) src = fmaf(gb_bg, rbf_d2(d, f_bg, rc_bg, p), src);
+      }
+      src = sum32(src);
+      if (lane == 0) g_dist[u] += src * dd;  // one warp per bond: no other writer
+    } else if (lane < R) {
       // d/dw of  nrm [ (w/rc) cos(w x)/d - sin(w x)/d^2 ] env + nrm sin(w x)/d env' ,  x = d/rc
       const Envelope ea = envelope(d, rc_ag, p), eb = envelope(d, rc_bg, p);
       float sn, cs;
@@ -534,7 +574,7 @@ bond_basis_bwd2_kernel(const float* __restrict__ dist, const float* __restrict__
       }
     }
   }
-  if (lane < R) {
+  if (!kGeom && lane < R) {
     atomicAdd(g_freq + lane, gf_ag);
     atomicAdd(g_freq + R + lane, gf_bg);
   }
@@ -589,12 +629,46 @@ angle_basis_tangent_kernel(const float* __restrict__ rhat, const float* __restri
   }
 }
 
-// g_freq += d/dfreq < lam_a0, (dF/dtheta thetadot) W >
+// theta, its tangent, and what the geometry derivative of the tangent needs, with 1 - u^2 formed as
+// (1 - c^2) + c^2 |rhat_i x rhat_j|^2: at an exactly collinear pair 1 - u^2 ~ 2e-6, and 1 - u*u in fp32
+// would lose ~3 % of it to cancellation (d^2 theta carries its -3/2 power)
+struct ThetaGeom {
+  float ri[3], rj[3], dri[3], drj[3];
+  float u, ud, th, th_u;  // u = c rhat_i . rhat_j, ud its tangent, th_u = d theta / du
+};
+__device__ __forceinline__ ThetaGeom theta_geom(const float* __restrict__ rhat, const float* __restrict__ drhat,
+                                                int di, int dj) {
+  ThetaGeom g;
+  g.u = angle_cos(rhat, di, dj, g.ri, g.rj);
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    g.dri[j] = drhat[(size_t)di * 3 + j];
+    g.drj[j] = drhat[(size_t)dj * 3 + j];
+  }
+  constexpr float c = 1.f - 1e-6f;
+  const float x0 = g.ri[1] * g.rj[2] - g.ri[2] * g.rj[1], x1 = g.ri[2] * g.rj[0] - g.ri[0] * g.rj[2],
+              x2 = g.ri[0] * g.rj[1] - g.ri[1] * g.rj[0];
+  const float one_m_c2 = 1e-6f * (2.f - 1e-6f);
+  const float q = fmaf(c * c, fmaf(x2, x2, fmaf(x1, x1, x0 * x0)), one_m_c2);
+  float ud = 0.f;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) ud = fmaf(g.dri[j], g.rj[j], fmaf(g.ri[j], g.drj[j], ud));
+  g.ud = ud * c;
+  g.th = acosf(g.u);
+  g.th_u = -rsqrtf(q);
+  return g;
+}
+
+__device__ __forceinline__ float pick3(const float (&v)[3], int k) { return k == 0 ? v[0] : (k == 1 ? v[1] : v[2]); }
+
+// kGeom = false: g_freq += d/dfreq < lam_a0, (dF/dtheta thetadot) W >                     (force / stress loss)
+// kGeom = true : g_rhat += d/d(rhat_i, rhat_j) < lam_a0, (dF/dtheta thetadot) W >, drhat fixed (Hessian-vector)
+template <bool kGeom>
 __global__ void __launch_bounds__(256)
 angle_basis_bwd2_kernel(const float* __restrict__ rhat, const float* __restrict__ drhat,
                         const int32_t* __restrict__ ang_di, const int32_t* __restrict__ ang_dj, int n_angles,
                         const float* __restrict__ freq, int nf, const float* __restrict__ w,
-                        const float* __restrict__ lam_a0, double* __restrict__ g_freq) {
+                        const float* __restrict__ lam_a0, double* __restrict__ g_freq, double* __restrict__ g_rhat) {
   extern __shared__ __align__(16) float s_w[];  // [64][2nf+1]
   const int nb = 2 * nf + 1;
   for (int i = threadIdx.x; i < nb * 64; i += blockDim.x) s_w[i] = w[i];
@@ -609,7 +683,14 @@ angle_basis_bwd2_kernel(const float* __restrict__ rhat, const float* __restrict_
   double gfr = 0.0;
   for (int a = warp; a < n_angles; a += n_warps) {
     float th, thd;
-    theta_dot(rhat, drhat, ang_di[a], ang_dj[a], th, thd);
+    ThetaGeom tg;
+    if constexpr (kGeom) {
+      tg = theta_geom(rhat, drhat, ang_di[a], ang_dj[a]);
+      th = tg.th;
+      thd = tg.th_u * tg.ud;
+    } else {
+      theta_dot(rhat, drhat, ang_di[a], ang_dj[a], th, thd);
+    }
     const float ga = lam_a0[(size_t)a * 64 + lane], gb = lam_a0[(size_t)a * 64 + lane + 32];
     float gf = 0.f;
     for (int n = 0; n < 32; ++n) {
@@ -619,12 +700,70 @@ angle_basis_bwd2_kernel(const float* __restrict__ rhat, const float* __restrict_
     float sn, cs;
     const float arg = wf * th;
     sincosf(arg, &sn, &cs);
-    // d/dw [ w cos(w th) ] = cos - w th sin ;  d/dw [ -w sin(w th) ] = -(sin + w th cos)
-    if (is_sin) gfr += (double)(gf * (cs - arg * sn) * thd * inv_sqrt_pi);
-    else if (is_cos) gfr -= (double)(gf * (sn + arg * cs) * thd * inv_sqrt_pi);
+    if constexpr (kGeom) {
+      // f1 = < gf, dF/dtheta >, f2 = < gf, d^2F/dtheta^2 >;  theta(u), u = c rhat_i . rhat_j:
+      // d/drhat_i [ F' thetadot ] = c (f2 thetadot th_u + f1 th_uu ud) rhat_j + c f1 th_u drhat_j   (i <-> j)
+      float f1 = 0.f, f2 = 0.f;
+      if (is_sin) {
+        f1 = gf * wf * cs;
+        f2 = -gf * wf * wf * sn;
+      } else if (is_cos) {
+        f1 = -gf * wf * sn;
+        f2 = -gf * wf * wf * cs;
+      }
+      f1 = sum32(f1) * inv_sqrt_pi;
+      f2 = sum32(f2) * inv_sqrt_pi;
+      constexpr float c = 1.f - 1e-6f;
+      const float th_uu = tg.th_u * tg.th_u * tg.th_u * tg.u;  // -u / (1 - u^2)^(3/2)
+      const float k_r = c * fmaf(f2 * thd, tg.th_u, f1 * th_uu * tg.ud), k_d = c * f1 * tg.th_u;
+      if (lane < 3) {
+        atomicAdd(g_rhat + (size_t)ang_di[a] * 3 + lane, (double)fmaf(k_r, pick3(tg.rj, lane), k_d * pick3(tg.drj, lane)));
+      } else if (lane < 6) {
+        const int k = lane - 3;
+        atomicAdd(g_rhat + (size_t)ang_dj[a] * 3 + k, (double)fmaf(k_r, pick3(tg.ri, k), k_d * pick3(tg.dri, k)));
+      }
+    } else {
+      // d/dw [ w cos(w th) ] = cos - w th sin ;  d/dw [ -w sin(w th) ] = -(sin + w th cos)
+      if (is_sin) gfr += (double)(gf * (cs - arg * sn) * thd * inv_sqrt_pi);
+      else if (is_cos) gfr -= (double)(gf * (sn + arg * cs) * thd * inv_sqrt_pi);
+    }
   }
-  if (is_sin) atomicAdd(g_freq + lane - 1, gfr);
-  else if (is_cos) atomicAdd(g_freq + lane - 1 - nf, gfr);
+  if constexpr (!kGeom) {
+    if (is_sin) atomicAdd(g_freq + lane - 1, gfr);
+    else if (is_cos) atomicAdd(g_freq + lane - 1 - nf, gfr);
+  }
+}
+
+// d/dr_e of  lam_d ddist + lam_rhat . drhat  with rdot held fixed (Hessian-vector products), scattered like
+// force_virial (force[c] -= g, force[n] += g).  ddist = rhat . rdot -> drhat;  drhat = (rdot - rhat ddist)/d ->
+// -[(mu . drhat) rhat + (mu . rhat) drhat + ddist (mu - rhat (rhat . mu))/d]/d,  mu = lam_rhat.  lam_d belongs to
+// the bond's representative edge only (the bond basis reads d there).
+__global__ void edge_tangent_bwd_kernel(const float* __restrict__ dist, const float* __restrict__ rhat,
+                                        const float* __restrict__ ddist, const float* __restrict__ drhat,
+                                        const float* __restrict__ lam_dist, const double* __restrict__ lam_rhat,
+                                        const int32_t* __restrict__ d2u, const int32_t* __restrict__ u2d,
+                                        const int32_t* __restrict__ center, const int32_t* __restrict__ nbr,
+                                        int n_edges, double* __restrict__ force) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_edges) return;
+  const int c = center[e], n = nbr[e], u = d2u[e];
+  double rh[3], rd[3], mu[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    rh[j] = (double)rhat[(size_t)e * 3 + j];
+    rd[j] = (double)drhat[(size_t)e * 3 + j];
+    mu[j] = lam_rhat[(size_t)e * 3 + j];
+  }
+  const double inv_d = 1.0 / (double)dist[e], dd = (double)ddist[e];
+  const double ld = (u2d[u] == e) ? (double)lam_dist[u] : 0.0;
+  const double m_rd = mu[0] * rd[0] + mu[1] * rd[1] + mu[2] * rd[2];
+  const double m_rh = mu[0] * rh[0] + mu[1] * rh[1] + mu[2] * rh[2];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const double g = ld * rd[j] - (m_rd * rh[j] + m_rh * rd[j] + dd * (mu[j] - rh[j] * m_rh) * inv_d) * inv_d;
+    atomicAdd(force + (size_t)c * 3 + j, -g);
+    atomicAdd(force + (size_t)n * 3 + j, g);
+  }
 }
 
 // ---- magmom head -------------------------------------------------------------------
@@ -844,8 +983,24 @@ extern "C" int chg_bond_basis_bwd2(const float* dist, const float* ddist, const 
   if (n_bonds == 0) return CHG_OK;
   CHG_CHECK_ARG(dist && ddist && u2d && freq_ag && freq_bg && w3 && lam_e0 && lam_wag && lam_wbg && g_freq, "null pointer");
   const int smem = 3 * n_radial * 64 * 4;
-  bond_basis_bwd2_kernel<<<warp_grid(n_bonds), 256, smem, as_stream(stream)>>>(
-      dist, ddist, u2d, n_bonds, freq_ag, freq_bg, n_radial, rc_ag, rc_bg, p, w3, lam_e0, lam_wag, lam_wbg, g_freq);
+  bond_basis_bwd2_kernel<false><<<warp_grid(n_bonds), 256, smem, as_stream(stream)>>>(
+      dist, ddist, u2d, n_bonds, freq_ag, freq_bg, n_radial, rc_ag, rc_bg, p, w3, lam_e0, lam_wag, lam_wbg, g_freq,
+      nullptr);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_bond_basis_hvp(const float* dist, const float* ddist, const int32_t* u2d, int32_t n_bonds,
+                                  const float* freq_ag, const float* freq_bg, int32_t n_radial, float rc_ag,
+                                  float rc_bg, int32_t p, const float* w3, const float* lam_e0, const float* lam_wag,
+                                  const float* lam_wbg, float* g_dist, void* stream) {
+  CHG_CHECK_ARG(n_bonds >= 0, "negative size");
+  CHG_CHECK_ARG(n_radial >= 1 && n_radial <= MAX_BASIS, "num_radial must be in [1, 32]");
+  if (n_bonds == 0) return CHG_OK;
+  CHG_CHECK_ARG(dist && ddist && u2d && freq_ag && freq_bg && w3 && lam_e0 && lam_wag && lam_wbg && g_dist, "null pointer");
+  const int smem = 3 * n_radial * 64 * 4;
+  bond_basis_bwd2_kernel<true><<<warp_grid(n_bonds), 256, smem, as_stream(stream)>>>(
+      dist, ddist, u2d, n_bonds, freq_ag, freq_bg, n_radial, rc_ag, rc_bg, p, w3, lam_e0, lam_wag, lam_wbg, nullptr,
+      g_dist);
   CHG_LAUNCH_END();
 }
 
@@ -870,7 +1025,33 @@ extern "C" int chg_angle_basis_bwd2(const float* rhat, const float* drhat, const
   if (n_angles == 0) return CHG_OK;
   CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && freq && w && lam_a0 && g_freq, "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
-  angle_basis_bwd2_kernel<<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(rhat, drhat, ang_di, ang_dj, n_angles,
-                                                                                freq, n_freq, w, lam_a0, g_freq);
+  angle_basis_bwd2_kernel<false><<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(
+      rhat, drhat, ang_di, ang_dj, n_angles, freq, n_freq, w, lam_a0, g_freq, nullptr);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_angle_basis_hvp(const float* rhat, const float* drhat, const int32_t* ang_di, const int32_t* ang_dj,
+                                   int32_t n_angles, const float* freq, int32_t n_freq, const float* w,
+                                   const float* lam_a0, double* g_rhat, void* stream) {
+  CHG_CHECK_ARG(n_angles >= 0, "negative size");
+  CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
+  if (n_angles == 0) return CHG_OK;
+  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && freq && w && lam_a0 && g_rhat, "null pointer");
+  const int smem = (2 * n_freq + 1) * 64 * 4;
+  angle_basis_bwd2_kernel<true><<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(
+      rhat, drhat, ang_di, ang_dj, n_angles, freq, n_freq, w, lam_a0, nullptr, g_rhat);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_edge_tangent_bwd(const float* dist, const float* rhat, const float* ddist, const float* drhat,
+                                    const float* lam_dist, const double* lam_rhat, const int32_t* d2u,
+                                    const int32_t* u2d, const int32_t* center, const int32_t* nbr, int32_t n_edges,
+                                    double* force, void* stream) {
+  CHG_CHECK_ARG(n_edges >= 0, "negative size");
+  if (n_edges == 0) return CHG_OK;
+  CHG_CHECK_ARG(dist && rhat && ddist && drhat && lam_dist && lam_rhat && d2u && u2d && center && nbr && force,
+                "null pointer");
+  edge_tangent_bwd_kernel<<<(n_edges + 255) / 256, 256, 0, as_stream(stream)>>>(
+      dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, n_edges, force);
   CHG_LAUNCH_END();
 }

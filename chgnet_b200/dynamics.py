@@ -142,6 +142,13 @@ class CHGNetCalculator(_Base):
         if self.return_site_energies:
             self.results["energies"] = pred["site_energies"]
 
+    def get_hessian(self, atoms=None):
+        """``[3N,3N]`` Hessian d^2E/dx dx of the total energy at fixed cell, in eV/A^2 (``CHGNet.predict_hessian``)."""
+        atoms = atoms if atoms is not None else self.atoms
+        cell = np.asarray(atoms.get_cell(), dtype=np.float64).reshape(3, 3)
+        frac = np.asarray(atoms.get_positions(), dtype=np.float64) @ np.linalg.inv(cell)
+        return self.model.predict_hessian((np.asarray(atoms.get_atomic_numbers()), frac, cell))
+
 
 class VelocityVerlet:
     """NVE molecular dynamics on the host (the integrator of ase.md.verlet restated): one calculator

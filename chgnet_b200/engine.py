@@ -264,8 +264,18 @@ class Engine:
         self._reverse(st, out, dict(seed_energy=seed_energy, seed_magmom=seed_magmom, grads=grads))
         return grads
 
+    def hessian_vector_products(self, b: DeviceBatch, directions: Tensor) -> Tensor:
+        """H v per atom, ``[N,3]`` fp64, H = d^2E/dx dx of the extensive model energy of each graph (cell fixed,
+        x Cartesian positions), v = ``directions`` ``[N,3]``.  A batch of K copies of one graph with a different
+        direction on each copy gives K products of that graph's Hessian in one call."""
+        out = self.run(b, need_grad=True, train=True)
+        self.input_grads(out, record=True)
+        st = out.extras.pop("train_state")
+        return self._second_order(st, dict(seed_energy=self._zeros(b, b.n_graphs, dtype=torch.float64), seed_magmom=None,
+                                           seed_force=None, seed_stress=None, grads=None, directions=directions))
+
     # ------------------------------------------------------------------ second order
-    def _second_order(self, st: dict, train: dict) -> None:
+    def _second_order(self, st: dict, train: dict) -> Tensor | None:
         """Parameter gradients of a loss that also depends on forces and stresses (reference
         model.py:518-535 ``create_graph=True`` + trainer.py:409 ``loss.backward()``).
 
@@ -276,6 +286,10 @@ class Engine:
         tangent quantity equals the ordinary adjoint lambda = dE/d(.) recorded by the force pass, so this
         reverse pass only propagates the adjoints of the PRIMAL intermediates ("bar"), seeded with the
         energy / magmom loss, and adds the second-order source terms inside the nonlinear kernels.
+
+        Hessian-vector mode (``train["grads"] is None``, ``train["directions"]`` = v per atom, zero energy seed):
+        rdot_e = v[c] - v[n], so T = <dE/dx, v>, and dT/dx = H v.  No parameter gradient is formed; the tail
+        differentiates T with respect to the geometry instead (:meth:`_geometry_tail`) and returns H v.
         """
         pw, K, hp = self.pw, self.K, self.pw.hp
         b: DeviceBatch = st["b"]
@@ -290,7 +304,7 @@ class Engine:
         use_ln = pw.atom[0].ln is not None
 
         def ln_acc():
-            return self._zeros(b, 256, dtype=torch.float64) if use_ln else None
+            return self._zeros(b, 256, dtype=torch.float64) if (G is not None and use_ln) else None
 
         def lin(x, wt, residual=None, x_rows=None):
             return self._lin(b, x, wt, None, residual, x_rows)
@@ -300,7 +314,12 @@ class Engine:
             return self._wgrad(b, x, g, n, **kw) + self._wgrad(b, xd, lam, n, **kw)
 
         # ---------------- tangent pass ----------------
-        u_atom = self._zeros(b, N, 3) if train["seed_force"] is None else (-train["seed_force"]).to(dt).contiguous()
+        if train.get("directions") is not None:
+            u_atom = train["directions"].to(dt).contiguous()
+        elif train["seed_force"] is not None:
+            u_atom = (-train["seed_force"]).to(dt).contiguous()
+        else:
+            u_atom = self._zeros(b, N, 3)
         w_graph = self._zeros(b, B, 9)
         if train["seed_stress"] is not None:
             scale = (EV_A3_TO_GPA / b.volume.to(torch.float64))[:, None, None]
@@ -362,13 +381,14 @@ class Engine:
         g_h0, hbar0, xhat, xhatd = (self._new(b, N, 64) for _ in range(4))
         K.readout_bwd2(st["x_last"], x_d, pw.readout_ln, pw.mlp_wt, pw.mlp_w, pw.mlp_b, pw.w_last, seed_atom, bar_x,
                        h_all, hd_all, gz_all, zbar_all, g_h0, hbar0, xhat, xhatd)
-        G["mlp_wt"] = torch.stack([wsum(h_all[l], zbar_all[l], 64, hd_all[l], gz_all[l]) for l in range(L)])
-        G["mlp_b"] = torch.stack([self._colsum(b, zbar_all[l]) for l in range(L)])
-        G["w_last"] = self._colsum(b, h_all[L], rowscale=seed_atom) + self._colsum(b, hd_all[L])
-        G["b_last"] = seed_atom.sum()
-        if pw.readout_ln is not None:
-            G["readout_ln"] = torch.stack([self._colsum(b, hbar0, xhat) + self._colsum(b, g_h0, xhatd),
-                                           self._colsum(b, hbar0)])
+        if G is not None:
+            G["mlp_wt"] = torch.stack([wsum(h_all[l], zbar_all[l], 64, hd_all[l], gz_all[l]) for l in range(L)])
+            G["mlp_b"] = torch.stack([self._colsum(b, zbar_all[l]) for l in range(L)])
+            G["w_last"] = self._colsum(b, h_all[L], rowscale=seed_atom) + self._colsum(b, hd_all[L])
+            G["b_last"] = seed_atom.sum()
+            if pw.readout_ln is not None:
+                G["readout_ln"] = torch.stack([self._colsum(b, hbar0, xhat) + self._colsum(b, g_h0, xhatd),
+                                               self._colsum(b, hbar0)])
 
         bar_e = None
         bar_wag = self._zeros(b, Eu, 64)
@@ -379,6 +399,8 @@ class Engine:
             return self._lin(b, x_in, wt, residual=dst)
 
         def w2_grads(key, pre, u, pre_d, g_p_lam, g_ln):
+            if G is None:
+                return
             w2t, b2, tmp = self._new(b, 64, 128), self._new(b, 128), self._new(b, 64, 128)
             for h in (slice(0, 64), slice(64, 128)):
                 K.wgrad(pre[:, h], u[:, h], w2t[:, h], b2[h], None, None, True)       # silu(pre)^T u
@@ -389,9 +411,10 @@ class Engine:
 
         def atom_bwd2(t, bar_xout, bar_e):
             gp, sv, la, tt = pw.atom[t], saved_atom[t], rec["atom"][t], t_atom[t]
-            G[f"atom.{t}.wo_t"] = wsum(sv["agg"], bar_xout, 64, tt["agg_d"], la["g_xout"])
-            if gp.extra["bo"] is not None:
-                G[f"atom.{t}.bo"] = self._colsum(b, bar_xout)
+            if G is not None:
+                G[f"atom.{t}.wo_t"] = wsum(sv["agg"], bar_xout, 64, tt["agg_d"], la["g_xout"])
+                if gp.extra["bo"] is not None:
+                    G[f"atom.{t}.bo"] = self._colsum(b, bar_xout)
             bar_agg = self._lin(b, bar_xout, gp.extra["wo"])
             bar_pre, bar_w, u, g_ln = self._new(b, Ed, 128), self._new(b, Ed, 64), self._new(b, Ed, 128), ln_acc()
             K.atom_conv_bwd2(sv["pre"], sv["p"], tt["pre_d"], tt["p_d"], la["g_p"], wag, wag_d, b.center, b.d2u,
@@ -401,9 +424,10 @@ class Engine:
             K.segment_sum(bar_pre, None, b.ptr_c, 0, sp[:, :128])
             K.segment_sum(bar_pre, b.perm_n, b.ptr_n, 0, sp[:, 128:])
             spe = self._seg(b, bar_pre, b.perm_u, b.ptr_u, Eu)
-            G[f"atom.{t}.wcn_t"] = wsum(sv["x"], sp, 256, tt["x_d"], la["sp"])
-            we_bar, G[f"atom.{t}.b1"] = self._wgrad(b, sv["e"], spe, 128, colsum=True)
-            G[f"atom.{t}.we_t"] = we_bar + self._wgrad(b, tt["e_d"], la["spe"], 128)
+            if G is not None:
+                G[f"atom.{t}.wcn_t"] = wsum(sv["x"], sp, 256, tt["x_d"], la["sp"])
+                we_bar, G[f"atom.{t}.b1"] = self._wgrad(b, sv["e"], spe, 128, colsum=True)
+                G[f"atom.{t}.we_t"] = we_bar + self._wgrad(b, tt["e_d"], la["spe"], 128)
             K.segment_sum(bar_w, b.perm_u, b.ptr_u, 1, bar_wag)
             return acc(bar_xout, sp, gp.extra["wcn_b"]), acc(bar_e, spe, gp.extra["we_b"])
 
@@ -415,10 +439,11 @@ class Engine:
                 bar_e = self._zeros(b, Eu, 64)
             K.linear(sp, ex["wij_b"], None, bar_e, bar_e, None, sid)
             spx = self._seg(b, bar_pre, b.perm_x, b.ptr_x, N)
-            G[f"{key}.wij_t"] = wsum(sv["e"], sp, 256, tt["e_d"], la["sp"], x_rows=sid)
-            G[f"{key}.wx_t"] = wsum(sv["x"], spx, 128, tt["x_d"], la["spx"])
-            w1a_bar, G[f"{key}.b1"] = self._wgrad(b, sv["ang"], bar_pre, 128, colsum=True)
-            G[f"{key}.w1a_t"] = w1a_bar + self._wgrad(b, tt["ang_d"], la["g_pre"], 128)
+            if G is not None:
+                G[f"{key}.wij_t"] = wsum(sv["e"], sp, 256, tt["e_d"], la["sp"], x_rows=sid)
+                G[f"{key}.wx_t"] = wsum(sv["x"], spx, 128, tt["x_d"], la["spx"])
+                w1a_bar, G[f"{key}.b1"] = self._wgrad(b, sv["ang"], bar_pre, 128, colsum=True)
+                G[f"{key}.w1a_t"] = w1a_bar + self._wgrad(b, tt["ang_d"], la["g_pre"], 128)
             return acc(bar_x, spx, ex["wx_b"]), bar_e
 
         bar_x, bar_e = atom_bwd2(n_conv - 1, bar_x, None)
@@ -440,10 +465,11 @@ class Engine:
                 gp, sv, la, tt = pw.bond[t], saved_bond[t], rec["bond"][t], t_bond[t]
                 if bar_e is None:
                     bar_e = self._zeros(b, Eu, 64)
-                G[f"bond.{t}.wo_t"] = (self._wgrad(b, sv["agg"], bar_e, 64, g_rows=sid)
-                                       + self._wgrad(b, tt["agg_d"], la["g_eout"], 64, g_rows=sid))
-                if gp.extra["bo"] is not None:
-                    G[f"bond.{t}.bo"] = self._colsum(b, bar_e)
+                if G is not None:
+                    G[f"bond.{t}.wo_t"] = (self._wgrad(b, sv["agg"], bar_e, 64, g_rows=sid)
+                                           + self._wgrad(b, tt["agg_d"], la["g_eout"], 64, g_rows=sid))
+                    if gp.extra["bo"] is not None:
+                        G[f"bond.{t}.bo"] = self._colsum(b, bar_e)
                 bar_agg = self._lin(b, bar_e, gp.extra["wo"], x_rows=sid)
                 bar_pre, u, g_ln = self._new(b, A, 128), self._new(b, A, 128), ln_acc()
                 bw_i, bw_j = self._new(b, A, 64), self._new(b, A, 64)
@@ -456,11 +482,14 @@ class Engine:
                 K.segment_sum(bw_j, b.perm_js, b.ptr_js, 1, bar_wbg)
             bar_x, bar_e = atom_bwd2(t, bar_x, bar_e)
 
-        # ---------------- embeddings, basis weights, basis frequencies ----------------
-        R, NA = pw.freq_ag.shape[0], pw.wang.shape[1]
         bar_wbg_full = self._zeros(b, Eu, 64)
         if has_ang:
             K.scatter_rows(bar_wbg, sid, bar_wbg_full)
+        if G is None:
+            return self._geometry_tail(st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a)
+
+        # ---------------- embeddings, basis weights, basis frequencies ----------------
+        R, NA = pw.freq_ag.shape[0], pw.wang.shape[1]
         order = torch.argsort(b.z.long(), stable=True).int()
         zptr = torch.zeros(95, dtype=torch.int32, device=b.z.device)
         zptr[1:] = torch.cumsum(torch.bincount(b.z.long() - 1, minlength=94), 0)
@@ -481,6 +510,30 @@ class Engine:
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, bar_a, None, g_fa)
             K.angle_basis_bwd2(rhat, drhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, rec["g_a0"], g_fa)
             G["freq_ang"] = g_fa.to(dt)
+
+    def _geometry_tail(self, st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a) -> Tensor:
+        """dT/dx (= H v) from the basis-level adjoints of the second reverse pass.  Per directed edge, dT/dr_e is
+        (a) the first-order geometry reverse fed with the bar adjoints, (b) lambda . d^2B/dd^2 ddist per bond,
+        (c) lambda_a0 . d^2 Fourier(theta) along (drhat_i, drhat_j), and (d) the derivative of the tangent map
+        (ddist, drhat)(r_e) with rdot fixed, weighted by the recorded lambda_d, lambda_rhat.  (a)-(c) meet in one
+        (g_dist, g_rhat) pair that chg_force_virial turns into -dT/dx; (d) accumulates there too."""
+        pw, K, hp = self.pw, self.K, self.pw.hp
+        b: DeviceBatch = st["b"]
+        rec, dist, rvec, rhat = st["rec"], st["dist"], st["rvec"], st["rhat"]
+        g_dist = self._new(b, b.n_bonds)
+        K.bond_basis_bwd(dist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
+                         hp.cutoff_coeff, pw.w3, bar_e, bar_wag, bar_wbg_full, g_dist)
+        K.bond_basis_hvp(dist, ddist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
+                         hp.cutoff_coeff, pw.w3, rec["g_e0"], rec["g_wag"], rec["g_wbg_full"], g_dist)
+        g_rhat = self._zeros(b, b.n_edges, 3, dtype=torch.float64)
+        if b.n_angles > 0:
+            K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, bar_a, g_rhat)
+            K.angle_basis_hvp(rhat, drhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, rec["g_a0"], g_rhat)
+        neg_hv = self._zeros(b, b.n_atoms, 3, dtype=torch.float64)
+        K.force_virial(rvec, dist, rhat, g_rhat, g_dist, b.d2u, b.u2d, b.center, b.nbr, b.owner, neg_hv,
+                       self._zeros(b, b.n_graphs, 9, dtype=torch.float64))
+        K.edge_tangent_bwd(dist, rhat, ddist, drhat, rec["g_dist"], rec["g_rhat"], b.d2u, b.u2d, b.center, b.nbr, neg_hv)
+        return neg_hv.neg_()
 
     def _wgrad(self, b, x, g, n, *, x_rows=None, g_rows=None, x_silu=False, colsum=False):
         out = self._new(b, 64, n)
@@ -677,6 +730,8 @@ class Engine:
         g_rhat = self._zeros(b, Ed, 3, dtype=torch.float64)
         if has_ang:
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, g_a, g_rhat)
+        if rec is not None:  # adjoints of the tangent inputs ddist, drhat (Hessian-vector products)
+            rec.update(g_dist=g_dist, g_rhat=g_rhat)
         force = self._zeros(b, N, 3, dtype=torch.float64)
         virial = self._zeros(b, B, 9, dtype=torch.float64)
         K.force_virial(rvec, dist, rhat, g_rhat, g_dist, b.d2u, b.u2d, b.center, b.nbr, b.owner, force, virial)

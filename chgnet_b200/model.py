@@ -748,6 +748,61 @@ class CHGNet(nn.Module):
                     predictions[start + i][key] = np.asarray(part)
         return predictions[0] if single else predictions
 
+    def _hessian_graph(self, structure_or_graph):
+        if is_graph_like(structure_or_graph):
+            return structure_or_graph
+        if self.graph_converter is None:
+            raise ValueError("graph_converter cannot be None!")
+        return self.graph_converter(structure_or_graph)
+
+    def _hvp_replicas(self, graph, v: np.ndarray, batch_size: int) -> np.ndarray:
+        """H v for K directions ``v [K,N,3]``: batches of up to ``batch_size`` copies of the graph, one direction per copy
+        (Engine.hessian_vector_products)."""
+        if batch_size < 1:
+            raise ValueError(f"{batch_size=} must be >= 1")
+        engine = self._get_engine()
+        compact = not self._arch.get("mlp_out_bias", False)
+        n_dirs, n = v.shape[0], v.shape[1]
+        out = np.empty((n_dirs, n, 3), dtype=np.float64)
+        batches: dict[int, DeviceBatch] = {}
+        for s in range(0, n_dirs, batch_size):
+            k = min(batch_size, n_dirs - s)
+            if k not in batches:  # the graph is fixed: one device batch per replica count
+                batches[k] = build_batch([graph] * k, self.device, with_reverse=True, compact_bonds=compact)
+            d = torch.as_tensor(v[s : s + k].reshape(k * n, 3), dtype=torch.float32).to(self.device)
+            out[s : s + k] = engine.hessian_vector_products(batches[k], d).view(k, n, 3).cpu().numpy()
+        return out
+
+    def hessian_vector_product(self, structure_or_graph, v, *, batch_size: int = 16) -> np.ndarray:
+        """H v with H = d^2E/dx dx (eV/A^2): E the total (extensive) energy, cell fixed, x the Cartesian positions.
+
+        ``v`` is ``[N,3]`` or ``[K,N,3]`` (K directions); the result is a float64 array of the same shape.  Exact
+        (analytic second derivatives through the kernels, no finite-difference step).  Accepts what
+        ``predict_structure`` accepts, or a ``CrystalGraph``; up to ``batch_size`` directions go through the engine
+        at once, as copies of the graph."""
+        graph = self._hessian_graph(structure_or_graph)
+        n = int(graph.atomic_number.shape[0])
+        v = np.asarray(v, dtype=np.float64)
+        if v.ndim not in (2, 3) or v.shape[-2:] != (n, 3):
+            raise ValueError(f"v must have shape [{n},3] or [K,{n},3], got {list(v.shape)}")
+        out = self._hvp_replicas(graph, v.reshape(-1, n, 3), batch_size)
+        return out.reshape(v.shape)
+
+    def predict_hessian(self, structure_or_graph, *, batch_size: int = 16) -> np.ndarray:
+        """Hessian of the total (extensive) energy with respect to the Cartesian positions at fixed cell, in eV/A^2:
+        a float64 array ``[3N,3N]`` with ``H[3*i + a, 3*j + b] = d^2E / dx_{i,a} dx_{j,b}``.
+
+        Column c is the exact Hessian-vector product with the unit vector e_c (no finite-difference step);
+        ``batch_size`` columns are computed per engine call, as copies of the graph.  H is returned as computed
+        (not symmetrised): its asymmetry is the fp32 rounding of the kernels.  The graph is built once, by
+        ``graph_converter`` (with its ``on_isolated_atoms`` policy) unless a ``CrystalGraph`` is given.
+
+        Phonopy's force-constant layout ``[N,N,3,3]`` is ``H.reshape(N, 3, N, 3).transpose(0, 2, 1, 3)``."""
+        graph = self._hessian_graph(structure_or_graph)
+        n = int(graph.atomic_number.shape[0])
+        cols = self._hvp_replicas(graph, np.eye(3 * n).reshape(3 * n, n, 3), batch_size)
+        return np.ascontiguousarray(cols.reshape(3 * n, 3 * n).T)
+
     def static_evaluator(self, graph, *, task: PredTask = "efsm"):
         """Evaluator for graph(s) whose TOPOLOGY stays fixed while coordinates / cells change (finite differences,
         phonon displacements, line searches): see ``StaticGraphEvaluator``."""

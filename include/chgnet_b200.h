@@ -510,6 +510,27 @@ int chg_readout_bwd2(const float* x, const float* xd, int32_t n_atoms, const flo
                      const float* seed, float* bar_x, float* h_all, float* hd_all, float* gz_all,
                      float* zbar_all, float* g_h0, float* hbar0, float* xhat, float* xhatd, void* stream);
 
+/* ======================= Hessian-vector products H v = d/dx <dE/dx, v> =======================
+ * The same tangent pass with rdot_e = v[c] - v[n], then the second reverse pass with a zero energy seed
+ * and, instead of parameter gradients, the geometry derivative of T: these three kernels add the
+ * second-order sources at the geometry inputs (the first-order parts reuse chg_bond_basis_bwd,
+ * chg_angle_basis_bwd and chg_force_virial).                                                        */
+/* g_dist [Eu] += < lam W^T, d^2B/dd^2 > ddist (all three radial embeddings, envelope included)       */
+int chg_bond_basis_hvp(const float* dist, const float* ddist, const int32_t* u2d, int32_t n_bonds,
+                       const float* freq_ag, const float* freq_bg, int32_t n_radial, float rc_ag,
+                       float rc_bg, int32_t p, const float* w3, const float* lam_e0, const float* lam_wag,
+                       const float* lam_wbg, float* g_dist, void* stream);
+/* g_rhat [Ed][3] (fp64) += d/d(rhat_i, rhat_j) < lam_a0, (dF/dtheta thetadot) W > with drhat held fixed */
+int chg_angle_basis_hvp(const float* rhat, const float* drhat, const int32_t* ang_di, const int32_t* ang_dj,
+                        int32_t n_angles, const float* freq, int32_t n_freq, const float* w,
+                        const float* lam_a0, double* g_rhat, void* stream);
+/* force [N][3] (fp64) -= d/dx of  lam_dist . ddist + lam_rhat . drhat  with rdot held fixed (the sign
+ * convention of chg_force_virial, so both accumulate into one buffer)                                */
+int chg_edge_tangent_bwd(const float* dist, const float* rhat, const float* ddist, const float* drhat,
+                         const float* lam_dist /* [Eu] */, const double* lam_rhat /* [Ed][3] */,
+                         const int32_t* d2u, const int32_t* u2d, const int32_t* center, const int32_t* nbr,
+                         int32_t n_edges, double* force, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
