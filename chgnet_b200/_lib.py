@@ -65,6 +65,7 @@ SIGNATURES: dict[str, list] = {
     "chg_bond_basis_hvp": [P, P, P, I, P, P, I, F, F, I, P, P, P, P, P, P],
     "chg_angle_basis_hvp": [P, P, P, P, I, P, I, P, P, P, P],
     "chg_edge_tangent_bwd": [P, P, P, P, P, P, P, P, P, P, I, P, P],
+    "chg_edge_tangent_bwd_virial": [P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P],
 }
 
 _lib = None
@@ -349,6 +350,12 @@ class CudaKernels:
         self._chk(dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, force)
         self._call("chg_edge_tangent_bwd", _p(dist), _p(rhat), _p(ddist), _p(drhat), _p(lam_dist), _p(lam_rhat), _p(d2u),
                    _p(u2d), _p(center), _p(nbr), center.shape[0], _p(force))
+
+    def edge_tangent_bwd_virial(self, rvec, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, owner,
+                                force, virial):
+        self._chk(rvec, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, owner, force, virial)
+        self._call("chg_edge_tangent_bwd_virial", _p(rvec), _p(dist), _p(rhat), _p(ddist), _p(drhat), _p(lam_dist),
+                   _p(lam_rhat), _p(d2u), _p(u2d), _p(center), _p(nbr), _p(owner), center.shape[0], _p(force), _p(virial))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

@@ -734,36 +734,88 @@ angle_basis_bwd2_kernel(const float* __restrict__ rhat, const float* __restrict_
   }
 }
 
+// virial[graph] += sum over the block's edges of r (x) g, row i column j at [i*3 + j].  Edges are grouped by graph,
+// so a block usually lies inside one graph: then a warp sum, a shared-memory sum over the 8 warps and 9 atomics per
+// block.  A block that spans graphs (a batch of small cells) falls back to one atomic per edge and component.  Every
+// thread of a 256-thread block calls it; threads past the last edge pass graph = -1 and r = g = 0.
+__device__ __forceinline__ void block_virial_add(const double (&r)[3], const double (&g)[3], int graph,
+                                                 const int32_t* __restrict__ center,
+                                                 const int32_t* __restrict__ owner, int n_edges,
+                                                 double* __restrict__ virial) {
+  __shared__ double s_v[8][9];
+  __shared__ int s_uniform;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int first = blockIdx.x * blockDim.x;
+  const int last = min(first + (int)blockDim.x, n_edges) - 1;
+  if (threadIdx.x == 0) s_uniform = owner[center[first]] == owner[center[last]];
+  __syncthreads();
+  if (s_uniform != 0) {
+    double v[9];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) v[i * 3 + j] = sum32d(r[i] * g[j]);
+    if (lane == 0) {
+#pragma unroll
+      for (int k = 0; k < 9; ++k) s_v[wid][k] = v[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < 9) {
+      double t = 0.0;
+      for (int w8 = 0; w8 < 8; ++w8) t += s_v[w8][threadIdx.x];
+      atomicAdd(virial + (size_t)owner[center[first]] * 9 + threadIdx.x, t);
+    }
+  } else if (graph >= 0) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) atomicAdd(virial + (size_t)graph * 9 + i * 3 + j, r[i] * g[j]);
+  }
+}
+
 // d/dr_e of  lam_d ddist + lam_rhat . drhat  with rdot held fixed (Hessian-vector products), scattered like
 // force_virial (force[c] -= g, force[n] += g).  ddist = rhat . rdot -> drhat;  drhat = (rdot - rhat ddist)/d ->
 // -[(mu . drhat) rhat + (mu . rhat) drhat + ddist (mu - rhat (rhat . mu))/d]/d,  mu = lam_rhat.  lam_d belongs to
 // the bond's representative edge only (the bond basis reads d there).
-__global__ void edge_tangent_bwd_kernel(const float* __restrict__ dist, const float* __restrict__ rhat,
-                                        const float* __restrict__ ddist, const float* __restrict__ drhat,
-                                        const float* __restrict__ lam_dist, const double* __restrict__ lam_rhat,
-                                        const int32_t* __restrict__ d2u, const int32_t* __restrict__ u2d,
-                                        const int32_t* __restrict__ center, const int32_t* __restrict__ nbr,
-                                        int n_edges, double* __restrict__ force) {
+// kVirial = true also adds sum_e r_e (x) g per graph to virial [B][9], as force_virial does (strain derivatives).
+template <bool kVirial>
+__global__ void __launch_bounds__(256)
+edge_tangent_bwd_kernel(const float* __restrict__ rvec, const float* __restrict__ dist,
+                        const float* __restrict__ rhat, const float* __restrict__ ddist,
+                        const float* __restrict__ drhat, const float* __restrict__ lam_dist,
+                        const double* __restrict__ lam_rhat, const int32_t* __restrict__ d2u,
+                        const int32_t* __restrict__ u2d, const int32_t* __restrict__ center,
+                        const int32_t* __restrict__ nbr, const int32_t* __restrict__ owner, int n_edges,
+                        double* __restrict__ force, double* __restrict__ virial) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n_edges) return;
-  const int c = center[e], n = nbr[e], u = d2u[e];
-  double rh[3], rd[3], mu[3];
+  double g[3] = {0.0, 0.0, 0.0}, r[3] = {0.0, 0.0, 0.0};
+  int graph = -1;
+  if (e < n_edges) {
+    const int c = center[e], n = nbr[e], u = d2u[e];
+    double rh[3], rd[3], mu[3];
 #pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    rh[j] = (double)rhat[(size_t)e * 3 + j];
-    rd[j] = (double)drhat[(size_t)e * 3 + j];
-    mu[j] = lam_rhat[(size_t)e * 3 + j];
-  }
-  const double inv_d = 1.0 / (double)dist[e], dd = (double)ddist[e];
-  const double ld = (u2d[u] == e) ? (double)lam_dist[u] : 0.0;
-  const double m_rd = mu[0] * rd[0] + mu[1] * rd[1] + mu[2] * rd[2];
-  const double m_rh = mu[0] * rh[0] + mu[1] * rh[1] + mu[2] * rh[2];
+    for (int j = 0; j < 3; ++j) {
+      rh[j] = (double)rhat[(size_t)e * 3 + j];
+      rd[j] = (double)drhat[(size_t)e * 3 + j];
+      mu[j] = lam_rhat[(size_t)e * 3 + j];
+    }
+    const double inv_d = 1.0 / (double)dist[e], dd = (double)ddist[e];
+    const double ld = (u2d[u] == e) ? (double)lam_dist[u] : 0.0;
+    const double m_rd = mu[0] * rd[0] + mu[1] * rd[1] + mu[2] * rd[2];
+    const double m_rh = mu[0] * rh[0] + mu[1] * rh[1] + mu[2] * rh[2];
 #pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    const double g = ld * rd[j] - (m_rd * rh[j] + m_rh * rd[j] + dd * (mu[j] - rh[j] * m_rh) * inv_d) * inv_d;
-    atomicAdd(force + (size_t)c * 3 + j, -g);
-    atomicAdd(force + (size_t)n * 3 + j, g);
+    for (int j = 0; j < 3; ++j) {
+      g[j] = ld * rd[j] - (m_rd * rh[j] + m_rh * rd[j] + dd * (mu[j] - rh[j] * m_rh) * inv_d) * inv_d;
+      atomicAdd(force + (size_t)c * 3 + j, -g[j]);
+      atomicAdd(force + (size_t)n * 3 + j, g[j]);
+    }
+    if constexpr (kVirial) {
+      graph = owner[c];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) r[j] = (double)rvec[(size_t)e * 3 + j];
+    }
   }
+  if constexpr (kVirial) block_virial_add(r, g, graph, center, owner, n_edges, virial);
 }
 
 // ---- magmom head -------------------------------------------------------------------
@@ -786,15 +838,7 @@ force_virial_kernel(const float* __restrict__ rvec, const float* __restrict__ di
                     const int32_t* __restrict__ center, const int32_t* __restrict__ nbr,
                     const int32_t* __restrict__ owner, int n_edges, double* __restrict__ force,
                     double* __restrict__ virial) {
-  __shared__ double s_v[8][9];
-  __shared__ int s_uniform;
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int first = blockIdx.x * blockDim.x;
-  const int last = min(first + (int)blockDim.x, n_edges) - 1;
-  if (threadIdx.x == 0) s_uniform = owner[center[first]] == owner[center[last]];
-  __syncthreads();
-  const bool uniform = s_uniform != 0;
   double g[3] = {0.0, 0.0, 0.0}, r[3] = {0.0, 0.0, 0.0};
   int graph = -1;
   if (e < n_edges) {
@@ -817,28 +861,7 @@ force_virial_kernel(const float* __restrict__ rvec, const float* __restrict__ di
       atomicAdd(force + (size_t)n * 3 + j, g[j]);
     }
   }
-  if (uniform) {
-    double v[9];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) v[i * 3 + j] = sum32d(r[i] * g[j]);
-    if (lane == 0) {
-#pragma unroll
-      for (int k = 0; k < 9; ++k) s_v[wid][k] = v[k];
-    }
-    __syncthreads();
-    if (threadIdx.x < 9) {
-      double t = 0.0;
-      for (int w8 = 0; w8 < 8; ++w8) t += s_v[w8][threadIdx.x];
-      atomicAdd(virial + (size_t)owner[center[first]] * 9 + threadIdx.x, t);
-    }
-  } else if (graph >= 0) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j) atomicAdd(virial + (size_t)graph * 9 + i * 3 + j, r[i] * g[j]);
-  }
+  block_virial_add(r, g, graph, center, owner, n_edges, virial);
 }
 
 inline int warp_grid(int n_items, int threads = 256) {
@@ -1051,7 +1074,22 @@ extern "C" int chg_edge_tangent_bwd(const float* dist, const float* rhat, const 
   if (n_edges == 0) return CHG_OK;
   CHG_CHECK_ARG(dist && rhat && ddist && drhat && lam_dist && lam_rhat && d2u && u2d && center && nbr && force,
                 "null pointer");
-  edge_tangent_bwd_kernel<<<(n_edges + 255) / 256, 256, 0, as_stream(stream)>>>(
-      dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, n_edges, force);
+  edge_tangent_bwd_kernel<false><<<(n_edges + 255) / 256, 256, 0, as_stream(stream)>>>(
+      nullptr, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, nullptr, n_edges, force, nullptr);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_edge_tangent_bwd_virial(const float* rvec, const float* dist, const float* rhat,
+                                           const float* ddist, const float* drhat, const float* lam_dist,
+                                           const double* lam_rhat, const int32_t* d2u, const int32_t* u2d,
+                                           const int32_t* center, const int32_t* nbr, const int32_t* atom_owner,
+                                           int32_t n_edges, double* force, double* virial, void* stream) {
+  CHG_CHECK_ARG(n_edges >= 0, "negative size");
+  if (n_edges == 0) return CHG_OK;
+  CHG_CHECK_ARG(rvec && dist && rhat && ddist && drhat && lam_dist && lam_rhat && d2u && u2d && center && nbr &&
+                    atom_owner && force && virial,
+                "null pointer");
+  edge_tangent_bwd_kernel<true><<<(n_edges + 255) / 256, 256, 0, as_stream(stream)>>>(
+      rvec, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, atom_owner, n_edges, force, virial);
   CHG_LAUNCH_END();
 }

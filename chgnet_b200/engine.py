@@ -272,10 +272,26 @@ class Engine:
         self.input_grads(out, record=True)
         st = out.extras.pop("train_state")
         return self._second_order(st, dict(seed_energy=self._zeros(b, b.n_graphs, dtype=torch.float64), seed_magmom=None,
-                                           seed_force=None, seed_stress=None, grads=None, directions=directions))
+                                           seed_force=None, seed_stress=None, grads=None, directions=directions))[0]
+
+    def second_derivatives(self, b: DeviceBatch, directions: Tensor, strain_directions: Tensor) -> tuple[Tensor, Tensor]:
+        """dT/dx per atom ``[N,3]`` and dT/d(strain) per graph ``[B,3,3]``, both fp64, for
+        T = <dE/dx, v> + <dE/dstrain, W> of each graph: v = ``directions`` ``[N,3]``, W = ``strain_directions``
+        ``[B,3,3]``.  Strain maps every edge vector r_e -> r_e (I + strain) (fractional coordinates fixed), so
+        dE/dstrain = sum_e r_e (x) dE/dr_e; E is the extensive model energy.  The two outputs are
+        H v + Lambda W and Lambda^T v + D W, with H = d^2E/dx dx, D = d^2E/dstrain dstrain and Lambda the
+        position-strain block d^2E/dx dstrain, all second derivatives of E(r) taken through the edge vectors with
+        rdot_e = v[c] - v[n] + r_e . W held fixed (for Lambda: -dF/dstrain at fixed fractional coordinates)."""
+        out = self.run(b, need_grad=True, train=True)
+        self.input_grads(out, record=True)
+        st = out.extras.pop("train_state")
+        hv, dt_dstrain = self._second_order(st, dict(
+            seed_energy=self._zeros(b, b.n_graphs, dtype=torch.float64), seed_magmom=None, seed_force=None,
+            seed_stress=None, grads=None, directions=directions, strain_directions=strain_directions))
+        return hv, dt_dstrain.view(b.n_graphs, 3, 3)
 
     # ------------------------------------------------------------------ second order
-    def _second_order(self, st: dict, train: dict) -> Tensor | None:
+    def _second_order(self, st: dict, train: dict) -> tuple[Tensor, Tensor] | None:
         """Parameter gradients of a loss that also depends on forces and stresses (reference
         model.py:518-535 ``create_graph=True`` + trainer.py:409 ``loss.backward()``).
 
@@ -289,7 +305,9 @@ class Engine:
 
         Hessian-vector mode (``train["grads"] is None``, ``train["directions"]`` = v per atom, zero energy seed):
         rdot_e = v[c] - v[n], so T = <dE/dx, v>, and dT/dx = H v.  No parameter gradient is formed; the tail
-        differentiates T with respect to the geometry instead (:meth:`_geometry_tail`) and returns H v.
+        differentiates T with respect to the geometry instead (:meth:`_geometry_tail`) and returns H v.  With
+        ``train["strain_directions"]`` = W per graph as well, rdot_e gains r_e . W and the tail also returns the
+        per-graph strain derivative of T (:meth:`second_derivatives`).
         """
         pw, K, hp = self.pw, self.K, self.pw.hp
         b: DeviceBatch = st["b"]
@@ -324,6 +342,9 @@ class Engine:
         if train["seed_stress"] is not None:
             scale = (EV_A3_TO_GPA / b.volume.to(torch.float64))[:, None, None]
             w_graph = (train["seed_stress"].to(torch.float64).view(B, 3, 3) * scale).to(dt).reshape(B, 9).contiguous()
+        per_graph = train.get("strain_directions") is not None
+        if per_graph:
+            w_graph = train["strain_directions"].to(dt).reshape(B, 9).contiguous()
         ddist, drhat = self._new(b, Ed), self._new(b, Ed, 3)
         K.edge_tangent(rvec, dist, rhat, b.center, b.nbr, b.owner, u_atom, w_graph, ddist, drhat)
         e_d, wag_d, wbg_d, tb = (self._new(b, Eu, 64) for _ in range(4))
@@ -486,7 +507,7 @@ class Engine:
         if has_ang:
             K.scatter_rows(bar_wbg, sid, bar_wbg_full)
         if G is None:
-            return self._geometry_tail(st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a)
+            return self._geometry_tail(st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a, per_graph)
 
         # ---------------- embeddings, basis weights, basis frequencies ----------------
         R, NA = pw.freq_ag.shape[0], pw.wang.shape[1]
@@ -511,12 +532,16 @@ class Engine:
             K.angle_basis_bwd2(rhat, drhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, rec["g_a0"], g_fa)
             G["freq_ang"] = g_fa.to(dt)
 
-    def _geometry_tail(self, st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a) -> Tensor:
+    def _geometry_tail(self, st, ddist, drhat, bar_e, bar_wag, bar_wbg_full, bar_a,
+                       per_graph: bool = False) -> tuple[Tensor, Tensor]:
         """dT/dx (= H v) from the basis-level adjoints of the second reverse pass.  Per directed edge, dT/dr_e is
         (a) the first-order geometry reverse fed with the bar adjoints, (b) lambda . d^2B/dd^2 ddist per bond,
         (c) lambda_a0 . d^2 Fourier(theta) along (drhat_i, drhat_j), and (d) the derivative of the tangent map
         (ddist, drhat)(r_e) with rdot fixed, weighted by the recorded lambda_d, lambda_rhat.  (a)-(c) meet in one
-        (g_dist, g_rhat) pair that chg_force_virial turns into -dT/dx; (d) accumulates there too."""
+        (g_dist, g_rhat) pair that chg_force_virial turns into -dT/dx; (d) accumulates there too.
+
+        Returns (dT/dx [N,3], virial [B,9]).  The virial sum_e r_e (x) dT/dr_e is dT/dstrain; it holds all four
+        terms only with ``per_graph`` (chg_edge_tangent_bwd_virial adds (d)), otherwise (a)-(c)."""
         pw, K, hp = self.pw, self.K, self.pw.hp
         b: DeviceBatch = st["b"]
         rec, dist, rvec, rhat = st["rec"], st["dist"], st["rvec"], st["rhat"]
@@ -530,10 +555,15 @@ class Engine:
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, bar_a, g_rhat)
             K.angle_basis_hvp(rhat, drhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, rec["g_a0"], g_rhat)
         neg_hv = self._zeros(b, b.n_atoms, 3, dtype=torch.float64)
-        K.force_virial(rvec, dist, rhat, g_rhat, g_dist, b.d2u, b.u2d, b.center, b.nbr, b.owner, neg_hv,
-                       self._zeros(b, b.n_graphs, 9, dtype=torch.float64))
-        K.edge_tangent_bwd(dist, rhat, ddist, drhat, rec["g_dist"], rec["g_rhat"], b.d2u, b.u2d, b.center, b.nbr, neg_hv)
-        return neg_hv.neg_()
+        virial = self._zeros(b, b.n_graphs, 9, dtype=torch.float64)
+        K.force_virial(rvec, dist, rhat, g_rhat, g_dist, b.d2u, b.u2d, b.center, b.nbr, b.owner, neg_hv, virial)
+        if per_graph:
+            K.edge_tangent_bwd_virial(rvec, dist, rhat, ddist, drhat, rec["g_dist"], rec["g_rhat"], b.d2u, b.u2d,
+                                      b.center, b.nbr, b.owner, neg_hv, virial)
+        else:
+            K.edge_tangent_bwd(dist, rhat, ddist, drhat, rec["g_dist"], rec["g_rhat"], b.d2u, b.u2d, b.center, b.nbr,
+                               neg_hv)
+        return neg_hv.neg_(), virial
 
     def _wgrad(self, b, x, g, n, *, x_rows=None, g_rows=None, x_silu=False, colsum=False):
         out = self._new(b, 64, n)

@@ -159,6 +159,40 @@ def _init_param(shape, kind: str, a: dict) -> Tensor:
     raise AssertionError(kind)
 
 
+def _voigt_directions() -> np.ndarray:
+    """[6,3,3] strain directions in Voigt order xx, yy, zz, yz, xz, xy: (E_ij + E_ji)/2 (engineering shears)."""
+    w = np.zeros((6, 3, 3))
+    for a, (i, j) in enumerate(((0, 0), (1, 1), (2, 2), (1, 2), (0, 2), (0, 1))):
+        w[a, i, j] += 0.5
+        w[a, j, i] += 0.5
+    return w
+
+
+_VOIGT_DIRECTIONS = _voigt_directions()
+
+
+def _relax_ions(clamped: np.ndarray, lam: np.ndarray, h: np.ndarray, scale: float) -> tuple[np.ndarray, int]:
+    """C - scale Lambda^T H+ Lambda in fp64 (CHGNet.predict_elastic_tensor), and the number of unstable modes.  H+ is the
+    inverse of the symmetrised H on the orthonormal complement of the rigid translations; eigenvalues with
+    |lambda| <= 1e-8 max|lambda| there count as zero."""
+    n = h.shape[0] // 3
+    if n < 2:  # one atom: nothing to relax
+        return clamped.copy(), 0
+    hs = 0.5 * (h + h.T)
+    trans = np.tile(np.eye(3), (n, 1)) / math.sqrt(n)  # orthonormal rigid translations [3N,3]
+    q = np.linalg.qr(trans, mode="complete")[0][:, 3:]  # orthonormal basis of their complement [3N,3N-3]
+    evals, vecs = np.linalg.eigh(q.T @ hs @ q)
+    top = float(np.abs(evals).max())
+    keep = np.abs(evals) > 1e-8 * top
+    unstable = int((evals < -1e-6 * float(np.abs(hs).max())).sum())
+    if unstable:
+        warnings.warn(f"the Hessian has {unstable} unstable mode(s) (smallest eigenvalue {evals.min():.4g} eV/A^2): "
+                      "the relaxed-ion tensor is the response of a stationary point, not of a minimum", RuntimeWarning,
+                      stacklevel=3)
+    ql = (q @ vecs[:, keep]).T @ lam  # Lambda in the kept eigenbasis
+    return clamped - scale * (ql.T / evals[keep]) @ ql, unstable
+
+
 class _ParamGradBridge(torch.autograd.Function):
     """Joins the kernel engine to autograd: backward = the engine's training reverse pass."""
 
@@ -755,23 +789,31 @@ class CHGNet(nn.Module):
             raise ValueError("graph_converter cannot be None!")
         return self.graph_converter(structure_or_graph)
 
-    def _hvp_replicas(self, graph, v: np.ndarray, batch_size: int) -> np.ndarray:
+    def _hvp_replicas(self, graph, v: np.ndarray, batch_size: int, w: np.ndarray | None = None):
         """H v for K directions ``v [K,N,3]``: batches of up to ``batch_size`` copies of the graph, one direction per copy
-        (Engine.hessian_vector_products)."""
+        (Engine.hessian_vector_products).  With strain directions ``w [K,3,3]`` as well, returns the pair
+        (dT/dx [K,N,3], dT/dstrain [K,3,3]) of ``Engine.second_derivatives`` instead."""
         if batch_size < 1:
             raise ValueError(f"{batch_size=} must be >= 1")
         engine = self._get_engine()
         compact = not self._arch.get("mlp_out_bias", False)
         n_dirs, n = v.shape[0], v.shape[1]
         out = np.empty((n_dirs, n, 3), dtype=np.float64)
+        out_strain = None if w is None else np.empty((n_dirs, 3, 3), dtype=np.float64)
         batches: dict[int, DeviceBatch] = {}
         for s in range(0, n_dirs, batch_size):
             k = min(batch_size, n_dirs - s)
             if k not in batches:  # the graph is fixed: one device batch per replica count
                 batches[k] = build_batch([graph] * k, self.device, with_reverse=True, compact_bonds=compact)
             d = torch.as_tensor(v[s : s + k].reshape(k * n, 3), dtype=torch.float32).to(self.device)
-            out[s : s + k] = engine.hessian_vector_products(batches[k], d).view(k, n, 3).cpu().numpy()
-        return out
+            if w is None:
+                out[s : s + k] = engine.hessian_vector_products(batches[k], d).view(k, n, 3).cpu().numpy()
+                continue
+            ws = torch.as_tensor(w[s : s + k], dtype=torch.float32).to(self.device)
+            hv, dstrain = engine.second_derivatives(batches[k], d, ws)
+            out[s : s + k] = hv.view(k, n, 3).cpu().numpy()
+            out_strain[s : s + k] = dstrain.cpu().numpy()
+        return out if w is None else (out, out_strain)
 
     def hessian_vector_product(self, structure_or_graph, v, *, batch_size: int = 16) -> np.ndarray:
         """H v with H = d^2E/dx dx (eV/A^2): E the total (extensive) energy, cell fixed, x the Cartesian positions.
@@ -802,6 +844,55 @@ class CHGNet(nn.Module):
         n = int(graph.atomic_number.shape[0])
         cols = self._hvp_replicas(graph, np.eye(3 * n).reshape(3 * n, n, 3), batch_size)
         return np.ascontiguousarray(cols.reshape(3 * n, 3 * n).T)
+
+    def predict_elastic_tensor(self, structure_or_graph, *, relaxed_ions: bool = True, batch_size: int = 16) -> dict:
+        """Clamped-ion (and relaxed-ion) elastic tensor of a cell from exact second derivatives of the energy: no
+        strain step, no ionic relaxations.  Accepts what ``predict_hessian`` accepts; the graph is built once.
+
+        Conventions:
+
+        * Strain acts as the stress's does: lattice -> lattice (I + strain) at fixed fractional coordinates, so every
+          edge vector goes r_e -> r_e (I + strain).
+        * Voigt order xx, yy, zz, yz, xz, xy with engineering shear strains: direction a is the symmetric strain
+          (E_ij + E_ji)/2, E_ii for a normal strain.
+        * ``clamped_ion`` ``[6,6]`` GPa: C_ab = (160.21766208 / V) d^2E/de_a de_b, E the total (extensive) model energy,
+          V the volume of the given cell.  Returned as computed, not symmetrised.
+        * ``internal_strain`` ``[3N,6]`` eV/A: Lambda[3i+b, a] = d^2E/dx_{i,b} de_a = -dF_{i,b}/de_a at fixed
+          fractional coordinates (rows laid out as in ``predict_hessian``).
+        * ``relaxed_ion`` ``[6,6]`` GPa (``relaxed_ions=True``): C - (160.21766208 / V) Lambda^T H+ Lambda, the response
+          when the ions relax to first order.  H is the Hessian symmetrised for this step; H+ inverts it on the
+          3N-3 dimensional complement of the rigid translations, which are projected out exactly, and treats
+          eigenvalues with |lambda| <= 1e-8 max|lambda| there as zero.  ``hessian`` ``[3N,3N]`` is the Hessian as
+          ``predict_hessian`` returns it.  ``unstable_modes`` counts the eigenvalues below -1e-6 max|H|: if there
+          are any, a ``RuntimeWarning`` is emitted and the result is still returned (the stationary-point response,
+          no longer the response of a minimum).
+
+        This is the energy-strain tensor at the given state.  For a cell under a residual stress sigma the
+        stress-strain coefficients differ from it by terms of order sigma, and residual forces make the relaxed-ion
+        correction a stationary-point estimate: relax the cell first (forces and stress ~ 0) for the tensor to
+        mean what is usually meant by the elastic constants.
+
+        The 6 strain directions (and, with ``relaxed_ions``, the 3N unit position directions) run as copies of the
+        graph, ``batch_size`` per engine call (``Engine.second_derivatives``)."""
+        graph = self._hessian_graph(structure_or_graph)
+        n = int(graph.atomic_number.shape[0])
+        lat = np.asarray(graph.lattice.detach().cpu().numpy() if torch.is_tensor(graph.lattice) else graph.lattice,
+                         dtype=np.float64).reshape(3, 3)
+        scale = EV_A3_TO_GPA / abs(float(np.linalg.det(lat)))
+        n_pos = 3 * n if relaxed_ions else 0
+        v = np.zeros((6 + n_pos, n, 3))
+        v.reshape(6 + n_pos, 3 * n)[6:] = np.eye(3 * n)[:n_pos]
+        w = np.zeros((6 + n_pos, 3, 3))
+        w[:6] = _VOIGT_DIRECTIONS
+        per_atom, per_strain = self._hvp_replicas(graph, v, batch_size, w)
+        clamped = scale * np.einsum("aij,bij->ab", _VOIGT_DIRECTIONS, per_strain[:6])
+        lam = np.ascontiguousarray(per_atom[:6].reshape(6, 3 * n).T)
+        out = {"clamped_ion": clamped, "internal_strain": lam}
+        if relaxed_ions:
+            h = np.ascontiguousarray(per_atom[6:].reshape(3 * n, 3 * n).T)
+            relaxed, unstable = _relax_ions(clamped, lam, h, scale)
+            out.update(relaxed_ion=relaxed, hessian=h, unstable_modes=unstable)
+        return out
 
     def static_evaluator(self, graph, *, task: PredTask = "efsm"):
         """Evaluator for graph(s) whose TOPOLOGY stays fixed while coordinates / cells change (finite differences,

@@ -530,6 +530,15 @@ int chg_edge_tangent_bwd(const float* dist, const float* rhat, const float* ddis
                          const float* lam_dist /* [Eu] */, const double* lam_rhat /* [Ed][3] */,
                          const int32_t* d2u, const int32_t* u2d, const int32_t* center, const int32_t* nbr,
                          int32_t n_edges, double* force, void* stream);
+/* chg_edge_tangent_bwd, and also virial [B][9] (fp64) += sum_e r_e (x) g_e per graph, g_e the same edge term, in
+ * the layout and sign of chg_force_virial's virial (so both accumulate into one buffer).  With a strain direction W
+ * in the tangent (rdot_e = u[c] - u[n] + r_e . W) this virial is the strain derivative of T = <dE/dr, rdot>:
+ * a column of d^2E/dstrain^2 and of the position-strain block (CHGNet.predict_elastic_tensor).           */
+int chg_edge_tangent_bwd_virial(const float* rvec, const float* dist, const float* rhat, const float* ddist,
+                                const float* drhat, const float* lam_dist /* [Eu] */,
+                                const double* lam_rhat /* [Ed][3] */, const int32_t* d2u, const int32_t* u2d,
+                                const int32_t* center, const int32_t* nbr, const int32_t* atom_owner,
+                                int32_t n_edges, double* force, double* virial, void* stream);
 
 #ifdef __cplusplus
 }
