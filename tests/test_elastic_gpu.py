@@ -53,6 +53,7 @@ def _recording_kernels():
 
 
 def test_every_second_derivatives_kernel_matches_its_spec(weights030):
+    import replay_fp64
     from kernel_replay import OUT_ARGS
 
     from chgnet_b200._lib import CudaKernels
@@ -68,23 +69,11 @@ def test_every_second_derivatives_kernel_matches_its_spec(weights030):
     rec = _recording_kernels()
     eng = Engine(pack_weights({k: torch.as_tensor(t) for k, t in weights030.items()}, None, device="cpu"), rec)
     eng.second_derivatives(build_batch(graphs, "cpu"), v, w)
-    K = CudaKernels()
-    seen = {}
-    for name, snap, outs in rec.calls:
-        args = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
-        getattr(K, name)(*args)
-        torch.cuda.synchronize()
-        for idx, want in outs.items():
-            got, want = args[idx].double().cpu(), want.double()
-            scale = float(want.abs().max()) if want.numel() else 1.0
-            err = float((got - want).abs().max()) if want.numel() else 0.0
-            # as in test_hessian_gpu: 1e-4 of scale for the second-derivative geometry kernels, 2e-5 for the others
-            tol = (1e-4 if name in SD_OUT_ARGS else 2e-5) * max(scale, 1.0) + 1e-6
-            assert err <= tol, f"{name} out[{idx}]: max err {err:.3e} > {tol:.3e} (scale {scale:.3e})"
-            seen[name] = max(seen.get(name, 0.0), err)
-    assert set(SD_OUT_ARGS) <= set(seen) and set(seen) <= set(OUT_ARGS) | set(SD_OUT_ARGS), sorted(seen)
-    assert "edge_tangent_bwd" not in seen
-    print({k: f"{e:.2e}" for k, e in seen.items()})
+    chk = replay_fp64.Checker()
+    replay_fp64.replay(rec.calls, CudaKernels(), chk)
+    chk.assert_ok("second derivatives")
+    assert set(SD_OUT_ARGS) <= chk.kernels and chk.kernels <= set(OUT_ARGS) | set(SD_OUT_ARGS), sorted(chk.kernels)
+    assert "edge_tangent_bwd" not in chk.kernels
 
 
 def _figures(got, want):

@@ -49,6 +49,7 @@ def _recording_kernels():
 
 
 def test_every_hvp_kernel_matches_its_spec(weights030):
+    import replay_fp64
     from kernel_replay import OUT_ARGS
 
     from chgnet_b200._lib import CudaKernels
@@ -59,23 +60,10 @@ def test_every_hvp_kernel_matches_its_spec(weights030):
     eng = Engine(pack_weights({k: torch.as_tensor(v) for k, v in weights030.items()}, None, device="cpu"), rec)
     v = torch.randn(n, 3, generator=torch.Generator().manual_seed(5))
     eng.hessian_vector_products(build_batch(graphs, "cpu"), v)
-    K = CudaKernels()
-    seen = {}
-    for name, snap, outs in rec.calls:
-        args = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
-        getattr(K, name)(*args)
-        torch.cuda.synchronize()
-        for idx, want in outs.items():
-            got, want = args[idx].double().cpu(), want.double()
-            scale = float(want.abs().max()) if want.numel() else 1.0
-            err = float((got - want).abs().max()) if want.numel() else 0.0
-            # fp32 kernels vs fp32 spec, different summation order; the new kernels hold second derivatives of
-            # acos, whose d^2 theta / du^2 reaches (2e-6)^(-3/2) near collinear pairs: 1e-4 of scale for those
-            tol = (1e-4 if name in HVP_OUT_ARGS else 2e-5) * max(scale, 1.0) + 1e-6
-            assert err <= tol, f"{name} out[{idx}]: max err {err:.3e} > {tol:.3e} (scale {scale:.3e})"
-            seen[name] = max(seen.get(name, 0.0), err)
-    assert set(HVP_OUT_ARGS) <= set(seen) and set(seen) <= set(OUT_ARGS) | set(HVP_OUT_ARGS), sorted(seen)
-    print({k: f"{e:.2e}" for k, e in seen.items()})
+    chk = replay_fp64.Checker()
+    replay_fp64.replay(rec.calls, CudaKernels(), chk)
+    chk.assert_ok("Hessian-vector products")
+    assert set(HVP_OUT_ARGS) <= chk.kernels and chk.kernels <= set(OUT_ARGS) | set(HVP_OUT_ARGS), sorted(chk.kernels)
 
 
 def _figures(h, want):

@@ -22,20 +22,14 @@ def _record(weights, graphs, **kw):
     return rec.calls
 
 
-def _close(name, idx, got, want):
-    got, want = got.double().cpu(), want.double()
-    scale = float(want.abs().max()) if want.numel() else 1.0
-    err = float((got - want).abs().max()) if want.numel() else 0.0
-    # fp32 kernels vs fp32 spec: different summation order only
-    tol = 2e-5 * max(scale, 1.0) + 1e-6
-    assert err <= tol, f"{name} out[{idx}]: max err {err:.3e} > {tol:.3e} (scale {scale:.3e})"
-    return err
-
-
 @pytest.fixture(scope="module")
 def recorded(weights030):
+    """The calls of a forward + reverse pass and their fp64 references (tests/replay_fp64.py)."""
+    import replay_fp64
+
     graphs = graphgen.random_graphs(3, 10, 16, 9300)
-    return _record(weights030, graphs, need_grad=True, need_magmom=True, need_atom_fea=True, need_crystal_fea=True)
+    calls = _record(weights030, graphs, need_grad=True, need_magmom=True, need_atom_fea=True, need_crystal_fea=True)
+    return calls, [replay_fp64.reference64(name, snap) for name, snap, _ in calls]
 
 
 # ids are the stable names of the implementation slots (option values); on sm_90a every tensor-core slot is a wgmma kernel
@@ -43,7 +37,9 @@ def recorded(weights030):
                          ids=["defaults: linear=tcgen05-ws,gated=fused-tcgen05-ws", "linear=tcgen05-ws,gated=ffma4x8",
                               "linear=tcgen05,gated=ffma4x8", "linear=ffma,gated=tcgen05", "linear=tcgen05+tma,gated=ffma8x8"])
 def test_every_kernel_matches_its_spec(recorded, linear_impl, gated_impl):
-    """Both implementations of every entry point (wgmma 3xTF32 and FFMA) against the spec."""
+    """Both implementations of every entry point (wgmma 3xTF32 and FFMA) against the fp64 spec."""
+    import replay_fp64
+
     from chgnet_b200._lib import CudaKernels
 
     K = CudaKernels()
@@ -51,16 +47,11 @@ def test_every_kernel_matches_its_spec(recorded, linear_impl, gated_impl):
     K.set_option("gated_impl", gated_impl)
     K.set_option("ws_min_rows", 0)  # the recorded graphs are small: run the tensor-core kernels on them anyway
     try:
-        seen = {}
-        for name, snap, outs in recorded:
-            args = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
-            getattr(K, name)(*args)
-            torch.cuda.synchronize()
-            for idx, want in outs.items():
-                err = _close(name, idx, args[idx], want)
-                seen[name] = max(seen.get(name, 0.0), err)
-        assert set(seen) == __import__("kernel_replay").INFER_KERNELS, sorted(seen)
-        print({k: f"{v:.2e}" for k, v in seen.items()})
+        chk = replay_fp64.Checker()
+        calls, refs = recorded
+        replay_fp64.replay(calls, K, chk, refs)
+        chk.assert_ok(f"linear_impl={linear_impl}, gated_impl={gated_impl}")
+        assert chk.kernels == __import__("kernel_replay").INFER_KERNELS, sorted(chk.kernels)
     finally:
         K.set_option("linear_impl", 3)
         K.set_option("gated_impl", 3)
@@ -70,6 +61,7 @@ def test_every_kernel_matches_its_spec(recorded, linear_impl, gated_impl):
 def test_every_training_kernel_matches_its_spec(weights030):
     """Training reverse pass (parameter gradients): every call of a real train step, replayed."""
     import kernel_replay
+    import replay_fp64
     from chgnet_b200._lib import CudaKernels
     from kernel_replay import RecordingKernels
 
@@ -87,16 +79,10 @@ def test_every_training_kernel_matches_its_spec(weights030):
     eng.input_grads(out, record=True)
     eng.param_grads(out, torch.randn(len(graphs), generator=gen), torch.randn(n_atoms, generator=gen),
                     torch.randn(n_atoms, 3, generator=gen), torch.randn(len(graphs), 3, 3, generator=gen))
-    K = CudaKernels()
-    seen = {}
-    for name, snap, outs in rec.calls:
-        args = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
-        getattr(K, name)(*args)
-        torch.cuda.synchronize()
-        for idx, want in outs.items():
-            seen[name] = max(seen.get(name, 0.0), _close(name, idx, args[idx], want))
-    assert kernel_replay.TRAIN_KERNELS <= set(seen), sorted(seen)
-    print({k: f"{v:.2e}" for k, v in seen.items()})
+    chk = replay_fp64.Checker()
+    replay_fp64.replay(rec.calls, CudaKernels(), chk)
+    chk.assert_ok("training")
+    assert kernel_replay.TRAIN_KERNELS <= chk.kernels, sorted(chk.kernels)
 
 
 def test_loss_terms_and_adam_match_torch():
@@ -167,6 +153,8 @@ def test_linear_large_ragged_calls(impl):
 
 def test_kernels_without_layernorm_and_small_basis(weights030):
     """v0.2.0-shaped path: no LayerNorm, 9 radial / 9 angular functions, mlp_out bias."""
+    import replay_fp64
+
     from chgnet_b200._lib import CudaKernels
     from oracle import chgnet_oracle as orc
 
@@ -182,12 +170,9 @@ def test_kernels_without_layernorm_and_small_basis(weights030):
     assert not pw.hp.use_ln and pw.hp.n_readout_hidden == 2 and pw.hp.num_radial == 9
     rec = RecordingKernels()
     Engine(pw, rec).run(build_batch(graphs, "cpu", compact_bonds=False), need_grad=True, need_magmom=True)
-    K = CudaKernels()
-    for name, snap, outs in rec.calls:
-        cargs = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
-        getattr(K, name)(*cargs)
-        for idx, want in outs.items():
-            _close(name, idx, cargs[idx], want)
+    chk = replay_fp64.Checker()
+    replay_fp64.replay(rec.calls, CudaKernels(), chk)
+    chk.assert_ok("no LayerNorm, small basis")
 
 
 def test_segment_sum_strided_output_and_determinism():
