@@ -66,6 +66,8 @@ SIGNATURES: dict[str, list] = {
     "chg_angle_basis_hvp": [P, P, P, P, I, P, I, P, P, P, P],
     "chg_edge_tangent_bwd": [P, P, P, P, P, P, P, P, P, P, I, P, P],
     "chg_edge_tangent_bwd_virial": [P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P],
+    # phonons
+    "chg_dynamical_matrices": [P, P, P, P, P, I, I, P, I, P, P],
 }
 
 _lib = None
@@ -356,6 +358,14 @@ class CudaKernels:
         self._chk(rvec, dist, rhat, ddist, drhat, lam_dist, lam_rhat, d2u, u2d, center, nbr, owner, force, virial)
         self._call("chg_edge_tangent_bwd_virial", _p(rvec), _p(dist), _p(rhat), _p(ddist), _p(drhat), _p(lam_dist),
                    _p(lam_rhat), _p(d2u), _p(u2d), _p(center), _p(nbr), _p(owner), center.shape[0], _p(force), _p(virial))
+
+    def dynamical_matrices(self, fc, img_ptr, img_vec, s2p, inv_sqrt_m, qpoints, dyn):
+        """dyn [Q, 3n, 3n] complex128 (overwritten) = D(q) of the compact force constants fc [n, N, 3, 3] (fp64)."""
+        self._chk(fc, img_ptr, img_vec, s2p, inv_sqrt_m, qpoints, dyn)
+        if dyn.dtype != torch.complex128 or fc.dtype != torch.float64 or qpoints.dtype != torch.float64:
+            raise ChgnetB200Error("dynamical_matrices: fc and qpoints must be float64, dyn complex128")
+        self._call("chg_dynamical_matrices", _p(fc), _p(img_ptr), _p(img_vec), _p(s2p), _p(inv_sqrt_m), fc.shape[0],
+                   fc.shape[1], _p(qpoints), qpoints.shape[0], _p(dyn))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

@@ -894,6 +894,30 @@ class CHGNet(nn.Module):
             out.update(relaxed_ion=relaxed, hessian=h, unstable_modes=unstable)
         return out
 
+    def phonons(self, structure, supercell_matrix, *, batch_size: int = 16):
+        """Harmonic phonons of a crystal from exact supercell force constants: a ``chgnet_b200.phonons.Phonons``.
+
+        ``structure`` is the primitive cell, in any form ``GraphConverter`` accepts (a structure-like object or a
+        ``(z, frac, lattice)`` tuple); ``supercell_matrix`` an integer 3x3 matrix M or a 3-vector meaning a diagonal.
+        The supercell has the lattice ``M @ lattice`` (rows are lattice vectors, as phonopy builds it) and atom-major
+        order: atom j = k n_cells + l is primitive atom k moved by lattice point l.  Its graph is built once, by
+        ``graph_converter``; the 3 n_prim Hessian-vector products that move the atoms of one primitive cell (as in
+        ``predict_hessian``, ``batch_size`` per engine call) give the compact force constants ``[n_prim, N, 3, 3]``
+        in eV/A^2, returned as computed (not symmetrised).  Frequencies (THz) and eigenvectors at any q, and the
+        harmonic free energy, entropy and heat capacity on a q mesh, come from ``Phonons.frequencies`` and
+        ``Phonons.thermal_properties``, with the dynamical matrices built on the device.
+
+        The supercell should be large enough that the force constants have decayed at its boundary, and the structure
+        should be relaxed: unstable modes are reported as imaginary (negative) frequencies, not hidden."""
+        from chgnet_b200.phonons import Phonons, compact_force_constants, make_supercell
+
+        if self.graph_converter is None:
+            raise ValueError("graph_converter cannot be None!")
+        sc = make_supercell(*self._structure_arrays(structure), supercell_matrix)
+        graph = self.graph_converter((sc.z, sc.frac, sc.lattice))
+        fc = compact_force_constants(lambda v: self._hvp_replicas(graph, v, batch_size), sc)
+        return Phonons(fc, sc, device=self.device)
+
     def static_evaluator(self, graph, *, task: PredTask = "efsm"):
         """Evaluator for graph(s) whose TOPOLOGY stays fixed while coordinates / cells change (finite differences,
         phonon displacements, line searches): see ``StaticGraphEvaluator``."""

@@ -1,0 +1,295 @@
+"""Harmonic phonons from supercell force constants (``CHGNet.phonons``).
+
+* ``make_supercell``: the supercell of a primitive cell for an integer matrix M (lattice ``M @ lattice``, rows are
+  lattice vectors, as phonopy builds it), its atom maps and the minimum-image table of every (primitive atom,
+  supercell atom) pair.
+* ``compact_force_constants``: the force constants ``[n_prim, N_super, 3, 3]`` (phonopy's compact layout) from the
+  3 n_prim Hessian-vector products that move the atoms of one primitive cell.  The supercell is periodic in the
+  primitive lattice, Phi(k l, k' l') = Phi(k 0, k' (l' - l)), so these columns determine every force constant.
+* ``Phonons``: dynamical matrices D(q) on the device (``chg_dynamical_matrices``, csrc/phonons.cu), frequencies and
+  eigenvectors by ``torch.linalg.eigh``, and harmonic thermodynamics on a Gamma-centred mesh.
+
+Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
+eV and eV/K per primitive cell for the thermodynamic functions.
+"""
+from __future__ import annotations
+
+import itertools
+import math
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from chgnet_b200.dynamics import ATOMIC_MASSES, KB
+
+# sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
+_EV, _AMU, _ANGSTROM = 1.602176634e-19, 1.66053906660e-27, 1e-10
+THZ_PER_SQRT_EV_A2_AMU = math.sqrt(_EV / (_ANGSTROM**2 * _AMU)) / (2 * math.pi) / 1e12
+H_EV_PER_THZ = 6.62607015e-34 / _EV * 1e12  # h nu in eV for nu in THz
+# image lengths within this of the shortest count as minimum images (A)
+IMAGE_TOL = 1e-5
+# modes below this |nu| (THz) are left out of the thermodynamic sums
+THERMAL_CUTOFF_THZ = 1e-3
+
+
+def supercell_matrix(m) -> np.ndarray:
+    """[3,3] integer matrix from a 3x3 matrix or a 3-vector (diagonal); raises ValueError if it is not integral or
+    its determinant is not positive."""
+    a = np.asarray(m, dtype=np.float64)
+    if a.shape == (3,):
+        a = np.diag(a)
+    if a.shape != (3, 3):
+        raise ValueError(f"supercell_matrix must be a 3x3 matrix or a 3-vector, got shape {list(a.shape)}")
+    if not np.all(np.isfinite(a)) or np.any(a != np.round(a)):
+        raise ValueError(f"supercell_matrix must be integral, got {a.tolist()}")
+    mi = np.round(a).astype(np.int64)
+    if round(np.linalg.det(mi)) <= 0:
+        raise ValueError(f"supercell_matrix must have a positive determinant, got {mi.tolist()}")
+    return mi
+
+
+def lattice_points(m: np.ndarray) -> np.ndarray:
+    """[det M, 3] integer vectors n (primitive fractional coordinates) with n M^-1 in [0,1)^3, origin first."""
+    det = int(round(np.linalg.det(m)))
+    adj = np.round(np.linalg.inv(m) * det).astype(np.int64)  # det M^-1, integral
+    corners = np.array(list(itertools.product((0, 1), repeat=3))) @ m
+    axes = [np.arange(corners[:, i].min(), corners[:, i].max() + 1) for i in range(3)]
+    n = np.array(np.meshgrid(*axes, indexing="ij")).reshape(3, -1).T
+    x = n @ adj  # det * (n M^-1), exact
+    n = n[np.all((x >= 0) & (x < det), axis=1)]
+    n = n[np.lexsort((n[:, 2], n[:, 1], n[:, 0], np.abs(n).sum(axis=1)))]
+    assert len(n) == det and not n[0].any()
+    return n
+
+
+def _reduce_basis(b: np.ndarray) -> np.ndarray:
+    """Unimodular U with U b pairwise reduced (|b_i . b_j| <= |b_j|^2 / 2): every step shortens a vector."""
+    b, u = b.copy(), np.eye(3, dtype=np.int64)
+    for _ in range(1000):
+        changed = False
+        for i, j in itertools.permutations(range(3), 2):
+            mu = int(np.round(b[i] @ b[j] / (b[j] @ b[j])))
+            if mu:
+                b[i] -= mu * b[j]
+                u[i] -= mu * u[j]
+                changed = True
+        if not changed:
+            return u
+    raise RuntimeError("supercell basis reduction did not converge")
+
+
+def minimum_images(frac_sc: np.ndarray, p2s: np.ndarray, m: np.ndarray, lattice: np.ndarray):
+    """Minimum images of r_j - r_p2s[k] over the supercell lattice, for every primitive atom k and supercell atom j.
+
+    Returns the CSR ``(img_ptr [n_prim N + 1] int32, img_vec [n_img, 3] fp64)``: the images of pair (k, j) are the rows
+    ``img_ptr[k N + j] : img_ptr[k N + j + 1]`` of ``img_vec``, in primitive fractional coordinates, every image whose
+    length is within ``IMAGE_TOL`` of the shortest.  The search runs in a reduced supercell basis over every lattice
+    vector that could be that short, so skewed supercells lose no image."""
+    s = m @ lattice
+    u = _reduce_basis(s.astype(np.float64))
+    red = u @ s  # reduced supercell basis (Cartesian rows)
+    red_m = u @ m  # the same in primitive fractional coordinates
+    to_red = np.linalg.inv(u.astype(np.float64))  # supercell frac -> reduced frac
+    n_super = len(frac_sc)
+    ptr, vecs = [0], []
+    d_red = [None] * len(p2s)
+    for k, k0 in enumerate(p2s):
+        d = (frac_sc - frac_sc[k0]) @ to_red
+        d_red[k] = d - np.round(d)  # nearest copy in the reduced cell
+    # |m_i| <= (|d'| + |d|) |column i of red^-1| for any image d' = d + m red no longer than d
+    longest = max(float(np.linalg.norm(d @ red, axis=1).max()) for d in d_red)
+    reach = np.ceil((2 * longest + IMAGE_TOL) * np.linalg.norm(np.linalg.inv(red), axis=0)).astype(int)
+    cand = np.array(list(itertools.product(*[range(-r, r + 1) for r in reach])), dtype=np.float64)
+    for k in range(len(p2s)):
+        v = d_red[k][:, None, :] + cand[None, :, :]  # [N, C, 3] reduced frac
+        length = np.linalg.norm(v @ red, axis=2)
+        keep = length <= length.min(axis=1, keepdims=True) + IMAGE_TOL
+        counts = keep.sum(axis=1)
+        vecs.append(v[keep] @ red_m)  # row-major: j ascending, candidates in a fixed order
+        ptr.extend(ptr[-1] + np.cumsum(counts))
+    img_ptr = np.asarray(ptr, dtype=np.int64)
+    assert len(img_ptr) == len(p2s) * n_super + 1
+    if img_ptr[-1] >= 2**31:
+        raise ValueError("minimum-image table too large")
+    return img_ptr.astype(np.int32), np.ascontiguousarray(np.concatenate(vecs), dtype=np.float64)
+
+
+@dataclass
+class Supercell:
+    """A supercell in atom-major order: atom j = k n_cells + l sits at r_k + R_l (modulo the supercell lattice)."""
+
+    z: np.ndarray  # [N] int32
+    frac: np.ndarray  # [N,3] supercell fractional coordinates, wrapped into [0,1)
+    lattice: np.ndarray  # [3,3] M @ primitive lattice
+    matrix: np.ndarray  # [3,3] int M
+    points: np.ndarray  # [n_cells,3] int lattice points R_l in primitive fractional coordinates, origin first
+    s2p: np.ndarray  # [N] primitive atom of each supercell atom
+    p2s: np.ndarray  # [n_prim] the l = 0 supercell atom of each primitive atom
+    prim_z: np.ndarray
+    prim_frac: np.ndarray
+    prim_lattice: np.ndarray
+    img_ptr: np.ndarray  # minimum-image CSR (minimum_images)
+    img_vec: np.ndarray
+
+    @property
+    def multiplicities(self) -> np.ndarray:
+        """[n_prim, N] number of minimum images of each pair."""
+        return np.diff(self.img_ptr).reshape(len(self.p2s), len(self.s2p))
+
+
+def make_supercell(z, frac, lattice, matrix) -> Supercell:
+    """Supercell of the primitive cell ``(z, frac, lattice)`` for the integer ``matrix`` (3x3, or a 3-vector meaning a
+    diagonal): lattice ``M @ lattice``; atom j = k n_cells + l is primitive atom k moved by lattice point l."""
+    m = supercell_matrix(matrix)
+    z = np.asarray(z, dtype=np.int32).reshape(-1)
+    frac = np.asarray(frac, dtype=np.float64).reshape(-1, 3)
+    lattice = np.asarray(lattice, dtype=np.float64).reshape(3, 3)
+    pts = lattice_points(m)
+    n_prim, n_cells = len(z), len(pts)
+    sc_frac = ((frac[:, None, :] + pts[None, :, :]) @ np.linalg.inv(m.astype(np.float64))).reshape(-1, 3)
+    sc_frac = sc_frac - np.floor(sc_frac)
+    s2p = np.repeat(np.arange(n_prim), n_cells).astype(np.int32)
+    p2s = (np.arange(n_prim) * n_cells).astype(np.int32)
+    img_ptr, img_vec = minimum_images(sc_frac, p2s, m, lattice)
+    return Supercell(z=np.repeat(z, n_cells), frac=sc_frac, lattice=m @ lattice, matrix=m, points=pts, s2p=s2p,
+                     p2s=p2s, prim_z=z, prim_frac=frac, prim_lattice=lattice, img_ptr=img_ptr, img_vec=img_vec)
+
+
+def compact_force_constants(hvp, sc: Supercell) -> np.ndarray:
+    """Compact force constants ``[n_prim, N, 3, 3]`` in eV/A^2: Phi[k, j, a, b] = (H e_{p2s[k], a})[j, b], H the
+    supercell Hessian.  ``hvp(v [K,N,3]) -> [K,N,3]`` computes H v for K directions; it is called once, with the
+    3 n_prim unit directions on the ``p2s`` atoms."""
+    n_prim, n = len(sc.p2s), len(sc.s2p)
+    v = np.zeros((n_prim, 3, n, 3))
+    for a in range(3):
+        v[np.arange(n_prim), a, sc.p2s, a] = 1.0
+    cols = np.asarray(hvp(v.reshape(3 * n_prim, n, 3)), dtype=np.float64)
+    return np.ascontiguousarray(cols.reshape(n_prim, 3, n, 3).transpose(0, 2, 1, 3))
+
+
+def acoustic_sum_rule(fc: np.ndarray, p2s: np.ndarray) -> tuple[np.ndarray, float]:
+    """Copy of ``fc`` with the self-term correction Phi(k0, k0) -= sum_j Phi(k0, j), and the largest entry of the
+    correction (eV/A^2)."""
+    corr = fc.sum(axis=1)  # [n_prim, 3, 3]
+    out = fc.copy()
+    out[np.arange(len(p2s)), p2s] -= corr
+    return out, float(np.abs(corr).max()) if corr.size else 0.0
+
+
+def thermal_properties_from_frequencies(freqs, temperatures) -> dict:
+    """Harmonic thermodynamics per primitive cell from the frequencies ``[Q, 3 n_prim]`` (THz) of a uniform q mesh.
+
+    Modes with nu < 1e-3 THz are left out (acoustic modes at Gamma and imaginary modes); ``n_imaginary`` counts the
+    modes below -1e-3 THz.  ``free_energy`` F = ZPE + k T sum ln(1 - e^-x) and ``zero_point_energy`` sum h nu / 2 in
+    eV, ``entropy`` k sum [x / (e^x - 1) - ln(1 - e^-x)] and ``heat_capacity`` (C_v) k sum x^2 e^x / (e^x - 1)^2 in
+    eV/K, with x = h nu / k T and every sum divided by Q."""
+    nu = np.asarray(freqs, dtype=np.float64)
+    n_q = nu.shape[0] if nu.ndim > 1 else 1
+    nu = nu.reshape(-1)
+    e = H_EV_PER_THZ * nu[nu >= THERMAL_CUTOFF_THZ]
+    temps = np.atleast_1d(np.asarray(temperatures, dtype=np.float64))
+    zpe = 0.5 * float(e.sum()) / n_q
+    f, s, c = np.full(len(temps), zpe), np.zeros(len(temps)), np.zeros(len(temps))
+    for i, t in enumerate(temps):
+        if t <= 0:
+            continue
+        x = e / (KB * t)
+        em = np.exp(-x)
+        ln = np.log1p(-em)
+        f[i] = zpe + KB * t * float(ln.sum()) / n_q
+        s[i] = KB * float((x * em / -np.expm1(-x) - ln).sum()) / n_q
+        c[i] = KB * float((x * x * em / np.expm1(-x) ** 2).sum()) / n_q
+    return {"temperatures": temps, "free_energy": f, "entropy": s, "heat_capacity": c, "zero_point_energy": zpe,
+            "n_imaginary": int((nu < -THERMAL_CUTOFF_THZ).sum())}
+
+
+def gamma_mesh(mesh) -> np.ndarray:
+    """[n1 n2 n3, 3] reduced q-points (i/n1, j/n2, k/n3) of a full Gamma-centred mesh."""
+    mesh = np.asarray(mesh, dtype=np.int64).reshape(-1)
+    if mesh.shape != (3,) or np.any(mesh < 1):
+        raise ValueError(f"mesh must be three positive integers, got {mesh.tolist()}")
+    axes = [np.arange(n) / n for n in mesh]
+    return np.array(np.meshgrid(*axes, indexing="ij")).reshape(3, -1).T.copy()
+
+
+class Phonons:
+    """Harmonic phonons of a crystal from its compact supercell force constants (``CHGNet.phonons``).
+
+    Attributes: ``force_constants`` ``[n_prim, N, 3, 3]`` eV/A^2 as computed (not symmetrised), relative to
+    ``supercell`` = ``(z, frac, lattice)``; ``p2s`` / ``s2p`` the atom maps (supercell atom j = k n_cells + l);
+    ``asr_correction`` the largest entry of the acoustic-sum-rule correction (eV/A^2); ``masses`` of the primitive
+    atoms (amu, ``chgnet_b200.dynamics.ATOMIC_MASSES``).
+
+    D(q) follows phonopy: the phase of the full interatomic vector r_j - r_k (basis offsets included) over the minimum
+    images of the supercell, each weighted by 1 / multiplicity; built from the force constants with the self-term
+    acoustic-sum-rule correction Phi(k0, k0) -= sum_j Phi(k0, j), made Hermitian as (D + D^H)/2.  ``kernels`` is the
+    object whose ``dynamical_matrices`` builds D (default: the CUDA kernels on ``device``)."""
+
+    # D(q) chunks stay below this many bytes (complex128)
+    chunk_bytes = 1 << 28
+
+    def __init__(self, force_constants: np.ndarray, sc: Supercell, *, device="cuda", kernels=None) -> None:
+        if kernels is None:
+            from chgnet_b200._lib import CudaKernels
+
+            kernels = CudaKernels(device)
+        self.kernels, self.device = kernels, torch.device(device)
+        self.force_constants = np.asarray(force_constants, dtype=np.float64)
+        n_prim, n = len(sc.p2s), len(sc.s2p)
+        if self.force_constants.shape != (n_prim, n, 3, 3):
+            raise ValueError(f"force constants must have shape {[n_prim, n, 3, 3]}, got {list(self.force_constants.shape)}")
+        self.cell = sc
+        self.supercell = (sc.z, sc.frac, sc.lattice)
+        self.p2s, self.s2p = sc.p2s, sc.s2p
+        self.masses = ATOMIC_MASSES[sc.prim_z - 1]
+        fc, self.asr_correction = acoustic_sum_rule(self.force_constants, sc.p2s)
+        dev = self.device
+        self._fc = torch.as_tensor(fc).to(dev)
+        self._img_ptr = torch.as_tensor(sc.img_ptr).to(dev)
+        self._img_vec = torch.as_tensor(sc.img_vec).to(dev)
+        self._s2p = torch.as_tensor(sc.s2p).to(dev)
+        self._inv_sqrt_m = torch.as_tensor(1.0 / np.sqrt(self.masses)).to(dev)
+
+    def dynamical_matrices(self, qpoints) -> torch.Tensor:
+        """D(q) ``[Q, 3 n_prim, 3 n_prim]`` complex128 on the device, in eV/(A^2 amu), for reduced ``qpoints [Q,3]``."""
+        q = torch.as_tensor(np.ascontiguousarray(np.asarray(qpoints, dtype=np.float64).reshape(-1, 3))).to(self.device)
+        n3 = 3 * len(self.p2s)
+        d = torch.empty(q.shape[0], n3, n3, dtype=torch.complex128, device=self.device)
+        self.kernels.dynamical_matrices(self._fc, self._img_ptr, self._img_vec, self._s2p, self._inv_sqrt_m, q, d)
+        return d
+
+    def frequencies(self, qpoints, *, eigenvectors: bool = False):
+        """Frequencies ``[Q, 3 n_prim]`` in THz at the reduced ``qpoints`` (``[Q,3]`` or ``[3]``), ascending per q;
+        an imaginary mode (negative eigenvalue of D) is given as a negative number, nu = sign(lambda) sqrt|lambda|
+        x 15.633304 THz.  With ``eigenvectors``, also ``[Q, 3 n_prim, 3 n_prim]`` complex128 whose column m is the unit
+        eigenvector of mode m (phonopy's layout and phase convention).  D is built and diagonalised on the device in
+        chunks of q that keep it below ``chunk_bytes``.  The force constants should come from a relaxed structure:
+        otherwise the modes describe the curvature at a non-stationary point, and unstable modes appear as imaginary
+        frequencies rather than being hidden."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = q.reshape(-1, 3)
+        n3 = 3 * len(self.p2s)
+        chunk = max(1, self.chunk_bytes // (16 * n3 * n3))
+        freqs = np.empty((len(q), n3))
+        vecs = np.empty((len(q), n3, n3), dtype=np.complex128) if eigenvectors else None
+        for s in range(0, len(q), chunk):
+            d = self.dynamical_matrices(q[s : s + chunk])
+            if eigenvectors:
+                w, v = torch.linalg.eigh(d)
+                vecs[s : s + chunk] = v.cpu().numpy()
+            else:
+                w = torch.linalg.eigvalsh(d)
+            freqs[s : s + chunk] = (torch.sign(w) * torch.sqrt(torch.abs(w)) * THZ_PER_SQRT_EV_A2_AMU).cpu().numpy()
+        if single:
+            freqs = freqs[0]
+            vecs = None if vecs is None else vecs[0]
+        return (freqs, vecs) if eigenvectors else freqs
+
+    def thermal_properties(self, mesh, temperatures) -> dict:
+        """Harmonic thermodynamics per primitive cell on a full Gamma-centred ``mesh`` (n1, n2, n3) at ``temperatures``
+        (K): ``free_energy`` and ``zero_point_energy`` in eV, ``entropy`` and ``heat_capacity`` (C_v) in eV/K, and
+        ``n_imaginary``, the number of modes below -1e-3 THz over the mesh.  Modes with nu < 1e-3 THz are left out of
+        the sums (``thermal_properties_from_frequencies``)."""
+        return thermal_properties_from_frequencies(self.frequencies(gamma_mesh(mesh)), temperatures)

@@ -540,6 +540,17 @@ int chg_edge_tangent_bwd_virial(const float* rvec, const float* dist, const floa
                                 const int32_t* center, const int32_t* nbr, const int32_t* atom_owner,
                                 int32_t n_edges, double* force, double* virial, void* stream);
 
+/* ======================= phonons (CHGNet.phonons) =======================
+ * dyn [n_q][3 n_prim][3 n_prim] interleaved complex128 (written in full, Hermitian: (D + D^H)/2) with
+ *   D(q)[k a, k' b] = sum_{j : s2p[j] = k'} fc[k][j][a][b] (1/m_kj) sum_{v} e^{2 pi i q.v} inv_sqrt_m[k] inv_sqrt_m[k']
+ * fc [n_prim][n_super][3][3] compact force constants (fp64); the minimum images of pair (k, j) are the rows
+ * img_vec[img_ptr[k n_super + j] .. img_ptr[k n_super + j + 1]) [][3], r_j - r_k + T in primitive fractional
+ * coordinates, m_kj their number; s2p [n_super] primitive atom of each supercell atom; inv_sqrt_m [n_prim];
+ * qpoints [n_q][3] reduced coordinates (fp64).  Deterministic (no atomics); at most 65535 * 128 q-points per call. */
+int chg_dynamical_matrices(const double* fc, const int32_t* img_ptr, const double* img_vec, const int32_t* s2p,
+                           const double* inv_sqrt_m, int32_t n_prim, int32_t n_super, const double* qpoints,
+                           int32_t n_q, double* dyn, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
