@@ -68,7 +68,12 @@ SIGNATURES: dict[str, list] = {
     "chg_edge_tangent_bwd_virial": [P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P],
     # phonons
     "chg_dynamical_matrices": [P, P, P, P, P, I, I, P, I, P, P],
+    "chg_dynamical_matrix_derivatives": [P, P, P, P, P, I, I, P, I, P, P, P],
+    "chg_tetrahedron_dos": [P, I, I, I, I, P, P, I, P, I, P, P, P, P, P],
 }
+
+# CHG_DOS_MAX_CHUNKS of include/chgnet_b200.h: chg_tetrahedron_dos needs this many (2 + n_proj) x n_freq scratch rows
+DOS_MAX_CHUNKS = 512
 
 _lib = None
 
@@ -366,6 +371,45 @@ class CudaKernels:
             raise ChgnetB200Error("dynamical_matrices: fc and qpoints must be float64, dyn complex128")
         self._call("chg_dynamical_matrices", _p(fc), _p(img_ptr), _p(img_vec), _p(s2p), _p(inv_sqrt_m), fc.shape[0],
                    fc.shape[1], _p(qpoints), qpoints.shape[0], _p(dyn))
+
+    def dynamical_matrix_derivatives(self, fc, img_ptr, img_vec, s2p, inv_sqrt_m, qpoints, prim_lattice, ddyn):
+        """ddyn [Q, 3, 3n, 3n] complex128 (overwritten) = dD/dQ_c, Q = q inv(prim_lattice)^T (1/A, no 2 pi), for the
+        arguments of ``dynamical_matrices`` and the primitive lattice [3, 3] (fp64, rows are lattice vectors, A)."""
+        self._chk(fc, img_ptr, img_vec, s2p, inv_sqrt_m, qpoints, prim_lattice, ddyn)
+        if (ddyn.dtype != torch.complex128 or fc.dtype != torch.float64 or qpoints.dtype != torch.float64
+                or prim_lattice.dtype != torch.float64):
+            raise ChgnetB200Error("dynamical_matrix_derivatives: fc, qpoints and prim_lattice must be float64, "
+                                  "ddyn complex128")
+        n3 = 3 * fc.shape[0]
+        if tuple(prim_lattice.shape) != (3, 3) or tuple(ddyn.shape) != (qpoints.shape[0], 3, n3, n3):
+            raise ChgnetB200Error(f"dynamical_matrix_derivatives: prim_lattice must be [3, 3] and ddyn "
+                                  f"[{qpoints.shape[0]}, 3, {n3}, {n3}]")
+        self._call("chg_dynamical_matrix_derivatives", _p(fc), _p(img_ptr), _p(img_vec), _p(s2p), _p(inv_sqrt_m),
+                   fc.shape[0], fc.shape[1], _p(qpoints), qpoints.shape[0], _p(prim_lattice), _p(ddyn))
+
+    def tetrahedron_dos(self, freqs, mesh, tetrahedra, omega, dos, idos, proj=None, pdos=None):
+        """Linear tetrahedron DOS on the full Gamma-centred ``mesh`` (n1, n2, n3): freqs [n1 n2 n3, n_band] fp64
+        (ascending per q), tetrahedra [6, 4, 3] int32 corner offsets, omega [F] fp64; writes dos [F], idos [F] and,
+        with proj [n1 n2 n3, n_band, S], pdos [S, F] (all fp64)."""
+        self._chk(freqs, tetrahedra, omega, dos, idos, proj, pdos)
+        n1, n2, n3 = (int(n) for n in mesh)
+        n_q, n_band = freqs.shape
+        f64 = torch.float64
+        if any(t is not None and t.dtype != f64 for t in (freqs, omega, dos, idos, proj, pdos)):
+            raise ChgnetB200Error("tetrahedron_dos: freqs, omega, proj and the outputs must be float64")
+        if tetrahedra.dtype != torch.int32 or tuple(tetrahedra.shape) != (6, 4, 3):
+            raise ChgnetB200Error("tetrahedron_dos: tetrahedra must be int32 [6, 4, 3]")
+        n_f = omega.shape[0]
+        if n_q != n1 * n2 * n3 or tuple(dos.shape) != (n_f,) or tuple(idos.shape) != (n_f,):
+            raise ChgnetB200Error(f"tetrahedron_dos: freqs must be [{n1 * n2 * n3}, n_band], dos and idos [{n_f}]")
+        n_proj = 0
+        if proj is not None:
+            n_proj = proj.shape[2]
+            if tuple(proj.shape[:2]) != (n_q, n_band) or pdos is None or tuple(pdos.shape) != (n_proj, n_f):
+                raise ChgnetB200Error(f"tetrahedron_dos: proj must be [{n_q}, {n_band}, S] and pdos [S, {n_f}]")
+        work = torch.empty(DOS_MAX_CHUNKS * (2 + n_proj) * max(n_f, 1), dtype=f64, device=freqs.device)
+        self._call("chg_tetrahedron_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(proj), n_proj, _p(omega),
+                   n_f, _p(dos), _p(idos), _p(pdos if proj is not None else None), _p(work))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

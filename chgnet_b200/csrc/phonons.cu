@@ -8,6 +8,14 @@
 // phase tensor never exists.  One thread per (q, unordered pair {k, k'}): it sums the blocks (k, k') and (k', k) in
 // fp64, in a fixed order, and writes both 3x3 blocks of the Hermitian part (D + D^H)/2.  No atomics: the result is
 // bitwise reproducible.
+//
+// The same sum with every image term multiplied by 2 pi i r_c, r = v . prim_lattice the Cartesian image vector (A), is
+// dD/dQ_c, the derivative with respect to the Cartesian wave vector Q = q . inv(prim_lattice)^T (no 2 pi; q.v = Q.r):
+// the group velocities of Phonons.group_velocities.  One more grid dimension runs over c.
+//
+// chg_tetrahedron_dos: the linear tetrahedron method (Bloechl's closed forms) on a full Gamma-centred mesh, see below.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace chg {
@@ -15,11 +23,13 @@ namespace {
 
 constexpr int DYN_THREADS = 128;  // q-points per block
 
-// re / im [3][3] = sum_{j : s2p[j] = kp} Phi[k, j] (1/m) sum_images e^{2 pi i q.v}
+// re / im [3][3] = sum_{j : s2p[j] = kp} Phi[k, j] (1/m) sum_images e^{2 pi i q.v}, times 2 pi i r_c per image with
+// DERIV (r_c = v . (l0, l1, l2), the column c of the primitive lattice)
+template <bool DERIV>
 __device__ __forceinline__ void phase_block(const double* __restrict__ fc, const int32_t* __restrict__ img_ptr,
                                             const double* __restrict__ img_vec, const int32_t* __restrict__ s2p,
                                             int n_super, int k, int kp, double q0, double q1, double q2,
-                                            double (&re)[9], double (&im)[9]) {
+                                            double l0, double l1, double l2, double (&re)[9], double (&im)[9]) {
 #pragma unroll
   for (int i = 0; i < 9; ++i) re[i] = im[i] = 0.0;
   // every thread of a block has the same (k, kp): the branch and the loads below are uniform across the warp
@@ -33,10 +43,21 @@ __device__ __forceinline__ void phase_block(const double* __restrict__ fc, const
       const double* v = img_vec + (size_t)t * 3;
       double sn, cs;
       sincospi(2.0 * fma(q0, __ldg(v), fma(q1, __ldg(v + 1), q2 * __ldg(v + 2))), &sn, &cs);
-      c += cs;
-      s += sn;
+      if constexpr (DERIV) {
+        const double r = fma(__ldg(v), l0, fma(__ldg(v + 1), l1, __ldg(v + 2) * l2));
+        c = fma(-r, sn, c);  // Re(i r e^{i phi})
+        s = fma(r, cs, s);
+      } else {
+        c += cs;
+        s += sn;
+      }
     }
-    const double inv_m = 1.0 / (double)(e - b);
+    double inv_m;
+    if constexpr (DERIV) {
+      inv_m = 6.283185307179586 / (double)(e - b);  // 2 pi
+    } else {
+      inv_m = 1.0 / (double)(e - b);
+    }
     c *= inv_m;
     s *= inv_m;
     const double* f = fc + pair * 9;
@@ -49,27 +70,36 @@ __device__ __forceinline__ void phase_block(const double* __restrict__ fc, const
   }
 }
 
+// D(q) [n_q][3n][3n], or with DERIV dD/dQ_c [n_q][3][3n][3n] (c = blockIdx.z, lattice the primitive lattice [3][3])
+template <bool DERIV>
 __global__ void __launch_bounds__(DYN_THREADS)
 dynamical_matrices_kernel(const double* __restrict__ fc, const int32_t* __restrict__ img_ptr,
                           const double* __restrict__ img_vec, const int32_t* __restrict__ s2p,
                           const double* __restrict__ inv_sqrt_m, int n_prim, int n_super,
-                          const double* __restrict__ qpoints, int n_q, double* __restrict__ dyn) {
+                          const double* __restrict__ qpoints, int n_q, const double* __restrict__ lattice,
+                          double* __restrict__ dyn) {
   const int k = blockIdx.x / n_prim, kp = blockIdx.x % n_prim;
   if (kp < k) return;  // block (kp, k) writes this pair
   const int iq = blockIdx.y * DYN_THREADS + threadIdx.x;
   if (iq >= n_q) return;
   const double q0 = qpoints[iq * 3], q1 = qpoints[iq * 3 + 1], q2 = qpoints[iq * 3 + 2];
+  double l0 = 0.0, l1 = 0.0, l2 = 0.0;
+  if constexpr (DERIV) {
+    const int c = blockIdx.z;
+    l0 = lattice[c], l1 = lattice[3 + c], l2 = lattice[6 + c];
+  }
   double r1[9], i1[9], r2[9], i2[9];
-  phase_block(fc, img_ptr, img_vec, s2p, n_super, k, kp, q0, q1, q2, r1, i1);
+  phase_block<DERIV>(fc, img_ptr, img_vec, s2p, n_super, k, kp, q0, q1, q2, l0, l1, l2, r1, i1);
   if (kp != k) {
-    phase_block(fc, img_ptr, img_vec, s2p, n_super, kp, k, q0, q1, q2, r2, i2);
+    phase_block<DERIV>(fc, img_ptr, img_vec, s2p, n_super, kp, k, q0, q1, q2, l0, l1, l2, r2, i2);
   } else {
 #pragma unroll
     for (int i = 0; i < 9; ++i) r2[i] = r1[i], i2[i] = i1[i];
   }
   const double w = 0.5 * inv_sqrt_m[k] * inv_sqrt_m[kp];
   const size_t n3 = 3 * (size_t)n_prim;
-  double* dq = dyn + (size_t)iq * n3 * n3 * 2;
+  const size_t mat = DERIV ? (size_t)iq * 3 + blockIdx.z : (size_t)iq;
+  double* dq = dyn + mat * n3 * n3 * 2;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
 #pragma unroll
@@ -87,22 +117,221 @@ dynamical_matrices_kernel(const double* __restrict__ fc, const int32_t* __restri
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Linear tetrahedron method.  Mesh cell (i, j, k) of the Gamma-centred mesh (q index (i n2 + j) n3 + k) is cut into 6
+// tetrahedra given by corner offsets tet[6][4][3] in {0, 1} (periodic wrap); each band is interpolated linearly on
+// each tetrahedron.  For sorted vertex values e0 <= e1 <= e2 <= e3 and the interpolant e(x), per unit volume:
+//   n(w) = vol{e <= w},  g(w) = dn/dw = int delta(w - e),  wt_i(w) = int delta(w - e) lambda_i  (sum_i wt_i = g),
+// lambda_i the barycentric coordinates.  The cross-section e = w is a triangle (w < e1, w >= e2) or a quadrilateral;
+// wt_i / g is the lambda_i of its centroid.  With f_ij = (w - e_j) / (e_i - e_j):
+//   e0 <= w < e1:  n = f10 f20 f30,  g = 3 f10 f20 / e30,  wt_j = g f_j0 / 3 (j > 0)
+//   e1 <= w < e2:  n (Bloechl) = [e10^2 + 3 e10 x + 3 x^2 - (e20 + e31) x^3 / (e21 e31)] / (e20 e30), x = w - e1;
+//                  g = 3 (f12 f20 + f21 f13) / e30.  The diagonal f02-f13 cuts the quadrilateral into triangles whose
+//                  areas are g (1 - s) and g s, g s = 3 f13 f20 / e30, so wt_0 = (g f02 + gs f03) / 3,
+//                  wt_1 = (g f13 + (g - gs) f12) / 3, wt_2 = (g f20 + (g - gs) f21) / 3, wt_3 = (g f31 + gs f30) / 3
+//   e2 <= w < e3:  n = 1 - f03 f13 f23,  g = 3 f03 f13 / e32,  wt_i = g f_i3 / 3 (i < 3)
+// and in each triangle case the remaining vertex takes g - the others.  The half-open intervals keep every divisor
+// non-zero, whatever values coincide.
+constexpr int DOS_MAX_THREADS = 256;  // frequency points per block, and pairs staged per tile
+constexpr int DOS_PROJ = 4;           // projection columns per block (grid z)
+
+__device__ __forceinline__ bool tetra_weights(double w, const double (&e)[4], double& n, double& g, double (&wt)[4]) {
+  if (w >= e[3]) {
+    n = 1.0;
+    return false;
+  }
+  if (w < e[1]) {
+    const double f10 = (w - e[0]) / (e[1] - e[0]), f20 = (w - e[0]) / (e[2] - e[0]), f30 = (w - e[0]) / (e[3] - e[0]);
+    n = f10 * f20 * f30;
+    g = 3.0 * f10 * f20 / (e[3] - e[0]);
+    const double g3 = g * (1.0 / 3.0);
+    wt[1] = g3 * f10, wt[2] = g3 * f20, wt[3] = g3 * f30;
+    wt[0] = g - wt[1] - wt[2] - wt[3];
+  } else if (w < e[2]) {
+    const double e10 = e[1] - e[0], e20 = e[2] - e[0], e30 = e[3] - e[0], e21 = e[2] - e[1], e31 = e[3] - e[1];
+    const double x = w - e[1];
+    n = (e10 * e10 + 3.0 * e10 * x + 3.0 * x * x - (e20 + e31) * x * x * x / (e21 * e31)) / (e20 * e30);
+    const double f02 = (w - e[2]) / (e[0] - e[2]), f03 = (w - e[3]) / (e[0] - e[3]);
+    const double f12 = (w - e[2]) / (e[1] - e[2]), f13 = (w - e[3]) / (e[1] - e[3]);
+    const double f20 = 1.0 - f02, f30 = 1.0 - f03, f21 = 1.0 - f12, f31 = 1.0 - f13;
+    g = 3.0 * (f12 * f20 + f21 * f13) / e30;
+    const double gs = 3.0 * f13 * f20 / e30, gr = g - gs;
+    wt[0] = (g * f02 + gs * f03) * (1.0 / 3.0);
+    wt[1] = (g * f13 + gr * f12) * (1.0 / 3.0);
+    wt[2] = (g * f20 + gr * f21) * (1.0 / 3.0);
+    wt[3] = (g * f31 + gs * f30) * (1.0 / 3.0);
+  } else {
+    const double f03 = (e[3] - w) / (e[3] - e[0]), f13 = (e[3] - w) / (e[3] - e[1]), f23 = (e[3] - w) / (e[3] - e[2]);
+    n = 1.0 - f03 * f13 * f23;
+    g = 3.0 * f03 * f13 / (e[3] - e[2]);
+    const double g3 = g * (1.0 / 3.0);
+    wt[0] = g3 * f03, wt[1] = g3 * f13, wt[2] = g3 * f23;
+    wt[3] = g - wt[0] - wt[1] - wt[2];
+  }
+  return true;
+}
+
+// One thread per frequency point; block x owns a contiguous range of (tetrahedron, band) pairs, z a group of
+// DOS_PROJ projection columns.  Each tile of pairs is staged, sorted, in shared memory by the block and then read
+// by every thread (broadcasts).  The block's sums go to work[chunk][row][F] (row 0 g, 1 n, 2 + s the projection s),
+// each element written by exactly one thread: no atomics, and dos_reduce_kernel adds the chunks in a fixed order.
+__global__ void __launch_bounds__(DOS_MAX_THREADS)
+tetrahedron_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
+                       const int32_t* __restrict__ tet, const double* __restrict__ proj, int n_proj,
+                       const double* __restrict__ omega, int n_freq, int64_t n_pairs, double* __restrict__ work) {
+  __shared__ double se[DOS_MAX_THREADS][4];
+  __shared__ int32_t sq[DOS_MAX_THREADS][4];
+  __shared__ int32_t sb[DOS_MAX_THREADS];
+  const int f = blockIdx.y * blockDim.x + threadIdx.x;
+  const bool active = f < n_freq;
+  const double w = active ? omega[f] : 0.0;
+  const int s0 = blockIdx.z * DOS_PROJ;
+  const int ns = proj ? min(DOS_PROJ, n_proj - s0) : 0;
+  double acc_g = 0.0, acc_n = 0.0, acc_p[DOS_PROJ];
+#pragma unroll
+  for (int s = 0; s < DOS_PROJ; ++s) acc_p[s] = 0.0;
+  const int64_t tile = blockDim.x;
+  const int64_t n_tiles = (n_pairs + tile - 1) / tile;
+  const int64_t t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  for (int64_t t = n_tiles * blockIdx.x / gridDim.x; t < t_end; ++t) {
+    const int64_t p = t * tile + threadIdx.x;
+    __syncthreads();  // the previous tile has been read
+    if (p < n_pairs) {
+      const int band = (int)(p % n_band);
+      const int64_t tt = p / n_band;
+      const int it = (int)(tt % 6);
+      const int64_t cell = tt / 6;
+      const int ci = (int)(cell / ((int64_t)n2 * n3)), cj = (int)((cell / n3) % n2), ck = (int)(cell % n3);
+      double e[4];
+      int32_t q[4];
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const int32_t* o = tet + (it * 4 + v) * 3;
+        int a = ci + __ldg(o), b = cj + __ldg(o + 1), c = ck + __ldg(o + 2);
+        a -= a >= n1 ? n1 : 0;
+        b -= b >= n2 ? n2 : 0;
+        c -= c >= n3 ? n3 : 0;
+        q[v] = (a * n2 + b) * n3 + c;
+        e[v] = __ldg(freqs + (int64_t)q[v] * n_band + band);
+      }
+      // sorting network, ascending (ties keep a fixed, data-determined order)
+#define CHG_CSWAP(i, j)                      \
+  if (e[j] < e[i]) {                         \
+    const double te = e[i];                  \
+    e[i] = e[j], e[j] = te;                  \
+    const int32_t tq = q[i];                 \
+    q[i] = q[j], q[j] = tq;                  \
+  }
+      CHG_CSWAP(0, 1) CHG_CSWAP(2, 3) CHG_CSWAP(0, 2) CHG_CSWAP(1, 3) CHG_CSWAP(1, 2)
+#undef CHG_CSWAP
+#pragma unroll
+      for (int v = 0; v < 4; ++v) se[threadIdx.x][v] = e[v], sq[threadIdx.x][v] = q[v];
+      sb[threadIdx.x] = band;
+    }
+    __syncthreads();
+    if (!active) continue;
+    const int n_here = (int)min(tile, n_pairs - t * tile);
+    for (int i = 0; i < n_here; ++i) {
+      const double e[4] = {se[i][0], se[i][1], se[i][2], se[i][3]};
+      if (w < e[0]) continue;
+      double n, g, wt[4];
+      const bool inside = tetra_weights(w, e, n, g, wt);
+      acc_n += n;
+      if (!inside) continue;
+      acc_g += g;
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const double* pv = proj + ((int64_t)sq[i][v] * n_band + sb[i]) * n_proj + s0;
+#pragma unroll
+        for (int s = 0; s < DOS_PROJ; ++s)
+          if (s < ns) acc_p[s] = fma(wt[v], __ldg(pv + s), acc_p[s]);
+      }
+    }
+  }
+  if (!active) return;
+  const int rows = 2 + (proj ? n_proj : 0);
+  double* out = work + (size_t)blockIdx.x * rows * n_freq + f;
+  if (blockIdx.z == 0) {
+    out[0] = acc_g;
+    out[n_freq] = acc_n;
+  }
+#pragma unroll
+  for (int s = 0; s < DOS_PROJ; ++s)
+    if (s < ns) out[(size_t)(2 + s0 + s) * n_freq] = acc_p[s];
+}
+
+// out[row][f] = scale * sum over chunks (in chunk order) of work[chunk][row][f]
+__global__ void dos_reduce_kernel(const double* __restrict__ work, int n_chunks, int rows, int n_freq, double scale,
+                                  double* __restrict__ dos, double* __restrict__ idos, double* __restrict__ pdos) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)rows * n_freq) return;
+  const int r = (int)(idx / n_freq), f = (int)(idx % n_freq);
+  double acc = 0.0;
+  for (int c = 0; c < n_chunks; ++c) acc += work[((size_t)c * rows + r) * n_freq + f];
+  double* out = r == 0 ? dos : (r == 1 ? idos : pdos + (size_t)(r - 2) * n_freq);
+  out[f] = acc * scale;
+}
+
 }  // namespace
 }  // namespace chg
 
 using namespace chg;
 
+#define CHG_DYN_CHECKS()                                                                     \
+  CHG_CHECK_ARG(n_prim >= 0 && n_super >= 0 && n_q >= 0, "negative size");                   \
+  if (n_prim == 0 || n_q == 0) return CHG_OK;                                                \
+  CHG_CHECK_ARG(fc && img_ptr && img_vec && s2p && inv_sqrt_m && qpoints && dyn, "null pointer"); \
+  CHG_CHECK_ARG((int64_t)n_prim * n_prim < (1ll << 31), "too many primitive atoms");         \
+  const int64_t q_blocks = ((int64_t)n_q + DYN_THREADS - 1) / DYN_THREADS;                    \
+  CHG_CHECK_ARG(q_blocks <= 65535, "too many q-points in one call (at most 65535 * 128)")
+
 extern "C" int chg_dynamical_matrices(const double* fc, const int32_t* img_ptr, const double* img_vec,
                                       const int32_t* s2p, const double* inv_sqrt_m, int32_t n_prim, int32_t n_super,
                                       const double* qpoints, int32_t n_q, double* dyn, void* stream) {
-  CHG_CHECK_ARG(n_prim >= 0 && n_super >= 0 && n_q >= 0, "negative size");
-  if (n_prim == 0 || n_q == 0) return CHG_OK;
-  CHG_CHECK_ARG(fc && img_ptr && img_vec && s2p && inv_sqrt_m && qpoints && dyn, "null pointer");
-  CHG_CHECK_ARG((int64_t)n_prim * n_prim < (1ll << 31), "too many primitive atoms");
-  const int64_t q_blocks = ((int64_t)n_q + DYN_THREADS - 1) / DYN_THREADS;
-  CHG_CHECK_ARG(q_blocks <= 65535, "too many q-points in one call (at most 65535 * 128)");
+  CHG_DYN_CHECKS();
   const dim3 grid((unsigned)(n_prim * n_prim), (unsigned)q_blocks);
-  dynamical_matrices_kernel<<<grid, DYN_THREADS, 0, as_stream(stream)>>>(fc, img_ptr, img_vec, s2p, inv_sqrt_m,
-                                                                          n_prim, n_super, qpoints, n_q, dyn);
+  dynamical_matrices_kernel<false><<<grid, DYN_THREADS, 0, as_stream(stream)>>>(
+      fc, img_ptr, img_vec, s2p, inv_sqrt_m, n_prim, n_super, qpoints, n_q, nullptr, dyn);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_dynamical_matrix_derivatives(const double* fc, const int32_t* img_ptr, const double* img_vec,
+                                                const int32_t* s2p, const double* inv_sqrt_m, int32_t n_prim,
+                                                int32_t n_super, const double* qpoints, int32_t n_q,
+                                                const double* prim_lattice, double* dyn, void* stream) {
+  CHG_DYN_CHECKS();
+  CHG_CHECK_ARG(prim_lattice, "null pointer");
+  const dim3 grid((unsigned)(n_prim * n_prim), (unsigned)q_blocks, 3);
+  dynamical_matrices_kernel<true><<<grid, DYN_THREADS, 0, as_stream(stream)>>>(
+      fc, img_ptr, img_vec, s2p, inv_sqrt_m, n_prim, n_super, qpoints, n_q, prim_lattice, dyn);
+  CHG_LAUNCH_END();
+}
+#undef CHG_DYN_CHECKS
+
+extern "C" int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                                   const int32_t* tetrahedra, const double* proj, int32_t n_proj,
+                                   const double* omega, int32_t n_freq, double* dos, double* idos, double* pdos,
+                                   double* work, void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_freq >= 0 && n_proj >= 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 < (1ll << 31), "mesh too large");
+  if (n_freq == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && tetrahedra && omega && dos && idos && work, "null pointer");
+  CHG_CHECK_ARG(!proj || (pdos && n_proj > 0), "projections need pdos and n_proj > 0");
+  const int64_t n_pairs = (int64_t)n1 * n2 * n3 * 6 * n_band;
+  const int threads = (int)std::min<int64_t>(DOS_MAX_THREADS, ((int64_t)n_freq + 31) / 32 * 32);
+  const int64_t f_blocks = ((int64_t)n_freq + threads - 1) / threads;
+  const int64_t n_tiles = (n_pairs + threads - 1) / threads;
+  const int chunks = (int)std::max<int64_t>(1, std::min<int64_t>(CHG_DOS_MAX_CHUNKS, n_tiles));
+  const int groups = proj ? (n_proj + DOS_PROJ - 1) / DOS_PROJ : 1;
+  CHG_CHECK_ARG(f_blocks <= 65535 && groups <= 65535, "too many frequency points or projections");
+  const int rows = 2 + (proj ? n_proj : 0);
+  tetrahedron_dos_kernel<<<dim3(chunks, (unsigned)f_blocks, groups), threads, 0, as_stream(stream)>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, proj, n_proj, omega, n_freq, n_pairs, work);
+  CHG_CUDA(cudaGetLastError());
+  chg::count_launch();
+  const int64_t n_out = (int64_t)rows * n_freq;
+  const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
+  dos_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, rows, n_freq, scale,
+                                                                                      dos, idos, pdos);
   CHG_LAUNCH_END();
 }

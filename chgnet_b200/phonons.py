@@ -7,10 +7,13 @@
   3 n_prim Hessian-vector products that move the atoms of one primitive cell.  The supercell is periodic in the
   primitive lattice, Phi(k l, k' l') = Phi(k 0, k' (l' - l)), so these columns determine every force constant.
 * ``Phonons``: dynamical matrices D(q) on the device (``chg_dynamical_matrices``, csrc/phonons.cu), frequencies and
-  eigenvectors by ``torch.linalg.eigh``, and harmonic thermodynamics on a Gamma-centred mesh.
+  eigenvectors by ``torch.linalg.eigh``, and harmonic thermodynamics on a Gamma-centred mesh; group velocities from
+  dD/dQ (``chg_dynamical_matrix_derivatives``) and the linear tetrahedron density of states, total and projected on
+  atoms (``chg_tetrahedron_dos``).
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
-eV and eV/K per primitive cell for the thermodynamic functions.
+eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
+primitive cell for densities of states.
 """
 from __future__ import annotations
 
@@ -31,6 +34,8 @@ H_EV_PER_THZ = 6.62607015e-34 / _EV * 1e12  # h nu in eV for nu in THz
 IMAGE_TOL = 1e-5
 # modes below this |nu| (THz) are left out of the thermodynamic sums
 THERMAL_CUTOFF_THZ = 1e-3
+# adjacent modes closer than this (THz) form a degenerate set for the group velocities
+DEGENERACY_THZ = 1e-4
 
 
 def supercell_matrix(m) -> np.ndarray:
@@ -213,6 +218,23 @@ def gamma_mesh(mesh) -> np.ndarray:
     return np.array(np.meshgrid(*axes, indexing="ij")).reshape(3, -1).T.copy()
 
 
+def tetrahedra(mesh, prim_lattice, diagonal=None) -> np.ndarray:
+    """[6, 4, 3] int32 corner offsets (in {0, 1}) of the 6 equal-volume tetrahedra of a cell of the Gamma-centred
+    ``mesh`` that share one body diagonal of the cell: the shortest in Cartesian reciprocal space (phonopy's choice; the
+    first of equal ones), or the one ``diagonal`` (0: 0 -> e1+e2+e3, 1, 2, 3: axis 1, 2, 3 reflected) names.  For the
+    diagonal 0 -> e1+e2+e3 the tetrahedra are {0, e_i, e_i + e_j, e1+e2+e3} over the permutations (i, j, k)."""
+    mesh = np.asarray(mesh, dtype=np.int64).reshape(3)
+    g = np.linalg.inv(np.asarray(prim_lattice, dtype=np.float64)).T / mesh[:, None]  # rows: mesh steps (1/A)
+    flips = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [0, 0, 1]])
+    if diagonal is None:
+        diagonal = int(np.argmin([np.linalg.norm((1 - 2 * f) @ g) for f in flips]))
+    eye = np.eye(3, dtype=np.int64)
+    tets = np.array([[np.zeros(3, np.int64), eye[i], eye[i] + eye[j], np.ones(3, np.int64)]
+                     for i, j, _ in itertools.permutations(range(3))])
+    f = flips[diagonal]
+    return np.ascontiguousarray(np.where(f == 1, 1 - tets, tets), dtype=np.int32)
+
+
 class Phonons:
     """Harmonic phonons of a crystal from its compact supercell force constants (``CHGNet.phonons``).
 
@@ -228,6 +250,8 @@ class Phonons:
 
     # D(q) chunks stay below this many bytes (complex128)
     chunk_bytes = 1 << 28
+    # q-points per batched eigendecomposition in dos and group_velocities (cuSOLVER rejects batches of ~30 000)
+    eigh_batch = 4096
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -250,6 +274,7 @@ class Phonons:
         self._img_vec = torch.as_tensor(sc.img_vec).to(dev)
         self._s2p = torch.as_tensor(sc.s2p).to(dev)
         self._inv_sqrt_m = torch.as_tensor(1.0 / np.sqrt(self.masses)).to(dev)
+        self._lattice = torch.as_tensor(np.ascontiguousarray(sc.prim_lattice, dtype=np.float64)).to(dev)
 
     def dynamical_matrices(self, qpoints) -> torch.Tensor:
         """D(q) ``[Q, 3 n_prim, 3 n_prim]`` complex128 on the device, in eV/(A^2 amu), for reduced ``qpoints [Q,3]``."""
@@ -293,3 +318,92 @@ class Phonons:
         ``n_imaginary``, the number of modes below -1e-3 THz over the mesh.  Modes with nu < 1e-3 THz are left out of
         the sums (``thermal_properties_from_frequencies``)."""
         return thermal_properties_from_frequencies(self.frequencies(gamma_mesh(mesh)), temperatures)
+
+    def group_velocities(self, qpoints) -> np.ndarray:
+        """Group velocities ``[Q, 3 n_prim, 3]`` (``[3 n_prim, 3]`` for one q) in THz*A (100 m/s) at the reduced
+        ``qpoints``: the Cartesian d nu / dQ = d omega / dk of each mode, in the order of ``frequencies(qpoints)``.
+
+        For a non-degenerate mode, v_c = c^2 Re<e|dD/dQ_c|e> / (2 |nu|) with c = ``THZ_PER_SQRT_EV_A2_AMU``: the
+        derivative of the signed frequency, so an imaginary mode (nu < 0) gets the derivative of -c sqrt|lambda|.  In a
+        set of degenerate modes (adjacent |d nu| < ``DEGENERACY_THZ``) component c comes from the ascending eigenvalues
+        of E^H dD/dQ_c E restricted to the set (phonopy's convention); the set's sum does not depend on the basis.
+        Modes with |nu| < ``THERMAL_CUTOFF_THZ`` get 0.  D, dD/dQ (``chg_dynamical_matrix_derivatives``) and the
+        eigenvectors are computed on the device in chunks of q that keep them below ``chunk_bytes``."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = np.ascontiguousarray(q.reshape(-1, 3))
+        n3 = 3 * len(self.p2s)
+        chunk = max(1, min(self.chunk_bytes // (4 * 16 * n3 * n3), self.eigh_batch))  # D and its three derivatives
+        dev, c2 = self.device, THZ_PER_SQRT_EV_A2_AMU**2
+        out = np.empty((len(q), n3, 3))
+        for s in range(0, len(q), chunk):
+            qd = torch.as_tensor(q[s : s + chunk]).to(dev)
+            nq = qd.shape[0]
+            d = torch.empty(nq, n3, n3, dtype=torch.complex128, device=dev)
+            self.kernels.dynamical_matrices(self._fc, self._img_ptr, self._img_vec, self._s2p, self._inv_sqrt_m, qd, d)
+            dd = torch.empty(nq, 3, n3, n3, dtype=torch.complex128, device=dev)
+            self.kernels.dynamical_matrix_derivatives(self._fc, self._img_ptr, self._img_vec, self._s2p,
+                                                      self._inv_sqrt_m, qd, self._lattice, dd)
+            lam, e = torch.linalg.eigh(d)
+            nu = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+            m = e.conj().transpose(1, 2)[:, None] @ dd @ e[:, None]  # [nq, 3, n3, n3]
+            dlam = torch.diagonal(m, dim1=-2, dim2=-1).real.clone()  # [nq, 3, n3]
+            # degenerate sets: set ids ascending along the (ascending) modes
+            gap = (nu[:, 1:] - nu[:, :-1]).abs() >= DEGENERACY_THZ
+            sid = torch.cat([torch.zeros(nq, 1, dtype=torch.long, device=dev), gap.long().cumsum(1)], dim=1)
+            idx = torch.nonzero((~gap).any(dim=1)).flatten()
+            if idx.numel():
+                ids = sid[idx]
+                mb = m[idx] * (ids[:, :, None] == ids[:, None, :])[:, None]  # block diagonal, one block per set
+                # shift set k by k * delta, delta > twice the Gershgorin radius: the ascending eigenvalues of the
+                # shifted matrix come set by set, each set's own eigenvalues in ascending order
+                delta = 2.5 * mb.abs().sum(-1).amax(-1) + torch.finfo(torch.float64).tiny  # [K, 3]
+                shift = ids[:, None, :] * delta[:, :, None]
+                ev = torch.linalg.eigvalsh(mb + torch.diag_embed(shift.to(torch.complex128)))
+                dlam[idx] = ev - shift
+            anu = nu.abs()[:, None, :]
+            v = torch.where(anu >= THERMAL_CUTOFF_THZ, c2 * dlam / (2 * anu.clamp_min(THERMAL_CUTOFF_THZ)), 0.0)
+            out[s : s + chunk] = v.transpose(1, 2).cpu().numpy()
+        return out[0] if single else out
+
+    def dos(self, mesh, frequency_points=None, *, projected: bool = False) -> dict:
+        """Phonon density of states by the linear tetrahedron method on a full Gamma-centred ``mesh`` (n1, n2, n3).
+
+        Returns ``frequency_points`` (THz; default 201 points from the lowest to the highest frequency of the mesh,
+        imaginary modes as negative numbers), ``total_dos`` (states/THz per primitive cell, integrating to 3 n_prim),
+        ``integrated_dos`` and, with ``projected``, ``projected_dos`` [n_prim, F]: the DOS projected on each primitive
+        atom with the weights sum_a |e_(k a)|^2 of the eigenvectors (the projections add up to ``total_dos``).
+
+        Each mesh cell is cut into 6 tetrahedra around its shortest body diagonal (``tetrahedra``), and each band,
+        ascending per q, is interpolated on its own (phonopy's method; its known error at band crossings falls with
+        the mesh).  Frequencies, eigenvector weights and the DOS (``chg_tetrahedron_dos``) stay on the device until
+        the result is returned."""
+        mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
+        q = gamma_mesh(mesh)
+        n_prim = len(self.p2s)
+        n3, dev = 3 * n_prim, self.device
+        nu = torch.empty(len(q), n3, dtype=torch.float64, device=dev)
+        proj = torch.empty(len(q), n3, n_prim, dtype=torch.float64, device=dev) if projected else None
+        chunk = max(1, min(self.chunk_bytes // (16 * n3 * n3), self.eigh_batch))
+        for s in range(0, len(q), chunk):
+            d = self.dynamical_matrices(q[s : s + chunk])
+            if projected:
+                lam, e = torch.linalg.eigh(d)
+                proj[s : s + chunk] = (e.abs() ** 2).view(-1, n_prim, 3, n3).sum(dim=2).transpose(1, 2)
+            else:
+                lam = torch.linalg.eigvalsh(d)
+            nu[s : s + chunk] = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+        if frequency_points is None:
+            t = torch.arange(201, dtype=torch.float64, device=dev) / 200  # lerp ends exactly on the maximum
+            omega = torch.lerp(nu.min().expand(201), nu.max().expand(201), t)
+        else:
+            omega = torch.as_tensor(np.asarray(frequency_points, dtype=np.float64).reshape(-1)).to(dev)
+        tets = torch.as_tensor(tetrahedra(mesh, self.cell.prim_lattice)).to(dev)
+        total, integrated = torch.empty_like(omega), torch.empty_like(omega)
+        pdos = torch.empty(n_prim, len(omega), dtype=torch.float64, device=dev) if projected else None
+        self.kernels.tetrahedron_dos(nu, mesh, tets, omega, total, integrated, proj, pdos)
+        out = {"frequency_points": omega.cpu().numpy(), "total_dos": total.cpu().numpy(),
+               "integrated_dos": integrated.cpu().numpy()}
+        if projected:
+            out["projected_dos"] = pdos.cpu().numpy()
+        return out

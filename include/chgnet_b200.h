@@ -550,6 +550,27 @@ int chg_edge_tangent_bwd_virial(const float* rvec, const float* dist, const floa
 int chg_dynamical_matrices(const double* fc, const int32_t* img_ptr, const double* img_vec, const int32_t* s2p,
                            const double* inv_sqrt_m, int32_t n_prim, int32_t n_super, const double* qpoints,
                            int32_t n_q, double* dyn, void* stream);
+/* ddyn [n_q][3][3 n_prim][3 n_prim] interleaved complex128 (written in full, Hermitian) = dD/dQ_c, c = x, y, z, in
+ * eV/(A amu): the sum of chg_dynamical_matrices with every image term multiplied by 2 pi i r_c, r = v . prim_lattice
+ * (A), the derivative with respect to the Cartesian wave vector Q = q . inv(prim_lattice)^T in 1/A without 2 pi
+ * (q.v = Q.r).  Same arguments as chg_dynamical_matrices, plus prim_lattice [3][3] (rows are lattice vectors, A,
+ * fp64, device memory).  Deterministic (no atomics).                                                              */
+int chg_dynamical_matrix_derivatives(const double* fc, const int32_t* img_ptr, const double* img_vec,
+                                     const int32_t* s2p, const double* inv_sqrt_m, int32_t n_prim, int32_t n_super,
+                                     const double* qpoints, int32_t n_q, const double* prim_lattice, double* ddyn,
+                                     void* stream);
+/* Linear tetrahedron density of states on the full Gamma-centred mesh n1 x n2 x n3 (q index (i n2 + j) n3 + k):
+ * freqs [n1 n2 n3][n_band] (fp64, ascending per q; each band is interpolated on its own); tetrahedra [6][4][3] int32
+ * corner offsets in {0, 1} of the 6 tetrahedra of a mesh cell (periodic wrap); omega [n_freq] the frequency points.
+ * With g_T, w_T,i and N_T the density, corner weights and volume fraction of one (tetrahedron, band), each weighted
+ * 1 / (6 n1 n2 n3):  dos[f] = sum g_T(omega_f),  idos[f] = sum N_T(omega_f),  and when proj [n1 n2 n3][n_band][n_proj]
+ * is given (else NULL, pdos unused), pdos [n_proj][n_freq] = sum_T sum_i w_T,i(omega_f) proj[q_i][band][s].
+ * work: CHG_DOS_MAX_CHUNKS * (2 + n_proj) * n_freq doubles of scratch.  Deterministic: two kernels, per-block partial
+ * sums added in a fixed order, no atomics.                                                                         */
+#define CHG_DOS_MAX_CHUNKS 512
+int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                        const int32_t* tetrahedra, const double* proj, int32_t n_proj, const double* omega,
+                        int32_t n_freq, double* dos, double* idos, double* pdos, double* work, void* stream);
 
 #ifdef __cplusplus
 }
