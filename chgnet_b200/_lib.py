@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int32, c_int64, c_void_p
+from ctypes import c_char_p, c_double, c_float, c_int32, c_int64, c_void_p
 
 import torch
 from torch import Tensor
@@ -16,7 +16,7 @@ from torch import Tensor
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libchgnet_b200.so")
 
-P, I, F, I64 = c_void_p, c_int32, c_float, c_int64
+P, I, F, D, I64 = c_void_p, c_int32, c_float, c_double, c_int64
 
 # name -> argument ctypes (the trailing stream pointer included); mirrors the header 1:1
 SIGNATURES: dict[str, list] = {
@@ -70,10 +70,13 @@ SIGNATURES: dict[str, list] = {
     "chg_dynamical_matrices": [P, P, P, P, P, I, I, P, I, P, P],
     "chg_dynamical_matrix_derivatives": [P, P, P, P, P, I, I, P, I, P, P, P],
     "chg_tetrahedron_dos": [P, I, I, I, I, P, P, I, P, I, P, P, P, P, P],
+    "chg_thermal_displacements": [P, P, I, I, P, I, D, P, P, P],
 }
 
 # CHG_DOS_MAX_CHUNKS of include/chgnet_b200.h: chg_tetrahedron_dos needs this many (2 + n_proj) x n_freq scratch rows
 DOS_MAX_CHUNKS = 512
+# CHG_TD_MAX_CHUNKS: chg_thermal_displacements needs this many n_t x n_prim x 6 scratch blocks
+TD_MAX_CHUNKS = 128
 
 _lib = None
 
@@ -410,6 +413,27 @@ class CudaKernels:
         work = torch.empty(DOS_MAX_CHUNKS * (2 + n_proj) * max(n_f, 1), dtype=f64, device=freqs.device)
         self._call("chg_tetrahedron_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(proj), n_proj, _p(omega),
                    n_f, _p(dos), _p(idos), _p(pdos if proj is not None else None), _p(work))
+
+    def thermal_displacements(self, freqs, eigvecs, temperatures, cutoff_thz, acc):
+        """acc [T, n_prim, 6] fp64 += sum over (q, mode) of w(nu, T) Re(e e^H) per atom in Voigt order (xx, yy, zz,
+        yz, xz, xy), w = (1 + 2 / expm1(h nu / k T)) / nu for nu >= cutoff_thz and 0 otherwise: freqs [Q, 3n] THz
+        (fp64, signed), eigvecs [Q, mode, 3n] complex128 (mode-major: ``e.mT`` of eigh's eigenvectors), temperatures
+        [T] K (fp64)."""
+        self._chk(freqs, eigvecs, temperatures, acc)
+        f64 = torch.float64
+        if (freqs.dtype != f64 or temperatures.dtype != f64 or acc.dtype != f64
+                or eigvecs.dtype != torch.complex128):
+            raise ChgnetB200Error("thermal_displacements: freqs, temperatures and acc must be float64, eigvecs "
+                                  "complex128")
+        n_q, n3 = freqs.shape
+        n_t = temperatures.shape[0]
+        if (n3 % 3 or tuple(eigvecs.shape) != (n_q, n3, n3) or temperatures.dim() != 1
+                or tuple(acc.shape) != (n_t, n3 // 3, 6)):
+            raise ChgnetB200Error(f"thermal_displacements: freqs must be [Q, 3n], eigvecs [{n_q}, {n3}, {n3}], "
+                                  f"temperatures [T] and acc [T, {n3 // 3}, 6]")
+        work = torch.empty(TD_MAX_CHUNKS * max(n_t * (n3 // 3) * 6, 1), dtype=f64, device=freqs.device)
+        self._call("chg_thermal_displacements", _p(freqs), _p(eigvecs), n_q, n3 // 3, _p(temperatures), n_t,
+                   float(cutoff_thz), _p(work), _p(acc))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

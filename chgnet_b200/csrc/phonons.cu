@@ -14,6 +14,8 @@
 // the group velocities of Phonons.group_velocities.  One more grid dimension runs over c.
 //
 // chg_tetrahedron_dos: the linear tetrahedron method (Bloechl's closed forms) on a full Gamma-centred mesh, see below.
+// chg_thermal_displacements: the mode- and temperature-weighted sums of Re(e e^H) per atom behind the thermal
+// displacement matrices, see below.
 #include <algorithm>
 
 #include "common.cuh"
@@ -272,6 +274,89 @@ __global__ void dos_reduce_kernel(const double* __restrict__ work, int n_chunks,
   out[f] = acc * scale;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Thermal displacements.  acc[t][k][c] += sum over (q, mode) of w(nu, T_t) Re(e e^H)_c, e the 3-component block of
+// atom k in the mode's unit eigenvector, c in Voigt order (xx, yy, zz, yz, xz, xy), and
+//   w = (1 + 2 / expm1(h nu / k T)) / nu  for nu >= cutoff,  0 otherwise  (1 + 2n = 1 at T = 0).
+// Grid x: contiguous ranges of q (chunks); y: groups of TD_ATOMS atoms; z: tiles of temperatures.  Thread (qi, ti)
+// takes the q-points q_begin + qi, q_begin + qi + n_qi, ... of its block's range at temperature t0 + ti, reads the
+// eigenvector blocks of the group's atoms (the same addresses for every ti of one q) and keeps 6 TD_ATOMS sums in
+// registers.  The block adds them over qi in a fixed order in shared memory and writes work[chunk][t][k][6];
+// td_reduce_kernel adds the chunks in chunk order to acc.  No atomics, and neither the (q, mode) products nor the
+// weights ever reach global memory.
+constexpr int TD_THREADS = 256;  // (q, temperature) slots per block
+constexpr int TD_ATOMS = 4;      // atoms per block (grid y)
+// h / k_B in K/THz: chgnet_b200.phonons.H_EV_PER_THZ / chgnet_b200.dynamics.KB, the same expression in the same order
+constexpr double TD_H_OVER_K = 6.62607015e-34 / 1.602176634e-19 * 1e12 / 8.617333262e-5;
+
+__global__ void __launch_bounds__(TD_THREADS)
+thermal_displacements_kernel(const double* __restrict__ freqs, const double2* __restrict__ eigvecs, int n_q,
+                             int n_prim, const double* __restrict__ temps, int n_t, int t_tile, double cutoff,
+                             double* __restrict__ work) {
+  __shared__ double red[TD_THREADS * 6];
+  const int n3 = 3 * n_prim;
+  const int n_qi = blockDim.x / t_tile;  // q-points per pass
+  const int qi = threadIdx.x / t_tile, ti = threadIdx.x % t_tile;
+  const int t0 = blockIdx.z * t_tile, k0 = blockIdx.y * TD_ATOMS;
+  const int n_here = min(TD_ATOMS, n_prim - k0);
+  const bool active = t0 + ti < n_t;
+  const double temp = active ? temps[t0 + ti] : 0.0;
+  const int q_begin = (int)((int64_t)n_q * blockIdx.x / gridDim.x);
+  const int q_end = (int)((int64_t)n_q * (blockIdx.x + 1) / gridDim.x);
+  double acc[TD_ATOMS][6];
+#pragma unroll
+  for (int a = 0; a < TD_ATOMS; ++a)
+#pragma unroll
+    for (int c = 0; c < 6; ++c) acc[a][c] = 0.0;
+  for (int q = q_begin + qi; active && q < q_end; q += n_qi) {
+    const double* nu_q = freqs + (size_t)q * n3;
+    const double2* e_q = eigvecs + (size_t)q * n3 * n3 + 3 * k0;
+    for (int m = 0; m < n3; ++m) {
+      const double nu = __ldg(nu_q + m);
+      if (!(nu >= cutoff)) continue;
+      const double coth = temp > 0.0 ? 1.0 + 2.0 / expm1(TD_H_OVER_K * nu / temp) : 1.0;
+      const double w = coth / nu;
+      const double2* e = e_q + (size_t)m * n3;
+#pragma unroll
+      for (int a = 0; a < TD_ATOMS; ++a) {
+        if (a >= n_here) break;
+        const double2 x = __ldg(e + 3 * a), y = __ldg(e + 3 * a + 1), z = __ldg(e + 3 * a + 2);
+        acc[a][0] = fma(w, fma(x.x, x.x, x.y * x.y), acc[a][0]);
+        acc[a][1] = fma(w, fma(y.x, y.x, y.y * y.y), acc[a][1]);
+        acc[a][2] = fma(w, fma(z.x, z.x, z.y * z.y), acc[a][2]);
+        acc[a][3] = fma(w, fma(y.x, z.x, y.y * z.y), acc[a][3]);
+        acc[a][4] = fma(w, fma(x.x, z.x, x.y * z.y), acc[a][4]);
+        acc[a][5] = fma(w, fma(x.x, y.x, x.y * y.y), acc[a][5]);
+      }
+    }
+  }
+  const int n_out = min(t_tile, n_t - t0) * 6;
+#pragma unroll
+  for (int a = 0; a < TD_ATOMS; ++a) {
+    if (a >= n_here) break;  // uniform across the block
+    __syncthreads();  // the previous atom's sums have been read
+#pragma unroll
+    for (int c = 0; c < 6; ++c) red[threadIdx.x * 6 + c] = acc[a][c];
+    __syncthreads();
+    for (int o = threadIdx.x; o < n_out; o += blockDim.x) {
+      const int tt = o / 6, c = o % 6;
+      double s = 0.0;
+      for (int i = 0; i < n_qi; ++i) s += red[(i * t_tile + tt) * 6 + c];
+      work[(((size_t)blockIdx.x * n_t + t0 + tt) * n_prim + k0 + a) * 6 + c] = s;
+    }
+  }
+}
+
+// acc[o] += sum over chunks (in chunk order) of work[chunk][o]
+__global__ void td_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out,
+                                 double* __restrict__ acc) {
+  const int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= n_out) return;
+  double s = 0.0;
+  for (int c = 0; c < n_chunks; ++c) s += work[(size_t)c * n_out + o];
+  acc[o] += s;
+}
+
 }  // namespace
 }  // namespace chg
 
@@ -333,5 +418,27 @@ extern "C" int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t 
   const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
   dos_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, rows, n_freq, scale,
                                                                                       dos, idos, pdos);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_thermal_displacements(const double* freqs, const double* eigvecs, int32_t n_q, int32_t n_prim,
+                                         const double* temperatures, int32_t n_t, double cutoff_thz, double* work,
+                                         double* acc, void* stream) {
+  CHG_CHECK_ARG(n_q >= 0 && n_prim >= 0 && n_t >= 0, "negative size");
+  if (n_q == 0 || n_prim == 0 || n_t == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && eigvecs && temperatures && work && acc, "null pointer");
+  const int64_t groups = ((int64_t)n_prim + TD_ATOMS - 1) / TD_ATOMS;
+  const int64_t t_tiles = ((int64_t)n_t + TD_THREADS - 1) / TD_THREADS;
+  CHG_CHECK_ARG(groups <= 65535 && t_tiles <= 65535, "too many atoms or temperatures");
+  const int t_tile = (int)((n_t + t_tiles - 1) / t_tiles);
+  const int n_qi = TD_THREADS / t_tile;
+  const int chunks = (int)std::min<int64_t>(CHG_TD_MAX_CHUNKS, ((int64_t)n_q + n_qi - 1) / n_qi);
+  thermal_displacements_kernel<<<dim3(chunks, (unsigned)groups, (unsigned)t_tiles), n_qi * t_tile, 0,
+                                 as_stream(stream)>>>(freqs, reinterpret_cast<const double2*>(eigvecs), n_q, n_prim,
+                                                      temperatures, n_t, t_tile, cutoff_thz, work);
+  CHG_CUDA(cudaGetLastError());
+  chg::count_launch();
+  const int64_t n_out = (int64_t)n_t * n_prim * 6;
+  td_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, n_out, acc);
   CHG_LAUNCH_END();
 }

@@ -9,11 +9,12 @@
 * ``Phonons``: dynamical matrices D(q) on the device (``chg_dynamical_matrices``, csrc/phonons.cu), frequencies and
   eigenvectors by ``torch.linalg.eigh``, and harmonic thermodynamics on a Gamma-centred mesh; group velocities from
   dD/dQ (``chg_dynamical_matrix_derivatives``) and the linear tetrahedron density of states, total and projected on
-  atoms (``chg_tetrahedron_dos``).
+  atoms (``chg_tetrahedron_dos``); anisotropic thermal displacement matrices U(T) on a mesh
+  (``chg_thermal_displacements``), Cartesian and in the CIF convention (``cif_displacement_matrices``).
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
-primitive cell for densities of states.
+primitive cell for densities of states, A^2 for thermal displacement matrices.
 """
 from __future__ import annotations
 
@@ -27,9 +28,13 @@ import torch
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
-_EV, _AMU, _ANGSTROM = 1.602176634e-19, 1.66053906660e-27, 1e-10
+_EV, _AMU, _ANGSTROM, _H = 1.602176634e-19, 1.66053906660e-27, 1e-10, 6.62607015e-34
 THZ_PER_SQRT_EV_A2_AMU = math.sqrt(_EV / (_ANGSTROM**2 * _AMU)) / (2 * math.pi) / 1e12
-H_EV_PER_THZ = 6.62607015e-34 / _EV * 1e12  # h nu in eV for nu in THz
+H_EV_PER_THZ = _H / _EV * 1e12  # h nu in eV for nu in THz
+# h / k_B in K/THz (the constant of chg_thermal_displacements)
+H_OVER_KB_K_PER_THZ = H_EV_PER_THZ / KB
+# hbar / (2 m omega) = C / (m [amu] nu [THz]) in A^2: C = h / (8 pi^2 amu 1 THz) = 0.5053790 A^2
+DISPLACEMENT_A2_AMU_THZ = _H / (8 * math.pi**2 * _AMU * 1e12) / _ANGSTROM**2
 # image lengths within this of the shortest count as minimum images (A)
 IMAGE_TOL = 1e-5
 # modes below this |nu| (THz) are left out of the thermodynamic sums
@@ -235,6 +240,16 @@ def tetrahedra(mesh, prim_lattice, diagonal=None) -> np.ndarray:
     return np.ascontiguousarray(np.where(f == 1, 1 - tets, tets), dtype=np.int32)
 
 
+def cif_displacement_matrices(u_cart, prim_lattice) -> np.ndarray:
+    """Cartesian displacement matrices ``u_cart [..., 3, 3]`` (A^2) in the CIF convention (Grosse-Kunstleve and Adams,
+    as phonopy): U_cif = N^-1 A^-1 U A^-T N^-1, A = ``prim_lattice``^T (lattice vectors as columns) and
+    N = diag(|a*|, |b*|, |c*|), a* the rows of inv(prim_lattice)^T.  An isotropic u I becomes u cos(a*_i, a*_j)."""
+    lat = np.asarray(prim_lattice, dtype=np.float64).reshape(3, 3)
+    recip = np.linalg.inv(lat).T  # rows a*, b*, c* (no 2 pi); A^-1 = recip
+    m = recip / np.linalg.norm(recip, axis=1)[:, None]  # N^-1 A^-1
+    return m @ np.asarray(u_cart, dtype=np.float64) @ m.T
+
+
 class Phonons:
     """Harmonic phonons of a crystal from its compact supercell force constants (``CHGNet.phonons``).
 
@@ -407,3 +422,44 @@ class Phonons:
         if projected:
             out["projected_dos"] = pdos.cpu().numpy()
         return out
+
+    def thermal_displacement_matrices(self, mesh, temperatures) -> dict:
+        """Anisotropic thermal displacement matrices of the primitive atoms on a full Gamma-centred ``mesh`` (n1, n2,
+        n3) at ``temperatures`` (K, finite and >= 0, else ValueError):
+
+            U_k(T) = hbar / (2 m_k N_q) sum_q sum_nu [1 + 2 n(nu, T)] / omega_nu(q) Re[e_k,nu(q) e_k,nu(q)^H]
+
+        over the N_q points of the mesh (Gamma included, phonopy's normalisation), e_k the 3-component block of atom k
+        in the unit eigenvector, omega = 2 pi nu and 1 + 2n = 1 + 2 / expm1(h nu / k T) (1 at T = 0).  Modes with
+        nu < ``THERMAL_CUTOFF_THZ`` are left out (imaginary and near-zero modes, as in ``thermal_properties``), and so
+        are, whatever their value, the three modes of smallest |nu| at Gamma: a Gamma acoustic mode lifted above the
+        cutoff by force-constant noise would otherwise add ~2 k T / (h nu^2) each.  The sum over the full mesh is
+        real (q and -q pair up), so only Re(e e^H) is accumulated.
+
+        Returns ``temperatures`` [T], ``cartesian`` [T, n_prim, 3, 3] and ``cif`` [T, n_prim, 3, 3] in A^2
+        (``cif_displacement_matrices``), and ``n_imaginary``, the number of modes below -``THERMAL_CUTOFF_THZ`` over
+        the mesh, as in ``thermal_properties``: U is not meaningful when it is not 0.  D(q), the eigenvectors and the
+        sums (``chg_thermal_displacements``) stay on the device, in chunks of at most ``eigh_batch`` q; only the
+        [T, n_prim, 6] sums are copied back."""
+        temps = np.asarray(temperatures, dtype=np.float64).reshape(-1)
+        if not np.all(np.isfinite(temps)) or np.any(temps < 0):
+            raise ValueError(f"temperatures must be finite and non-negative, got {temps.tolist()}")
+        q = gamma_mesh(mesh)
+        n_prim = len(self.p2s)
+        n3, dev = 3 * n_prim, self.device
+        t = torch.as_tensor(temps).to(dev)
+        acc = torch.zeros(len(temps), n_prim, 6, dtype=torch.float64, device=dev)
+        n_imaginary = torch.zeros((), dtype=torch.int64, device=dev)
+        chunk = max(1, min(self.chunk_bytes // (16 * n3 * n3), self.eigh_batch))
+        for s in range(0, len(q), chunk):
+            lam, e = torch.linalg.eigh(self.dynamical_matrices(q[s : s + chunk]))
+            nu = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+            n_imaginary += (nu < -THERMAL_CUTOFF_THZ).sum()
+            if s == 0:  # q index 0 is Gamma
+                nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0
+            # eigh returns column-major matrices: e.mT is the mode-major layout of the kernel, without a copy
+            self.kernels.thermal_displacements(nu, e.mT.contiguous(), t, THERMAL_CUTOFF_THZ, acc)
+        v = acc.cpu().numpy() * (DISPLACEMENT_A2_AMU_THZ / len(q)) / self.masses[None, :, None]
+        cart = v[..., [[0, 5, 4], [5, 1, 3], [4, 3, 2]]]  # Voigt xx, yy, zz, yz, xz, xy -> 3x3
+        return {"temperatures": temps, "cartesian": cart, "cif": cif_displacement_matrices(cart, self.cell.prim_lattice),
+                "n_imaginary": int(n_imaginary)}

@@ -571,6 +571,17 @@ int chg_dynamical_matrix_derivatives(const double* fc, const int32_t* img_ptr, c
 int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
                         const int32_t* tetrahedra, const double* proj, int32_t n_proj, const double* omega,
                         int32_t n_freq, double* dos, double* idos, double* pdos, double* work, void* stream);
+/* Thermal displacement sums: acc [n_t][n_prim][6] += sum over (q, mode) of w(nu, T) Re(e e^H), e the 3-component
+ * block of atom k in the mode's eigenvector, in Voigt order (xx, yy, zz, yz, xz, xy), with
+ *   w = (1 + 2 / expm1(h nu / k_B T)) / nu  for nu >= cutoff_thz  (1 at the numerator for T <= 0),  0 otherwise.
+ * freqs [n_q][3 n_prim] fp64 THz (signed); eigvecs [n_q][mode][3 n_prim] interleaved complex128, mode-major (the
+ * transpose of eigh's column-eigenvector matrices); temperatures [n_t] K (fp64).  Masses and h / (8 pi^2 amu THz)
+ * are left to the caller.  work: CHG_TD_MAX_CHUNKS * n_t * n_prim * 6 doubles of scratch.  Deterministic: two
+ * kernels, per-block partial sums added in a fixed order, no atomics.                                            */
+#define CHG_TD_MAX_CHUNKS 128
+int chg_thermal_displacements(const double* freqs, const double* eigvecs, int32_t n_q, int32_t n_prim,
+                              const double* temperatures, int32_t n_t, double cutoff_thz, double* work, double* acc,
+                              void* stream);
 
 #ifdef __cplusplus
 }
