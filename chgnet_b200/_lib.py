@@ -71,12 +71,15 @@ SIGNATURES: dict[str, list] = {
     "chg_dynamical_matrix_derivatives": [P, P, P, P, P, I, I, P, I, P, P, P],
     "chg_tetrahedron_dos": [P, I, I, I, I, P, P, I, P, I, P, P, P, P, P],
     "chg_thermal_displacements": [P, P, I, I, P, I, D, P, P, P],
+    "chg_joint_dos": [P, I, I, I, I, P, P, I, P, I, P, I, D, P, P, P],
 }
 
 # CHG_DOS_MAX_CHUNKS of include/chgnet_b200.h: chg_tetrahedron_dos needs this many (2 + n_proj) x n_freq scratch rows
 DOS_MAX_CHUNKS = 512
 # CHG_TD_MAX_CHUNKS: chg_thermal_displacements needs this many n_t x n_prim x 6 scratch blocks
 TD_MAX_CHUNKS = 128
+# CHG_JDOS_MAX_CHUNKS: chg_joint_dos needs this many n_target x (1 + n_t) x 2 x n_freq scratch blocks
+JDOS_MAX_CHUNKS = 64
 
 _lib = None
 
@@ -434,6 +437,34 @@ class CudaKernels:
         work = torch.empty(TD_MAX_CHUNKS * max(n_t * (n3 // 3) * 6, 1), dtype=f64, device=freqs.device)
         self._call("chg_thermal_displacements", _p(freqs), _p(eigvecs), n_q, n3 // 3, _p(temperatures), n_t,
                    float(cutoff_thz), _p(work), _p(acc))
+
+    def joint_dos(self, freqs, mesh, tetrahedra, targets, omega, temperatures, cutoff_thz, out):
+        """Two-phonon joint densities of states on the full Gamma-centred ``mesh`` (n1, n2, n3): freqs [n1 n2 n3,
+        n_band] fp64 THz (ascending per q), tetrahedra [6, 4, 3] int32, targets [Q] int32 mesh indices, omega [Q, F]
+        fp64 THz (the frequency points of each target), temperatures [T] fp64 K or None; writes out [Q, 1 + T, 2, F]
+        fp64 (slot 0: D2 classes 1 and 2; slot 1 + t: N2 at temperatures[t]), modes below cutoff_thz left out."""
+        self._chk(freqs, tetrahedra, targets, omega, temperatures, out)
+        n1, n2, n3 = (int(n) for n in mesh)
+        f64 = torch.float64
+        if any(t is not None and t.dtype != f64 for t in (freqs, omega, temperatures, out)):
+            raise ChgnetB200Error("joint_dos: freqs, omega, temperatures and out must be float64")
+        if tetrahedra.dtype != torch.int32 or tuple(tetrahedra.shape) != (6, 4, 3):
+            raise ChgnetB200Error("joint_dos: tetrahedra must be int32 [6, 4, 3]")
+        if targets.dtype != torch.int32 or targets.dim() != 1:
+            raise ChgnetB200Error("joint_dos: targets must be int32 [Q]")
+        n_q, n_band = freqs.shape
+        n_target = targets.shape[0]
+        n_t = 0 if temperatures is None else temperatures.shape[0]
+        if temperatures is not None and temperatures.dim() != 1:
+            raise ChgnetB200Error("joint_dos: temperatures must be [T]")
+        if n_q != n1 * n2 * n3 or omega.dim() != 2 or omega.shape[0] != n_target:
+            raise ChgnetB200Error(f"joint_dos: freqs must be [{n1 * n2 * n3}, n_band] and omega [{n_target}, F]")
+        n_f = omega.shape[1]
+        if tuple(out.shape) != (n_target, 1 + n_t, 2, n_f):
+            raise ChgnetB200Error(f"joint_dos: out must be [{n_target}, {1 + n_t}, 2, {n_f}]")
+        work = torch.empty(JDOS_MAX_CHUNKS * max(n_target * (1 + n_t) * 2 * n_f, 1), dtype=f64, device=freqs.device)
+        self._call("chg_joint_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(targets), n_target, _p(omega),
+                   n_f, _p(temperatures), n_t, float(cutoff_thz), _p(out), _p(work))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

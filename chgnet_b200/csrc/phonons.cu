@@ -16,6 +16,10 @@
 // chg_tetrahedron_dos: the linear tetrahedron method (Bloechl's closed forms) on a full Gamma-centred mesh, see below.
 // chg_thermal_displacements: the mode- and temperature-weighted sums of Re(e e^H) per atom behind the thermal
 // displacement matrices, see below.
+// chg_joint_dos: the two-phonon joint densities of states D2 and their occupation-weighted forms N2 at target q-points,
+// by the same tetrahedron method, see below.
+#include <math_constants.h>
+
 #include <algorithm>
 
 #include "common.cuh"
@@ -357,6 +361,154 @@ __global__ void td_reduce_kernel(const double* __restrict__ work, int n_chunks, 
   acc[o] += s;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Joint densities of states.  For a target q and an item (cell, tetrahedron, l1, l2) the corners are q1_i of the
+// tetrahedron and q2_i = q - q1_i (integer mesh arithmetic); nu1_i = freqs[q1_i][l1], nu2_i = freqs[q2_i][l2].  The item
+// gives two interpolants with corner factors c_i:
+//   class 1: f_i = nu2_i - nu1_i  (the term delta(w + nu1 - nu2)),  c_i = m_i (slot 0) or m_i (n1_i - n2_i) (slot 1 + t)
+//   class 2: f_i = nu1_i + nu2_i,                                   c_i = m_i           or m_i (n1_i + n2_i + 1)
+// m_i = [nu1_i >= cutoff and nu2_i >= cutoff], n = 1 / expm1(h nu / k T) (0 at T = 0).  The other class-1 term,
+// delta(w - nu1 + nu2), is the same sum mapped by q1 -> q - q1, l1 <-> l2 (the 6-tetrahedron set is inversion
+// symmetric): jdos_reduce_kernel doubles class 1, which also gives N2(1)'s difference.  The contribution at w is
+// sum_i wt_i(w) c_i with tetra_weights' corner weights, each tetrahedron weighted 1 / (6 N).
+//
+// Block (x, y): JDOS_THREADS threads as blockDim.y target slots of blockDim.x (a multiple of 32) frequency points.
+// Grid x: contiguous ranges of item tiles (chunks); y: groups of blockDim.y targets x tiles of blockDim.x points;
+// z: the slot (0: D2, 1 + t: N2 at temperatures[t]).  Each warp of a target slot stages one sorted tile of
+// blockDim.x items of its own target in shared memory (values and corner factors of both classes), then every
+// thread of that slot evaluates the tile at its own frequency point (shared-memory broadcasts).  The block writes
+// work[chunk][target][slot][class][f], each element by exactly one thread; jdos_reduce_kernel adds the chunks in a
+// fixed order.  No atomics, and no per-item value leaves the SM.
+constexpr int JDOS_THREADS = 256;
+
+__device__ __forceinline__ double bose(double nu, double temp) {
+  return temp > 0.0 ? 1.0 / expm1(TD_H_OVER_K * nu / temp) : 0.0;
+}
+
+// sort the corner values ascending, carrying their factors (ties keep a fixed, data-determined order)
+__device__ __forceinline__ void sort4(double (&e)[4], double (&c)[4]) {
+#define CHG_CSWAP(i, j)        \
+  if (e[j] < e[i]) {           \
+    const double te = e[i];    \
+    e[i] = e[j], e[j] = te;    \
+    const double tc = c[i];    \
+    c[i] = c[j], c[j] = tc;    \
+  }
+  CHG_CSWAP(0, 1) CHG_CSWAP(2, 3) CHG_CSWAP(0, 2) CHG_CSWAP(1, 3) CHG_CSWAP(1, 2)
+#undef CHG_CSWAP
+}
+
+__global__ void __launch_bounds__(JDOS_THREADS)
+joint_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
+                 const int32_t* __restrict__ tet, const int32_t* __restrict__ targets, int n_target,
+                 const double* __restrict__ omega, int n_freq, const double* __restrict__ temps, double cutoff,
+                 int64_t n_items, double* __restrict__ work) {
+  // [slot y * blockDim.x + item][class][e0..e3, c0..c3]
+  __shared__ double st[JDOS_THREADS][2][8];
+  const int tile = blockDim.x;
+  const int ti = blockIdx.y / ((n_freq + tile - 1) / tile) * blockDim.y + threadIdx.y;  // target of this slot
+  const int f = blockIdx.y % ((n_freq + tile - 1) / tile) * tile + threadIdx.x;
+  const bool has_target = ti < n_target;
+  const bool active = has_target && f < n_freq;
+  const double w = active ? omega[(size_t)ti * n_freq + f] : 0.0;
+  const int slot = blockIdx.z;
+  const double temp = slot > 0 ? temps[slot - 1] : 0.0;
+  int qa = 0, qb = 0, qc = 0;
+  if (has_target) {
+    const int q = targets[ti];
+    qa = q / (n2 * n3), qb = (q / n3) % n2, qc = q % n3;
+  }
+  double (*my)[2][8] = st + threadIdx.y * tile;
+  double acc1 = 0.0, acc2 = 0.0;
+  const int64_t n_tiles = (n_items + tile - 1) / tile;
+  const int64_t t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  for (int64_t t = n_tiles * blockIdx.x / gridDim.x; t < t_end; ++t) {
+    const int64_t p = t * tile + threadIdx.x;
+    __syncthreads();  // the previous tile has been read
+    if (has_target && p < n_items) {
+      const int l2 = (int)(p % n_band);
+      const int64_t r = p / n_band;
+      const int l1 = (int)(r % n_band);
+      const int64_t tt = r / n_band;
+      const int it = (int)(tt % 6);
+      const int64_t cell = tt / 6;
+      const int ci = (int)(cell / ((int64_t)n2 * n3)), cj = (int)((cell / n3) % n2), ck = (int)(cell % n3);
+      double e1[4], c1[4], e2[4], c2[4];
+      bool any = false;
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const int32_t* o = tet + (it * 4 + v) * 3;
+        int a = ci + __ldg(o), b = cj + __ldg(o + 1), c = ck + __ldg(o + 2);
+        a -= a >= n1 ? n1 : 0;
+        b -= b >= n2 ? n2 : 0;
+        c -= c >= n3 ? n3 : 0;
+        int a2 = qa - a, b2 = qb - b, c2i = qc - c;
+        a2 += a2 < 0 ? n1 : 0;
+        b2 += b2 < 0 ? n2 : 0;
+        c2i += c2i < 0 ? n3 : 0;
+        const double nu1 = __ldg(freqs + (int64_t)((a * n2 + b) * n3 + c) * n_band + l1);
+        const double nu2 = __ldg(freqs + (int64_t)((a2 * n2 + b2) * n3 + c2i) * n_band + l2);
+        e1[v] = nu2 - nu1;
+        e2[v] = nu1 + nu2;
+        const bool keep = nu1 >= cutoff && nu2 >= cutoff;
+        any |= keep;
+        if (!keep) {
+          c1[v] = c2[v] = 0.0;
+        } else if (slot == 0) {
+          c1[v] = c2[v] = 1.0;
+        } else {
+          const double b1 = bose(nu1, temp), b2v = bose(nu2, temp);
+          c1[v] = b1 - b2v;
+          c2[v] = b1 + b2v + 1.0;
+        }
+      }
+      sort4(e1, c1);
+      sort4(e2, c2);
+      if (!any) e1[0] = e2[0] = CUDART_INF;  // every corner masked: no frequency point is evaluated
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        my[threadIdx.x][0][v] = e1[v], my[threadIdx.x][0][4 + v] = c1[v];
+        my[threadIdx.x][1][v] = e2[v], my[threadIdx.x][1][4 + v] = c2[v];
+      }
+    }
+    __syncthreads();
+    if (!active) continue;
+    const int n_here = (int)min((int64_t)tile, n_items - t * tile);
+    for (int i = 0; i < n_here; ++i) {
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const double* s = my[i][k];
+        if (!(w >= s[0] && w < s[3])) continue;
+        const double e[4] = {s[0], s[1], s[2], s[3]};
+        double n, g, wt[4];
+        tetra_weights(w, e, n, g, wt);
+        const double x = fma(wt[0], s[4], fma(wt[1], s[5], fma(wt[2], s[6], wt[3] * s[7])));
+        if (k == 0) {
+          acc1 += x;
+        } else {
+          acc2 += x;
+        }
+      }
+    }
+  }
+  if (!active) return;
+  const int n_slots = gridDim.z;
+  double* out = work + (((size_t)blockIdx.x * n_target + ti) * n_slots + slot) * 2 * n_freq + f;
+  out[0] = acc1;
+  out[n_freq] = acc2;
+}
+
+// out[o] = scale_class * sum over chunks (in chunk order) of work[chunk][o], o = ((target, slot), class, f); class 1
+// carries both of its terms (x 2)
+__global__ void jdos_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out, int n_freq,
+                                   double scale, double* __restrict__ out) {
+  const int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= n_out) return;
+  double s = 0.0;
+  for (int c = 0; c < n_chunks; ++c) s += work[(size_t)c * n_out + o];
+  out[o] = s * ((o / n_freq) % 2 == 0 ? 2.0 * scale : scale);
+}
+
 }  // namespace
 }  // namespace chg
 
@@ -440,5 +592,37 @@ extern "C" int chg_thermal_displacements(const double* freqs, const double* eigv
   chg::count_launch();
   const int64_t n_out = (int64_t)n_t * n_prim * 6;
   td_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, n_out, acc);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_joint_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                             const int32_t* tetrahedra, const int32_t* targets, int32_t n_target, const double* omega,
+                             int32_t n_freq, const double* temperatures, int32_t n_t, double cutoff_thz, double* out,
+                             double* work, void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_target >= 0 && n_freq >= 0 && n_t >= 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 * std::max(n_band, 1) < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(n_t < 65535, "too many temperatures");
+  if (n_target == 0 || n_freq == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && tetrahedra && targets && omega && out && work && (n_t == 0 || temperatures), "null pointer");
+  const int64_t n_items = (int64_t)n1 * n2 * n3 * 6 * n_band * n_band;
+  const int threads = (int)std::min<int64_t>(JDOS_THREADS, ((int64_t)n_freq + 31) / 32 * 32);
+  const int per_block = JDOS_THREADS / threads;  // target slots per block
+  const int64_t f_tiles = ((int64_t)n_freq + threads - 1) / threads;
+  const int64_t groups = ((int64_t)n_target + per_block - 1) / per_block * f_tiles;
+  CHG_CHECK_ARG(groups <= 65535, "too many targets or frequency points in one call");
+  const int n_slots = 1 + n_t;
+  // enough chunks for about 4 096 blocks in all, at most CHG_JDOS_MAX_CHUNKS and one tile each
+  const int64_t n_tiles = (n_items + threads - 1) / threads;
+  const int64_t want = (4096 + groups * n_slots - 1) / (groups * n_slots);
+  const int chunks = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)CHG_JDOS_MAX_CHUNKS, n_tiles, want}));
+  joint_dos_kernel<<<dim3(chunks, (unsigned)groups, n_slots), dim3(threads, per_block), 0, as_stream(stream)>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, targets, n_target, omega, n_freq, temperatures, cutoff_thz,
+      n_items, work);
+  CHG_CUDA(cudaGetLastError());
+  chg::count_launch();
+  const int64_t n_out = (int64_t)n_target * n_slots * 2 * n_freq;
+  const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
+  jdos_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, n_out, n_freq,
+                                                                                       scale, out);
   CHG_LAUNCH_END();
 }

@@ -10,11 +10,13 @@
   eigenvectors by ``torch.linalg.eigh``, and harmonic thermodynamics on a Gamma-centred mesh; group velocities from
   dD/dQ (``chg_dynamical_matrix_derivatives``) and the linear tetrahedron density of states, total and projected on
   atoms (``chg_tetrahedron_dos``); anisotropic thermal displacement matrices U(T) on a mesh
-  (``chg_thermal_displacements``), Cartesian and in the CIF convention (``cif_displacement_matrices``).
+  (``chg_thermal_displacements``), Cartesian and in the CIF convention (``cif_displacement_matrices``); two-phonon
+  joint densities of states and their occupation-weighted forms at mesh q-points, and per mode as the three-phonon
+  phase space (``chg_joint_dos``).
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
-primitive cell for densities of states, A^2 for thermal displacement matrices.
+primitive cell for densities of states, A^2 for thermal displacement matrices, 1/THz for joint densities of states.
 """
 from __future__ import annotations
 
@@ -25,6 +27,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from chgnet_b200._lib import JDOS_MAX_CHUNKS
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -267,6 +270,8 @@ class Phonons:
     chunk_bytes = 1 << 28
     # q-points per batched eigendecomposition in dos and group_velocities (cuSOLVER rejects batches of ~30 000)
     eigh_batch = 4096
+    # joint_dos and phase_space: targets per chg_joint_dos call keep its output and scratch below this many bytes
+    jdos_chunk_bytes = 1 << 28
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -381,19 +386,11 @@ class Phonons:
             out[s : s + chunk] = v.transpose(1, 2).cpu().numpy()
         return out[0] if single else out
 
-    def dos(self, mesh, frequency_points=None, *, projected: bool = False) -> dict:
-        """Phonon density of states by the linear tetrahedron method on a full Gamma-centred ``mesh`` (n1, n2, n3).
-
-        Returns ``frequency_points`` (THz; default 201 points from the lowest to the highest frequency of the mesh,
-        imaginary modes as negative numbers), ``total_dos`` (states/THz per primitive cell, integrating to 3 n_prim),
-        ``integrated_dos`` and, with ``projected``, ``projected_dos`` [n_prim, F]: the DOS projected on each primitive
-        atom with the weights sum_a |e_(k a)|^2 of the eigenvectors (the projections add up to ``total_dos``).
-
-        Each mesh cell is cut into 6 tetrahedra around its shortest body diagonal (``tetrahedra``), and each band,
-        ascending per q, is interpolated on its own (phonopy's method; its known error at band crossings falls with
-        the mesh).  Frequencies, eigenvector weights and the DOS (``chg_tetrahedron_dos``) stay on the device until
-        the result is returned."""
-        mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
+    def _mesh_frequencies(self, mesh, *, projected: bool = False):
+        """Frequencies ``[N, 3 n_prim]`` (THz, ascending per q) on the device at the points of the full Gamma-centred
+        ``mesh``, and with ``projected`` the eigenvector weights ``[N, 3 n_prim, n_prim]`` sum_a |e_(k a)|^2 (else
+        None): D(q) and ``torch.linalg.eigvalsh`` (``eigh``) in chunks of at most ``eigh_batch`` q that keep D below
+        ``chunk_bytes``."""
         q = gamma_mesh(mesh)
         n_prim = len(self.p2s)
         n3, dev = 3 * n_prim, self.device
@@ -408,6 +405,23 @@ class Phonons:
             else:
                 lam = torch.linalg.eigvalsh(d)
             nu[s : s + chunk] = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+        return nu, proj
+
+    def dos(self, mesh, frequency_points=None, *, projected: bool = False) -> dict:
+        """Phonon density of states by the linear tetrahedron method on a full Gamma-centred ``mesh`` (n1, n2, n3).
+
+        Returns ``frequency_points`` (THz; default 201 points from the lowest to the highest frequency of the mesh,
+        imaginary modes as negative numbers), ``total_dos`` (states/THz per primitive cell, integrating to 3 n_prim),
+        ``integrated_dos`` and, with ``projected``, ``projected_dos`` [n_prim, F]: the DOS projected on each primitive
+        atom with the weights sum_a |e_(k a)|^2 of the eigenvectors (the projections add up to ``total_dos``).
+
+        Each mesh cell is cut into 6 tetrahedra around its shortest body diagonal (``tetrahedra``), and each band,
+        ascending per q, is interpolated on its own (phonopy's method; its known error at band crossings falls with
+        the mesh).  Frequencies, eigenvector weights and the DOS (``chg_tetrahedron_dos``) stay on the device until
+        the result is returned."""
+        mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
+        n_prim, dev = len(self.p2s), self.device
+        nu, proj = self._mesh_frequencies(mesh, projected=projected)
         if frequency_points is None:
             t = torch.arange(201, dtype=torch.float64, device=dev) / 200  # lerp ends exactly on the maximum
             omega = torch.lerp(nu.min().expand(201), nu.max().expand(201), t)
@@ -463,3 +477,106 @@ class Phonons:
         cart = v[..., [[0, 5, 4], [5, 1, 3], [4, 3, 2]]]  # Voigt xx, yy, zz, yz, xz, xy -> 3x3
         return {"temperatures": temps, "cartesian": cart, "cif": cif_displacement_matrices(cart, self.cell.prim_lattice),
                 "n_imaginary": int(n_imaginary)}
+
+    def _jdos_mesh(self, mesh, temperatures):
+        """The mesh, its frequencies on the device with the three modes of smallest |nu| at Gamma set to 0 (still
+        ascending), ``n_imaginary`` (counted before that), the tetrahedra and the temperatures (None or [T] on the
+        device) for ``joint_dos`` and ``phase_space``."""
+        temps = None
+        if temperatures is not None:
+            temps = np.asarray(temperatures, dtype=np.float64).reshape(-1)
+            if not np.all(np.isfinite(temps)) or np.any(temps < 0):
+                raise ValueError(f"temperatures must be finite and non-negative, got {temps.tolist()}")
+        mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
+        nu = self._mesh_frequencies(mesh)[0]
+        n_imaginary = (nu < -THERMAL_CUTOFF_THZ).sum()
+        nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0  # q index 0 is Gamma
+        tets = torch.as_tensor(tetrahedra(mesh, self.cell.prim_lattice)).to(self.device)
+        t = None if temps is None else torch.as_tensor(temps).to(self.device)
+        return mesh, nu, n_imaginary, tets, temps, t
+
+    def _joint_dos_chunks(self, mesh, nu, tets, targets, omega, t) -> torch.Tensor:
+        """[Q, 1 + T, 2, F] from ``chg_joint_dos`` over chunks of targets whose output and scratch stay below
+        ``jdos_chunk_bytes``."""
+        n_slots = 1 + (0 if t is None else len(t))
+        per_target = 8 * (JDOS_MAX_CHUNKS + 1) * n_slots * 2 * omega.shape[1]
+        chunk = max(1, self.jdos_chunk_bytes // per_target)
+        out = torch.empty(len(targets), n_slots, 2, omega.shape[1], dtype=torch.float64, device=self.device)
+        for s in range(0, len(targets), chunk):
+            self.kernels.joint_dos(nu, mesh, tets, targets[s : s + chunk], omega[s : s + chunk], t,
+                                   THERMAL_CUTOFF_THZ, out[s : s + chunk])
+        return out
+
+    def joint_dos(self, mesh, qpoints, frequency_points=None, temperatures=None) -> dict:
+        """Two-phonon joint densities of states (phono3py's ``--jdos``) at ``qpoints`` ([Q, 3] or [3], reduced, on the
+        full Gamma-centred ``mesh``: q * mesh integral to 1e-8, else ValueError), in 1/THz:
+
+            D2(1)(q, w) = 1/N sum [d(w + nu1 - nu2) + d(w - nu1 + nu2)]   (class 1: absorption)
+            D2(2)(q, w) = 1/N sum d(w - nu1 - nu2)                        (class 2: decay)
+            N2(1)(q, w; T) = 1/N sum (n1 - n2) [d(w + nu1 - nu2) - d(w - nu1 + nu2)]
+            N2(2)(q, w; T) = 1/N sum (n1 + n2 + 1) d(w - nu1 - nu2)
+
+        over the N mesh points q1 and every ordered band pair, nu1 = nu_l1(q1), nu2 = nu_l2(q - q1) and
+        n = 1 / expm1(h nu / k T) (0 at T = 0).  The deltas are integrated over q1 by the linear tetrahedron method
+        with the tetrahedra of ``dos``.  A corner where nu1 or nu2 is below ``THERMAL_CUTOFF_THZ`` is left out
+        (imaginary and near-zero modes), and so are the three modes of smallest |nu| at Gamma, whatever their value:
+        n ~ k T / h nu diverges for an acoustic mode that force-constant noise lifts above the cutoff.
+
+        Returns ``frequency_points`` [F] (THz; default 201 points from 0 to twice the highest frequency of the mesh),
+        ``jdos`` [Q, 2, F] (classes 1 and 2), ``n_imaginary`` (the modes below -``THERMAL_CUTOFF_THZ`` over the
+        mesh, as in ``thermal_properties``) and, with ``temperatures`` (K, finite and >= 0, else ValueError),
+        ``temperatures`` and ``weighted_jdos`` [T, Q, 2, F].  Frequencies and sums (``chg_joint_dos``) stay on the
+        device until the result is returned."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = q.reshape(-1, 3)
+        m = np.asarray(mesh, dtype=np.int64).reshape(-1)
+        x = q * m
+        if not np.all(np.isfinite(x)) or np.any(np.abs(x - np.round(x)) > 1e-8):
+            raise ValueError(f"qpoints must lie on the {m.tolist()} mesh (q * mesh integral), got {q.tolist()}")
+        mesh, nu, n_imaginary, tets, temps, t = self._jdos_mesh(mesh, temperatures)
+        idx = np.round(x).astype(np.int64) % m
+        targets = torch.as_tensor(((idx[:, 0] * m[1] + idx[:, 1]) * m[2] + idx[:, 2]).astype(np.int32)).to(self.device)
+        if frequency_points is None:
+            top = 2 * nu.max()
+            omega = torch.lerp(torch.zeros_like(top).expand(201), top.expand(201),
+                               torch.arange(201, dtype=torch.float64, device=self.device) / 200)
+        else:
+            omega = torch.as_tensor(np.asarray(frequency_points, dtype=np.float64).reshape(-1)).to(self.device)
+        out = self._joint_dos_chunks(mesh, nu, tets, targets, omega[None].expand(len(q), -1).contiguous(), t)
+        res = {"frequency_points": omega.cpu().numpy(), "jdos": out[:, 0].cpu().numpy(),
+               "n_imaginary": int(n_imaginary)}
+        if temps is not None:
+            res["temperatures"] = temps
+            res["weighted_jdos"] = out[:, 1:].transpose(0, 1).cpu().numpy()
+        if single:
+            res["jdos"] = res["jdos"][0]
+            if temps is not None:
+                res["weighted_jdos"] = res["weighted_jdos"][:, 0]
+        return res
+
+    def phase_space(self, mesh, temperatures=None) -> dict:
+        """The three-phonon phase space: the quantities of ``joint_dos`` per mode, at w = nu_l(q) for every q of the
+        full Gamma-centred ``mesh`` (n1, n2, n3) and every mode l.
+
+        Returns ``frequencies`` [N, 3 n_prim] (THz, the mesh frequencies the sums use: the three modes of smallest |nu|
+        at Gamma set to 0), ``jdos`` [N, 3 n_prim, 2] (classes 1 and 2, 1/THz), ``average_jdos`` [2] (the mean over
+        the modes kept, nu >= ``THERMAL_CUTOFF_THZ``; the screening proxy for anharmonic scattering: a small phase space
+        means weak three-phonon scattering) and ``n_imaginary``; with ``temperatures`` also ``temperatures``,
+        ``weighted_jdos`` [T, N, 3 n_prim, 2] and ``average_weighted_jdos`` [T, 2].  Modes below the cutoff get 0.
+        Every q is a target of ``chg_joint_dos``, in chunks of ``jdos_chunk_bytes``; everything stays on the device
+        until the result is returned."""
+        mesh, nu, n_imaginary, tets, temps, t = self._jdos_mesh(mesh, temperatures)
+        targets = torch.arange(nu.shape[0], dtype=torch.int32, device=self.device)
+        out = self._joint_dos_chunks(mesh, nu, tets, targets, nu, t)  # [N, 1 + T, 2, 3n]
+        kept = nu >= THERMAL_CUTOFF_THZ
+        out = torch.where(kept[:, None, None, :], out, 0.0).permute(1, 0, 3, 2)  # [1 + T, N, 3n, 2]
+        n_kept = kept.sum().clamp_min(1)
+        avg = out.sum(dim=(1, 2)) / n_kept  # [1 + T, 2]
+        res = {"frequencies": nu.cpu().numpy(), "jdos": out[0].cpu().numpy(), "average_jdos": avg[0].cpu().numpy(),
+               "n_imaginary": int(n_imaginary)}
+        if temps is not None:
+            res["temperatures"] = temps
+            res["weighted_jdos"] = out[1:].cpu().numpy()
+            res["average_weighted_jdos"] = avg[1:].cpu().numpy()
+        return res

@@ -582,6 +582,20 @@ int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t
 int chg_thermal_displacements(const double* freqs, const double* eigvecs, int32_t n_q, int32_t n_prim,
                               const double* temperatures, int32_t n_t, double cutoff_thz, double* work, double* acc,
                               void* stream);
+/* Two-phonon joint densities of states at target q-points of the full Gamma-centred mesh n1 x n2 x n3, by the linear
+ * tetrahedron method over q1 (tetrahedra [6][4][3] as chg_tetrahedron_dos), q2 = q - q1 on the mesh, over every
+ * ordered band pair (l1, l2); freqs [n1 n2 n3][n_band] fp64 THz (signed, ascending per q); targets [n_target] mesh
+ * indices; omega [n_target][n_freq] the frequency points of each target; temperatures [n_t] K (fp64, >= 0).
+ *   out [n_target][1 + n_t][2][n_freq]: slot 0 (D2(1), D2(2)), slot 1 + t (N2(1), N2(2)) at temperatures[t], with
+ *   D2(1) = 1/N sum [d(w + nu1 - nu2) + d(w - nu1 + nu2)],  D2(2) = 1/N sum d(w - nu1 - nu2),
+ *   N2(1) = 1/N sum (n1 - n2) [d(w + nu1 - nu2) - d(w - nu1 + nu2)],  N2(2) = 1/N sum (n1 + n2 + 1) d(w - nu1 - nu2),
+ * n = 1 / expm1(h nu / k_B T) (0 at T = 0), every corner with nu1 or nu2 below cutoff_thz left out.  1/THz.
+ * work: CHG_JDOS_MAX_CHUNKS * n_target * (1 + n_t) * 2 * n_freq doubles of scratch.  Deterministic: two kernels,
+ * per-block partial sums added in a fixed order, no atomics.                                                       */
+#define CHG_JDOS_MAX_CHUNKS 64
+int chg_joint_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3, const int32_t* tetrahedra,
+                  const int32_t* targets, int32_t n_target, const double* omega, int32_t n_freq,
+                  const double* temperatures, int32_t n_t, double cutoff_thz, double* out, double* work, void* stream);
 
 #ifdef __cplusplus
 }
