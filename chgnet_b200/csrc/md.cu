@@ -8,7 +8,7 @@
 //                       max |x - x_ref|^2 for the neighbour-list skin test
 //   chg_md_kick       : v += dt/2 F/m ; kinetic energy
 //   chg_fire_step     : FIRE (Bitzek et al. 2006; the reference's default optimizer, dynamics.py:190-204) with its
-//                       state (dt, alpha, counters) in device memory: two launches, no host decision in the loop
+//                       state (dt, alpha, counters) in device memory: four launches, no host decision in the loop
 #include "common.cuh"
 
 namespace chg {
@@ -69,8 +69,9 @@ __global__ void md_kick_kernel(double* __restrict__ v, const double* __restrict_
   if (e_kin != nullptr && (threadIdx.x & 31) == 0 && ke != 0.0) atomicAdd(e_kin, ke);
 }
 
-// FIRE state in device memory: [0] dt, [1] alpha, [2] n_pos (as double), [3] power, [4] |v|^2, [5] |f|^2, [6] max |f_i|^2,
-// [7] max step^2 of the last update
+// FIRE state in device memory (the 12 slots are documented at chg_fire_step in include/chgnet_b200.h): [0] dt, [1] alpha,
+// [2] n_pos (as double); scratch [3] power, [4] |v|^2, [5] |f|^2, [6] max |f_i|^2, [7] max |dt v_i|^2 of this update;
+// published [8..10] the new dt, alpha, n_pos and [11] max |f_i|^2
 __global__ void fire_reduce_kernel(const double* __restrict__ v, const double* __restrict__ f, int n, double* __restrict__ st) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double p = 0.0, vv = 0.0, ff = 0.0;
@@ -94,9 +95,8 @@ __global__ void fire_reduce_kernel(const double* __restrict__ v, const double* _
   }
 }
 
-__global__ void fire_update_kernel(double* __restrict__ x, double* __restrict__ v, const double* __restrict__ f, int n,
-                                   double* __restrict__ st, Mat3 inv_l, double* __restrict__ frac64, float* __restrict__ frac32,
-                                   double dt_max, double max_step) {
+__global__ void fire_update_kernel(double* __restrict__ v, const double* __restrict__ f, int n, double* __restrict__ st,
+                                   double dt_max) {
   // every thread derives the same scalars from the reduced state (written by the previous launch)
   const double n_min = 5.0, f_inc = 1.1, f_dec = 0.5, alpha_start = 0.1, f_alpha = 0.99;
   double dt = st[0], alpha = st[1], n_pos = st[2];
@@ -115,40 +115,47 @@ __global__ void fire_update_kernel(double* __restrict__ x, double* __restrict__ 
   }
   const double mix = uphill ? 0.0 : st[1] * vnorm / fmax(fnorm, 1e-30);
   const double keep = uphill ? 0.0 : 1.0 - st[1];
-  // the largest displacement of this update bounds the step (ase's maxstep): |dr_i| <= dt |v_i| with
-  // |v_new| <= |v| + dt |f|; use the exact per-atom value via a two-phase trick: scale computed from the global maxima
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
-    double dr[3], vn[3], d2 = 0.0;
+    double d2 = 0.0;
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
-      vn[j] = keep * v[3 * i + j] + mix * f[3 * i + j] + dt * f[3 * i + j];
-      dr[j] = dt * vn[j];
-      d2 += dr[j] * dr[j];
+      const double vn = keep * v[3 * i + j] + mix * f[3 * i + j] + dt * f[3 * i + j];
+      const double dr = dt * vn;
+      v[3 * i + j] = vn;
+      d2 += dr * dr;
     }
-    // per-atom clamp to max_step (a conservative form of ase's global rescaling: never moves an atom further)
-    const double s = d2 > max_step * max_step ? max_step / sqrt(d2) : 1.0;
-    double xi[3];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      v[3 * i + j] = vn[j];
-      xi[j] = x[3 * i + j] + s * dr[j];
-      x[3 * i + j] = xi[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double fj = xi[0] * inv_l.m[j] + xi[1] * inv_l.m[3 + j] + xi[2] * inv_l.m[6 + j];
-      frac64[3 * i + j] = fj;
-      frac32[3 * i + j] = (float)fj;
-    }
+    // no atom moves yet: the step limit needs the largest per-atom step of the whole update (fire_move)
+    atomic_max_nonneg(st + 7, d2);
   }
-  __syncthreads();
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
-    // last block publishes the new scalars for the host / the next step; the sums are re-zeroed by the caller
+    // the new scalars for fire_move, the host and the next step
     st[8] = dt;
     st[9] = alpha;
     st[10] = n_pos;
     st[11] = st[6];  // max |f_i|^2 seen by this step
+  }
+}
+
+// x += s dt v with one scale s = min(1, max_step / max_i |dt v_i|) for all atoms (fire_relax's step limit: the update
+// keeps its direction, every atom keeps its share of it); v itself is not scaled
+__global__ void fire_move_kernel(double* __restrict__ x, const double* __restrict__ v, int n, const double* __restrict__ st,
+                                 Mat3 inv_l, double* __restrict__ frac64, float* __restrict__ frac32, double max_step) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double dt = st[8], norm = sqrt(st[7]);
+  const double s = norm > max_step ? max_step / norm : 1.0;
+  double xi[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    xi[j] = x[3 * i + j] + (dt * v[3 * i + j]) * s;
+    x[3 * i + j] = xi[j];
+  }
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const double fj = xi[0] * inv_l.m[j] + xi[1] * inv_l.m[3 + j] + xi[2] * inv_l.m[6 + j];
+    frac64[3 * i + j] = fj;
+    frac32[3 * i + j] = (float)fj;
   }
 }
 
@@ -157,7 +164,7 @@ __global__ void fire_commit_kernel(double* __restrict__ st) {
   st[0] = st[8];
   st[1] = st[9];
   st[2] = st[10];
-  st[3] = st[4] = st[5] = st[6] = 0.0;
+  st[3] = st[4] = st[5] = st[6] = st[7] = 0.0;
 }
 
 inline unsigned blocks(int n) { return (unsigned)((n + 255) / 256); }
@@ -199,7 +206,9 @@ extern "C" int chg_fire_step(double* x, double* v, const double* f, int32_t n_at
   cudaStream_t st = as_stream(stream);
   fire_reduce_kernel<<<blocks(n_atoms), 256, 0, st>>>(v, f, n_atoms, state);
   count_launch();
-  fire_update_kernel<<<blocks(n_atoms), 256, 0, st>>>(x, v, f, n_atoms, state, il, frac64, frac32, dt_max, max_step);
+  fire_update_kernel<<<blocks(n_atoms), 256, 0, st>>>(v, f, n_atoms, state, dt_max);
+  count_launch();
+  fire_move_kernel<<<blocks(n_atoms), 256, 0, st>>>(x, v, n_atoms, state, il, frac64, frac32, max_step);
   count_launch();
   fire_commit_kernel<<<1, 1, 0, st>>>(state);
   CHG_LAUNCH_END();

@@ -191,13 +191,44 @@ class VelocityVerlet:
         return log
 
 
+FIRE_N_MIN, FIRE_F_INC, FIRE_F_DEC, FIRE_ALPHA_START, FIRE_F_ALPHA = 5, 1.1, 0.5, 0.1, 0.99
+
+
+def fire_update(x, v, f, state, dt_max: float = 1.0, max_step: float = 0.2):
+    """One FIRE update (Bitzek et al. 2006) in fp64: the specification of ``fire_relax`` and of ``chg_fire_step``.
+
+    ``x, v, f`` are [N, 3] positions, velocities and forces; ``state = (dt, alpha, n_pos)``.  A step with
+    power f.v > 0 mixes v towards f, counts itself downhill and, after more than ``n_min`` downhill steps in a row,
+    grows dt (capped at ``dt_max``) and decays alpha; any other step (v = 0 included) zeroes v, halves dt and resets
+    alpha and the count.  Then v += dt f and dr = dt v; when the largest per-atom step max_i |dr_i| exceeds
+    ``max_step`` the whole dr is scaled by ``max_step / max_i |dr_i|``, so every atom keeps its direction and its
+    share of the step.  The returned v is not scaled.  Returns ``(x + dr, v, (dt, alpha, n_pos))``; the inputs are
+    not modified."""
+    dt, alpha, n_pos = state
+    power = float((f * v).sum())
+    if power > 0:
+        v = (1 - alpha) * v + alpha * f * np.linalg.norm(v) / max(np.linalg.norm(f), 1e-30)
+        n_pos += 1
+        if n_pos > FIRE_N_MIN:
+            dt, alpha = min(dt * FIRE_F_INC, dt_max), alpha * FIRE_F_ALPHA
+    else:
+        v = np.zeros_like(v)
+        dt, alpha, n_pos = dt * FIRE_F_DEC, FIRE_ALPHA_START, 0
+    v = v + dt * f
+    dr = dt * v
+    norm = np.sqrt((dr**2).sum(axis=1)).max()
+    if norm > max_step:  # ase's maxstep
+        dr *= max_step / norm
+    return x + dr, v, (dt, alpha, n_pos)
+
+
 def fire_relax(atoms, calculator: CHGNetCalculator, fmax: float = 0.1, steps: int = 500, dt: float = 0.1,
-               dt_max: float = 1.0, task: PredTask = "ef") -> dict:
+               dt_max: float = 1.0, task: PredTask = "ef", max_step: float = 0.2) -> dict:
     """Atomic-position relaxation with FIRE (Bitzek et al. 2006; the reference's default optimizer,
-    dynamics.py:190-204), fixed cell.  Returns the trajectory of energies and the final max force."""
-    n_min, f_inc, f_dec, alpha_start, f_alpha = 5, 1.1, 0.5, 0.1, 0.99
+    dynamics.py:190-204), fixed cell, one ``fire_update`` per force evaluation.  Returns the trajectory of
+    energies and the final max force."""
     v = np.zeros_like(atoms.positions)
-    alpha, n_pos = alpha_start, 0
+    state = (dt, FIRE_ALPHA_START, 0)
     energies = []
     for step in range(steps):
         calculator.calculate(atoms, task=task)
@@ -206,19 +237,5 @@ def fire_relax(atoms, calculator: CHGNetCalculator, fmax: float = 0.1, steps: in
         fnorm = float(np.sqrt((f**2).sum(axis=1)).max())
         if fnorm < fmax:
             break
-        power = float((f * v).sum())
-        if power > 0:
-            v = (1 - alpha) * v + alpha * f * np.linalg.norm(v) / max(np.linalg.norm(f), 1e-30)
-            n_pos += 1
-            if n_pos > n_min:
-                dt, alpha = min(dt * f_inc, dt_max), alpha * f_alpha
-        else:
-            v[:] = 0.0
-            dt, alpha, n_pos = dt * f_dec, alpha_start, 0
-        v = v + dt * f
-        dr = dt * v
-        norm = np.sqrt((dr**2).sum(axis=1)).max()
-        if norm > 0.2:  # ase's maxstep
-            dr *= 0.2 / norm
-        atoms.positions = atoms.positions + dr
+        atoms.positions, v, state = fire_update(atoms.positions, v, f, state, dt_max, max_step)
     return {"energies": energies, "fmax": fnorm, "steps": step + 1, "converged": fnorm < fmax}

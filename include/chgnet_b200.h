@@ -339,7 +339,14 @@ int chg_graph_build_device(const double* frac, const double* lattice, int32_t n_
  * (frac = x @ inv_lattice).  frac64 feeds chg_graph_build_device, frac32 is chg_batch.frac.
  *   chg_md_kick_drift: v += dt/2 f/m; x += dt v; frac; max_disp2 (device double, may be NULL) = max |x - x_ref|^2
  *   chg_md_kick      : v += dt/2 f/m; *e_kin (device double, may be NULL) += kinetic energy
- *   chg_fire_step    : one FIRE update with its state in device memory (12 doubles: dt, alpha, n_pos, sums, ...)   */
+ *   chg_fire_step    : one FIRE update (chgnet_b200.dynamics.fire_update) with its state in device memory, 12 doubles:
+ *                        [0] dt, [1] alpha, [2] n_pos (as a double): set by the caller before the first step (e.g. 0.1,
+ *                            0.1, 0), then advanced by every step;
+ *                        [3] power f.v, [4] |v|^2, [5] |f|^2, [6] max_i |f_i|^2, [7] max_i |dt v_i|^2: scratch, zero
+ *                            before the first step and zero again after every step;
+ *                        [8] dt, [9] alpha, [10] n_pos after the step (= [0..2]) and [11] max_i |f_i|^2 of the forces
+ *                            the step used: published for the host.
+ *                      When max_i |dt v_i| > max_step every atom's step is scaled by max_step / max_i |dt v_i|.      */
 int chg_md_kick_drift(double* x, double* v, const double* f, const double* inv_mass, int32_t n_atoms, double dt,
                       const double* inv_lattice, double* frac64, float* frac32, const double* x_ref,
                       double* max_disp2, void* stream);

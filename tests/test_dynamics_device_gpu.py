@@ -20,8 +20,8 @@ def model():
     return CHGNet.from_file(path, version="0.3.0").to("cuda")
 
 
-def _system(seed=4200):
-    z, frac, lat = graphgen.limno2_structure((2, 2, 1), 0.03, seed)
+def _system(seed=4200, rattle=0.03):
+    z, frac, lat = graphgen.limno2_structure((2, 2, 1), rattle, seed)
     return z, frac @ lat, lat
 
 
@@ -85,3 +85,31 @@ def test_device_fire_relaxes(model):
           f"{res['graph_builds']} graph builds")
     assert res["fmax"] < f_start and fire.potential_energy < e_start
     assert res["converged"]
+
+
+def test_device_fire_follows_fire_relax(model, monkeypatch):
+    """DeviceFIRE and the host fire_relax take the same 30 FIRE steps from a hard rattle; the 0.2 A step limit is
+    active on some of them (seen through fire_update on the host trajectory)."""
+    from chgnet_b200 import dynamics
+    from chgnet_b200.dynamics import Atoms, CHGNetCalculator, fire_relax
+    from chgnet_b200.dynamics_device import DeviceFIRE
+
+    steps, dt0 = 30, 0.4
+    z, pos, cell = _system(4203, rattle=0.1)
+    spec, clamped = dynamics.fire_update, []
+
+    def recording_update(x, v, f, state, dt_max, max_step):
+        out = spec(x, v, f, state, dt_max, max_step)
+        clamped.append(bool(np.sqrt(((out[2][0] * out[1]) ** 2).sum(axis=1)).max() > max_step))
+        return out
+
+    monkeypatch.setattr(dynamics, "fire_update", recording_update)
+    host_atoms = Atoms(z, pos, cell)
+    fire_relax(host_atoms, CHGNetCalculator(model=model, on_isolated_atoms="ignore"), fmax=0.0, steps=steps, dt=dt0)
+    dev = DeviceFIRE(model, z, pos, cell, dt=dt0)
+    res = dev.run(fmax=0.0, steps=steps)
+    dx = np.abs(dev.positions() - host_atoms.positions).max()
+    print(f"FIRE {steps} steps: max |x_DeviceFIRE - x_fire_relax| = {dx:.2e} A; step limit active on steps "
+          f"{[i for i, c in enumerate(clamped) if c]}")
+    assert len(clamped) == steps and res["steps"] == steps and any(clamped)
+    assert dx < 1e-4
