@@ -923,13 +923,15 @@ extern "C" int chg_bond_basis_bwd(const float* dist, const int32_t* u2d, int32_t
   CHG_LAUNCH_END();
 }
 
+// The angle-basis entry points take freq == nullptr when n_freq == 0 (num_angular = 1: the constant term only); no
+// lane reads a frequency or writes a frequency gradient then.
 extern "C" int chg_angle_basis_embed(const float* rhat, const int32_t* ang_di, const int32_t* ang_dj,
                                      int32_t n_angles, const float* freq, int32_t n_freq, const float* wt, float* a0,
                                      float* basis_out, void* stream) {
   CHG_CHECK_ARG(n_angles >= 0, "negative size");
   CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
   if (n_angles == 0) return CHG_OK;
-  CHG_CHECK_ARG(rhat && ang_di && ang_dj && freq && wt && a0, "null pointer");
+  CHG_CHECK_ARG(rhat && ang_di && ang_dj && (freq || n_freq == 0) && wt && a0, "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
   angle_basis_embed_kernel<<<warp_grid((n_angles + 3) / 4), 256, smem, as_stream(stream)>>>(rhat, ang_di, ang_dj, n_angles,
                                                                                   freq, n_freq, wt, a0, basis_out);
@@ -941,8 +943,8 @@ extern "C" int chg_angle_basis_bwd(const float* rhat, const int32_t* ang_di, con
                                    double* g_rhat, double* g_freq, void* stream) {
   CHG_CHECK_ARG(n_angles >= 0, "negative size");
   CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
-  if (n_angles == 0) return CHG_OK;
-  CHG_CHECK_ARG(rhat && ang_di && ang_dj && freq && w && g_a0 && (g_rhat || g_freq), "null pointer");
+  if (n_angles == 0 || (g_rhat == nullptr && n_freq == 0)) return CHG_OK;  // num_angular = 1: g_freq has no entries
+  CHG_CHECK_ARG(rhat && ang_di && ang_dj && (freq || n_freq == 0) && w && g_a0 && (g_rhat || g_freq), "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
   angle_basis_bwd_kernel<<<warp_grid((n_angles + 15) / 16), 256, smem, as_stream(stream)>>>(rhat, ang_di, ang_dj, n_angles, freq,
                                                                                 n_freq, w, g_a0, g_rhat, g_freq);
@@ -1033,7 +1035,7 @@ extern "C" int chg_angle_basis_tangent(const float* rhat, const float* drhat, co
   CHG_CHECK_ARG(n_angles >= 0, "negative size");
   CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
   if (n_angles == 0) return CHG_OK;
-  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && freq && wt && a0d && tbasis, "null pointer");
+  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && (freq || n_freq == 0) && wt && a0d && tbasis, "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
   angle_basis_tangent_kernel<<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(rhat, drhat, ang_di, ang_dj, n_angles,
                                                                                    freq, n_freq, wt, a0d, tbasis);
@@ -1045,8 +1047,8 @@ extern "C" int chg_angle_basis_bwd2(const float* rhat, const float* drhat, const
                                     const float* lam_a0, double* g_freq, void* stream) {
   CHG_CHECK_ARG(n_angles >= 0, "negative size");
   CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
-  if (n_angles == 0) return CHG_OK;
-  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && freq && w && lam_a0 && g_freq, "null pointer");
+  if (n_angles == 0 || n_freq == 0) return CHG_OK;  // num_angular = 1: g_freq has no entries
+  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && (freq || n_freq == 0) && w && lam_a0 && g_freq, "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
   angle_basis_bwd2_kernel<false><<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(
       rhat, drhat, ang_di, ang_dj, n_angles, freq, n_freq, w, lam_a0, g_freq, nullptr);
@@ -1059,7 +1061,7 @@ extern "C" int chg_angle_basis_hvp(const float* rhat, const float* drhat, const 
   CHG_CHECK_ARG(n_angles >= 0, "negative size");
   CHG_CHECK_ARG(n_freq >= 0 && 2 * n_freq + 1 <= MAX_BASIS, "num_angular must be odd and <= 31");
   if (n_angles == 0) return CHG_OK;
-  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && freq && w && lam_a0 && g_rhat, "null pointer");
+  CHG_CHECK_ARG(rhat && drhat && ang_di && ang_dj && (freq || n_freq == 0) && w && lam_a0 && g_rhat, "null pointer");
   const int smem = (2 * n_freq + 1) * 64 * 4;
   angle_basis_bwd2_kernel<true><<<warp_grid(n_angles), 256, smem, as_stream(stream)>>>(
       rhat, drhat, ang_di, ang_dj, n_angles, freq, n_freq, w, lam_a0, nullptr, g_rhat);

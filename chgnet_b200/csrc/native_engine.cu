@@ -384,7 +384,8 @@ int run_schedule(const chg_hparams& hp, const Weights& W, const chg_batch& b, co
                                               hp.bond_graph_cutoff, hp.cutoff_coeff, W.w3, g_e, g_wag, g_wbg_full, g_dist, nullptr, st));
   double* g_rhat = static_cast<double*>(c.ar.tmp((size_t)Ed * 3 * 8));
   c.zero(g_rhat, (size_t)Ed * 24);
-  if (has_ang)
+  // with one block no BondConv reverse ran: the angle features feed nothing, dE/d(angle basis) = 0 and g_rhat stays zero
+  if (has_ang && g_a_live)
     RUN(c, "angle_basis_bwd", chg_angle_basis_bwd(rhat, b.ang_di, b.ang_dj, A, W.freq_ang, (hp.num_angular - 1) / 2, W.wang, g_a,
                                                   g_rhat, nullptr, st));
   c.zero(o.force, (size_t)N * 24);

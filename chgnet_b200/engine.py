@@ -525,7 +525,7 @@ class Engine:
         K.bond_basis_bwd2(dist, ddist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
                           hp.cutoff_coeff, pw.w3, rec["g_e0"], rec["g_wag"], rec["g_wbg_full"], g_freq)
         G["freq_ag"], G["freq_bg"] = g_freq[0].to(dt), g_freq[1].to(dt)
-        if has_ang:
+        if bar_a is not None:  # None with one block (no angle adjoint, rec["g_a0"] is None too)
             G["wang_t"] = wsum(tr["fb"], bar_a, 64, tfb, rec["g_a0"])[:NA]
             g_fa = self._zeros(b, pw.freq_ang.shape[0], dtype=torch.float64)
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, bar_a, None, g_fa)
@@ -551,7 +551,7 @@ class Engine:
         K.bond_basis_hvp(dist, ddist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
                          hp.cutoff_coeff, pw.w3, rec["g_e0"], rec["g_wag"], rec["g_wbg_full"], g_dist)
         g_rhat = self._zeros(b, b.n_edges, 3, dtype=torch.float64)
-        if b.n_angles > 0:
+        if bar_a is not None:  # None with one block: no angle adjoint
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, bar_a, g_rhat)
             K.angle_basis_hvp(rhat, drhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, rec["g_a0"], g_rhat)
         neg_hv = self._zeros(b, b.n_atoms, 3, dtype=torch.float64)
@@ -747,7 +747,7 @@ class Engine:
             K.bond_basis_bwd(dist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
                              hp.cutoff_coeff, pw.w3, g_e, g_wag, g_wbg_full, g_dist, g_freq)
             G["freq_ag"], G["freq_bg"] = g_freq[0].to(g_e.dtype), g_freq[1].to(g_e.dtype)
-            if has_ang:
+            if g_a is not None:  # None with one block: the angle features feed nothing
                 G["wang_t"] = self._wgrad(b, tr["fb"], g_a, 64)[:NA]
                 g_fa = self._zeros(b, pw.freq_ang.shape[0], dtype=torch.float64)
                 K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, g_a, None, g_fa)
@@ -758,7 +758,7 @@ class Engine:
         K.bond_basis_bwd(dist, b.u2d, pw.freq_ag, pw.freq_bg, hp.atom_graph_cutoff, hp.bond_graph_cutoff,
                          hp.cutoff_coeff, pw.w3, g_e, g_wag, g_wbg_full, g_dist)
         g_rhat = self._zeros(b, Ed, 3, dtype=torch.float64)
-        if has_ang:
+        if g_a is not None:  # with one block no BondConv reverse ran: dE/d(angle basis) = 0, g_rhat stays zero
             K.angle_basis_bwd(rhat, b.ang_di, b.ang_dj, pw.freq_ang, pw.wang, g_a, g_rhat)
         if rec is not None:  # adjoints of the tangent inputs ddist, drhat (Hessian-vector products)
             rec.update(g_dist=g_dist, g_rhat=g_rhat)

@@ -14,7 +14,9 @@ kernels through the C ABI — inference as ONE native call (``chg_forward``,
 (``e / f / s / m`` then carry autograd history to the parameters).  No CPU path.
 
 Limits (raise, never fall back): feature dims must be 64, GatedMLP hidden dims 64 (conv) /
-0 (angle), layer- or no normalisation, ``mlp_first=True``.
+0 (angle), layer- or no normalisation, ``mlp_first=True``, ``num_radial`` 1..32, odd ``num_angular``
+1..31, ``n_conv`` 1..8, 1 to 4 readout hidden layers of width 64; a one-block model has no magnetic
+moments (the reference reads them after block ``n_conv - 1``).
 """
 from __future__ import annotations
 
@@ -32,7 +34,7 @@ from chgnet_b200 import PredTask
 from chgnet_b200.batch import DeviceBatch, build_batch
 from chgnet_b200.engine import EV_A3_TO_GPA, Engine
 from chgnet_b200.graph import CrystalGraph, is_graph_like
-from chgnet_b200.weights import pack_weights, unpack_grads
+from chgnet_b200.weights import check_architecture, pack_weights, unpack_grads
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _REPO = os.path.dirname(_HERE)
@@ -387,6 +389,9 @@ class CHGNet(nn.Module):
             raise NotImplementedError("chgnet_b200 kernels implement mlp_first=True (per-site energies) only")
         if conv_dropout or mlp_dropout:
             raise NotImplementedError("dropout is not implemented (all pretrained models use 0)")
+        widths = [] if mlp_hidden_dims in (None, 0) else (
+            [mlp_hidden_dims] if isinstance(mlp_hidden_dims, int) else list(mlp_hidden_dims))
+        check_architecture(num_radial, num_angular, n_conv, widths)
         self.atom_fea_dim, self.bond_fea_dim = atom_fea_dim, bond_fea_dim
         self.is_intensive, self.n_conv, self.mlp_first = is_intensive, n_conv, mlp_first
         a = dict(self.model_args)
@@ -503,6 +508,9 @@ class CHGNet(nn.Module):
         Inference = one native ``chg_forward`` call (native.py; ``CHGNET_B200_ENGINE=python`` selects the
         call-by-call Python schedule of engine.py instead, same kernels); training = engine.py."""
         need_grad = "f" in task or "s" in task
+        if "m" in task and self.n_conv < 2:
+            raise ValueError(f"n_conv={self.n_conv}: magnetic moments are read after block n_conv - 1, which a model "
+                             "with one block does not have (task without 'm')")
         # mlp_out bias (0.2.0) touches every bond: no bond-graph compaction in that case
         compact = not self._arch.get("mlp_out_bias", False)
         if batch is None:

@@ -17,9 +17,7 @@ from torch import Tensor
 
 from chgnet_b200._lib import ChgnetB200Error, load_library
 from chgnet_b200.batch import DeviceBatch
-from chgnet_b200.weights import HyperParams, infer_hyper_params
-
-MAX_CONV = 8
+from chgnet_b200.weights import MAX_CONV, HyperParams, infer_hyper_params, readout_layer_indices
 FP = POINTER(c_float)
 
 
@@ -125,8 +123,7 @@ def pack_weights_native(state_dict: dict, model_args: dict | None = None) -> tup
     for t in range(hp.n_conv - 1):
         s.bond[t] = gated(f"bond_conv_layers.{t}.twoBody_bond", "layers.0", "layers.3", f"bond_conv_layers.{t}.mlp_out.layers.1")
         s.angle[t] = gated(f"angle_layers.{t}.twoBody_bond", "layers.1", None, None)
-    hidden = sorted(int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight") and sd[k].shape[0] == 64)
-    last = max(int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight"))
+    hidden, last = readout_layer_indices(sd)
     for l, i in enumerate(hidden):
         s.mlp_w[l], s.mlp_b[l] = ptr(f"mlp.layers.{i}.weight"), ptr(f"mlp.layers.{i}.bias")
     s.mlp_last_w, s.mlp_last_b = ptr(f"mlp.layers.{last}.weight"), float(sd[f"mlp.layers.{last}.bias"].reshape(-1)[0])

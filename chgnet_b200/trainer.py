@@ -141,6 +141,9 @@ class Trainer:
         self.model = model
         self.cfg = LossConfig(targets, criterion, energy_loss_ratio, force_loss_ratio, stress_loss_ratio,
                               mag_loss_ratio, delta)
+        if "m" in targets and model.n_conv < 2:
+            raise ValueError(f"n_conv={model.n_conv}: magnetic moments are read after block n_conv - 1, which a model "
+                             f"with one block does not have (targets={targets!r})")
         self.lr, self.weight_decay, self.betas, self.eps = learning_rate, weight_decay, betas, eps
         self.group = process_group
         self.step_count = 0

@@ -83,6 +83,38 @@ def _ln_pack(sd: dict, prefix: str) -> Tensor | None:
     ).contiguous()
 
 
+MAX_CONV = 8  # CHG_MAX_CONV (include/chgnet_b200.h)
+MAX_READOUT_HIDDEN = 4  # MAX_HIDDEN of csrc/readout.cu and csrc/train.cu
+
+
+def check_architecture(num_radial: int, num_angular: int, n_conv: int, readout_widths: list[int]) -> None:
+    """Raise for a shape the kernels cannot run.  The radial basis is one lane of a warp per function (1..32), the
+    Fourier basis one lane per function with the constant term (odd, 1..31), the native schedule holds up to
+    ``MAX_CONV`` blocks, and the readout kernels take 1..``MAX_READOUT_HIDDEN`` hidden layers of width 64."""
+    if not 1 <= num_radial <= 32:
+        raise ValueError(f"num_radial={num_radial} is outside 1..32 (the radial basis is one warp lane per function)")
+    if not 1 <= num_angular <= 31 or num_angular % 2 != 1:
+        raise ValueError(f"num_angular={num_angular} must be odd and within 1..31 (one warp lane per Fourier function)")
+    if not 1 <= n_conv <= MAX_CONV:
+        raise ValueError(f"n_conv={n_conv} is outside 1..{MAX_CONV}")
+    if not 1 <= len(readout_widths) <= MAX_READOUT_HIDDEN:
+        raise NotImplementedError(f"mlp_hidden_dims={list(readout_widths)}: the readout kernels take 1 to "
+                                  f"{MAX_READOUT_HIDDEN} hidden layers")
+    if any(int(w) != 64 for w in readout_widths):
+        raise NotImplementedError(f"mlp_hidden_dims={list(readout_widths)}: every readout hidden layer must be 64 wide")
+
+
+def readout_layer_indices(sd: dict) -> tuple[list[int], int]:
+    """(hidden Linear indices, last Linear index) of the readout MLP ``mlp.layers.*``, found as the reference's forward
+    walks it (functions.py:81-92): hidden Linears at 0, 2, 4 ... while the layer exists and does not map to one output."""
+    hidden, idx = [], 0
+    while f"mlp.layers.{idx}.weight" in sd and sd[f"mlp.layers.{idx}.weight"].shape[0] != 1:
+        hidden.append(idx)
+        idx += 2
+    last = max(int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight"))
+    return hidden, last
+
+
 def infer_hyper_params(sd: dict, model_args: dict | None = None) -> HyperParams:
     a = model_args or {}
     hp = HyperParams()
@@ -95,7 +127,8 @@ def infer_hyper_params(sd: dict, model_args: dict | None = None) -> HyperParams:
     hp.use_ln = "atom_conv_layers.0.twoBody_atom.bn1.weight" in sd
     hp.readout_ln = "readout_norm.weight" in sd
     hp.is_intensive = bool(a.get("is_intensive", True))
-    hidden = [k for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight") and sd[k].shape[0] == 64]
+    hidden, _ = readout_layer_indices(sd)
+    check_architecture(hp.num_radial, hp.num_angular, hp.n_conv, [sd[f"mlp.layers.{i}.weight"].shape[0] for i in hidden])
     hp.n_readout_hidden = len(hidden)
     return hp
 
@@ -173,10 +206,7 @@ def pack_weights(state_dict: dict, model_args: dict | None = None, device=None, 
         )
         angle.append(gp)
 
-    hidden_idx = sorted(
-        int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight") and sd[k].shape[0] == 64
-    )
-    last_idx = max(int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight"))
+    hidden_idx, last_idx = readout_layer_indices(sd)
     mlp_w = torch.stack([sd[f"mlp.layers.{i}.weight"] for i in hidden_idx]).contiguous()
     return PackedWeights(
         hp=hp,
@@ -275,10 +305,7 @@ def unpack_grads(G: dict, state_dict: dict) -> dict[str, Tensor]:
     if "readout_ln" in G:
         put("readout_norm.weight", G["readout_ln"][0])
         put("readout_norm.bias", G["readout_ln"][1])
-    hidden_idx = sorted(
-        int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight") and sd[k].shape[0] == 64
-    )
-    last_idx = max(int(k.split(".")[2]) for k in sd if k.startswith("mlp.layers.") and k.endswith(".weight"))
+    hidden_idx, last_idx = readout_layer_indices(sd)
     for l, i in enumerate(hidden_idx):
         put(f"mlp.layers.{i}.weight", G["mlp_wt"][l].T)
         put(f"mlp.layers.{i}.bias", G["mlp_b"][l])
