@@ -21,10 +21,16 @@ void set_error(const char* fmt, ...) {
 }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
-int sm_count() {  // of the CURRENT device (cached per device ordinal)
-  static std::atomic<int> cache[64];
+int device_ordinal() {
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;  // H100 SXM
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEVICES) return 0;
+  return dev;
+}
+
+int sm_count() {  // of the CURRENT device (cached per device ordinal)
+  static std::atomic<int> cache[MAX_DEVICES];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEVICES) return 132;  // H100 SXM
   int n = cache[dev].load(std::memory_order_relaxed);
   if (n == 0) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;

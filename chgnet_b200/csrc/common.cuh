@@ -11,6 +11,11 @@ namespace chg {
 void set_error(const char* fmt, ...);
 void count_launch();
 int sm_count();
+// ordinal of the current device, the index of the per-device caches of launch set-up: cudaFuncSetAttribute and the
+// occupancy it enables belong to each device's context, so a flag kept once per process would skip them on a second
+// device and its large-shared-memory launches would fail
+constexpr int MAX_DEVICES = 64;
+int device_ordinal();
 int linear_impl();  // 0 = FFMA, 1..3 = tensor cores (wgmma)
 int gated_impl();
 int segsum_unroll();   // 4 or 8 input rows in flight per lane-group of chg_segment_sum

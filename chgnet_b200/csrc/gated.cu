@@ -706,7 +706,8 @@ template <int MODE>
 int launch_fwd(const FwdArgs& a, cudaStream_t stream) {
   if (a.n_rows == 0) return CHG_OK;
   constexpr int smem = FwdSmem<MODE>::TOTAL_BYTES;
-  static int slots = 0;
+  static int slots_of[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& slots = slots_of[device_ordinal()];
   if (slots == 0) {
     CHG_CUDA(cudaFuncSetAttribute(gated_fwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     slots = resident_ctas(gated_fwd_kernel<MODE>, smem);
@@ -722,7 +723,8 @@ int launch_bwd_t(const BwdArgs& a, cudaStream_t stream) {
   // the TRAIN epilogue reduces through 16 x 256 floats of shared memory
   constexpr int smem = TRAIN ? (BwdSmem<MODE>::TOTAL_BYTES > 16 * 256 * 4 ? BwdSmem<MODE>::TOTAL_BYTES : 16 * 256 * 4)
                              : BwdSmem<MODE>::TOTAL_BYTES;
-  static int slots = 0;
+  static int slots_of[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& slots = slots_of[device_ordinal()];
   if (slots == 0) {
     CHG_CUDA(cudaFuncSetAttribute(gated_bwd_kernel<MODE, TRAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     slots = resident_ctas(gated_bwd_kernel<MODE, TRAIN>, smem);
@@ -767,8 +769,8 @@ extern "C" int chg_atom_conv_fwd(const float* pcn, const float* pe, const float*
   const bool train = save_pre != nullptr;  // training extras exist in the default implementation only
   if (gated_impl() == 1 && !train) return atom_conv_fwd_tc(a, as_stream(stream));  // 3 (fused default) -> FFMA here
   if (gated_impl() == 2 && !train) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
-    static int slots = 0;
-    return launch2(gated2_fwd_kernel<ATOM>, a, slots, as_stream(stream));
+    static int slots[MAX_DEVICES] = {};
+    return launch2(gated2_fwd_kernel<ATOM>, a, slots[device_ordinal()], as_stream(stream));
   }
   return launch_fwd<ATOM>(a, as_stream(stream));
 }
@@ -785,8 +787,8 @@ extern "C" int chg_atom_conv_bwd(const float* pcn, const float* pe, const float*
   if (gated_impl() == 3 && !train && n_edges >= ws_min_rows()) return atom_conv_bwd_ws(a, as_stream(stream));  // warp-specialised wgmma (default)
   if (gated_impl() == 1 && !train) return atom_conv_bwd_tc(a, as_stream(stream));
   if (gated_impl() == 2 && !train) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
-    static int slots = 0;
-    return launch2(gated2_bwd_kernel<ATOM>, a, slots, as_stream(stream));
+    static int slots[MAX_DEVICES] = {};
+    return launch2(gated2_bwd_kernel<ATOM>, a, slots[device_ordinal()], as_stream(stream));
   }
   return launch_bwd<ATOM>(a, as_stream(stream));
 }
@@ -801,8 +803,8 @@ extern "C" int chg_bond_conv_fwd(const float* pij, const float* px, const float*
   FwdArgs a{pij, px, pa, nullptr, wbg, ang_i, ang_j, ang_atom, n_angles, w2t, b2, ln, upd, save_pre, save_p};
   if (gated_impl() == 1) return bond_conv_fwd_tc(a, as_stream(stream));
   if (gated_impl() == 2) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
-    static int slots = 0;
-    return launch2(gated2_fwd_kernel<BOND>, a, slots, as_stream(stream));
+    static int slots[MAX_DEVICES] = {};
+    return launch2(gated2_fwd_kernel<BOND>, a, slots[device_ordinal()], as_stream(stream));
   }
   return launch_fwd<BOND>(a, as_stream(stream));
 }
@@ -820,8 +822,8 @@ extern "C" int chg_bond_conv_bwd(const float* save_pre, const float* save_p, con
   if (gated_impl() == 3 && !train && n_angles >= ws_min_rows()) return bond_conv_bwd_ws(a, as_stream(stream));  // warp-specialised wgmma (default)
   if (gated_impl() == 1 && !train) return bond_conv_bwd_tc(a, as_stream(stream));
   if (gated_impl() == 2 && !train) {  // 8x8-tile variant (measured slower end to end; kept for A/B)
-    static int slots = 0;
-    return launch2(gated2_bwd_kernel<BOND>, a, slots, as_stream(stream));
+    static int slots[MAX_DEVICES] = {};
+    return launch2(gated2_bwd_kernel<BOND>, a, slots[device_ordinal()], as_stream(stream));
   }
   return launch_bwd<BOND>(a, as_stream(stream));
 }

@@ -449,7 +449,8 @@ template <int MODE>
 int launch_tan(const TanArgs& a, cudaStream_t stream) {
   if (a.n_rows == 0) return CHG_OK;
   constexpr int smem = TanSmem<MODE>::TOTAL_BYTES;
-  static int slots = 0;
+  static int slots_of[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& slots = slots_of[device_ordinal()];
   if (slots == 0) {
     CHG_CUDA(cudaFuncSetAttribute(gated_tan_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     slots = resident_ctas(gated_tan_kernel<MODE>, smem);
@@ -463,7 +464,8 @@ template <int MODE>
 int launch_bwd2(const Bwd2Args& a, cudaStream_t stream) {
   if (a.n_rows == 0) return CHG_OK;
   constexpr int smem = Bwd2Smem<MODE>::TOTAL_BYTES;
-  static int slots = 0;
+  static int slots_of[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& slots = slots_of[device_ordinal()];
   if (slots == 0) {
     CHG_CUDA(cudaFuncSetAttribute(gated_bwd2_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     slots = resident_ctas(gated_bwd2_kernel<MODE>, smem);

@@ -335,10 +335,11 @@ template <int MODE>
 int launch_fused(const FusedArgs& a, cudaStream_t stream) {
   if (a.n_seg == 0) return CHG_OK;
   if (a.n_rows > 0) {
-    static bool attr_set = false;
-    if (!attr_set) {
+    static bool attr_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+    bool& set = attr_set[device_ordinal()];
+    if (!set) {
       CHG_CUDA(cudaFuncSetAttribute(gated_ws_fwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, WsSmem::TOTAL));
-      attr_set = true;
+      set = true;
     }
     const int n_tiles = (a.n_rows + TR - 1) / TR;
     gated_ws_fwd_kernel<MODE><<<min(n_tiles, sm_count()), WS_THREADS, WsSmem::TOTAL, stream>>>(a);
@@ -669,10 +670,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
 template <int MODE>
 int launch_ws_bwd(const BwdArgs& a, cudaStream_t stream) {
   if (a.n_rows == 0) return CHG_OK;
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  bool& set = attr_set[device_ordinal()];
+  if (!set) {
     CHG_CUDA(cudaFuncSetAttribute(gated_ws_bwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, WsBwdSmem::TOTAL));
-    attr_set = true;
+    set = true;
   }
   const int n_tiles = (a.n_rows + TR - 1) / TR;
   gated_ws_bwd_kernel<MODE><<<min(n_tiles, sm_count()), WS_THREADS, WsBwdSmem::TOTAL, stream>>>(a);

@@ -109,10 +109,11 @@ template <int NT>
 int launch_linear(const float* x, const int32_t* x_rows, int m, int k, const float* wt, const float* bias,
                   const float* residual, const int32_t* y_rows, int n_out, float* y, cudaStream_t stream) {
   const int smem = (k * NT + TM * XS) * 4;
-  static int max_smem_set = 0;
-  if (smem > max_smem_set) {
+  static int max_smem_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& smem_set = max_smem_set[device_ordinal()];
+  if (smem > smem_set) {
     CHG_CUDA(cudaFuncSetAttribute(linear_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_smem_set = smem;
+    smem_set = smem;
   }
   const int n_tiles = (m + TM - 1) / TM;
   const int col_tiles = n_out / NT;

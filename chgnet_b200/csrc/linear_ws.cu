@@ -200,10 +200,11 @@ template <int NT>
 int launch_ws(const CUtensorMap& mx, const CUtensorMap& my, const CUtensorMap& mr, int m, int k, const float* wt,
               const float* bias, int has_residual, int n_out, cudaStream_t stream) {
   const int smem = S_IN * IN_STAGE + (NT / 32) * PANEL + 2 * NT * k * 4 + 1024;
-  static int max_smem_set = 0;
-  if (smem > max_smem_set) {
+  static int max_smem_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& smem_set = max_smem_set[device_ordinal()];
+  if (smem > smem_set) {
     CHG_CUDA(cudaFuncSetAttribute(linear_ws_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_smem_set = smem;
+    smem_set = smem;
   }
   const int n_tiles = (m + 127) / 128;
   const int col_tiles = n_out / NT;

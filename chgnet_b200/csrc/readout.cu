@@ -124,10 +124,11 @@ extern "C" int chg_readout(const float* x, const int32_t* z, const int32_t* atom
                 "null pointer");
   CHG_CHECK_ARG(g_x == nullptr || mlp_w != nullptr, "mlp_w is required when g_x is requested");
   const int smem = 2 * n_hidden * 4096 * 4;
-  static int max_smem_set = 0;
-  if (smem > max_smem_set) {
+  static int max_smem_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& smem_set = max_smem_set[device_ordinal()];
+  if (smem > smem_set) {
     CHG_CUDA(cudaFuncSetAttribute(readout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_smem_set = smem;
+    smem_set = smem;
   }
   const int blocks = max(1, min((n_atoms + 7) / 8, sm_count() * 2));
   readout_kernel<<<blocks, 256, smem, as_stream(stream)>>>(x, z, atom_owner, n_atoms, ln, mlp_wt, mlp_w, mlp_b,

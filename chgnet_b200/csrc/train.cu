@@ -561,10 +561,11 @@ extern "C" int chg_readout_bwd(const float* x, int32_t n_atoms, const float* ln,
   CHG_CHECK_ARG(x && mlp_wt && mlp_w && mlp_b && w_last && seed && g_x && h_all && gz_all && g_h0, "null pointer");
   CHG_CHECK_ARG(ln == nullptr || xhat != nullptr, "xhat is required with LayerNorm");
   const int smem = 2 * n_hidden * 4096 * 4;
-  static int max_smem_set = 0;
-  if (smem > max_smem_set) {
+  static int max_smem_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& smem_set = max_smem_set[device_ordinal()];
+  if (smem > smem_set) {
     CHG_CUDA(cudaFuncSetAttribute(readout_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_smem_set = smem;
+    smem_set = smem;
   }
   const int blocks = max(1, min((n_atoms + 7) / 8, sm_count() * 2));
   readout_bwd_kernel<<<blocks, 256, smem, as_stream(stream)>>>(x, n_atoms, ln, mlp_wt, mlp_w, mlp_b, n_hidden, w_last,
@@ -615,10 +616,11 @@ extern "C" int chg_readout_bwd2(const float* x, const float* xd, int32_t n_atoms
                     g_h0 && hbar0, "null pointer");
   CHG_CHECK_ARG(ln == nullptr || (xhat != nullptr && xhatd != nullptr), "xhat / xhatd are required with LayerNorm");
   const int smem = 2 * n_hidden * 4096 * 4;
-  static int max_smem_set = 0;
-  if (smem > max_smem_set) {
+  static int max_smem_set[MAX_DEVICES] = {};  // per device: the attribute belongs to its context
+  int& smem_set = max_smem_set[device_ordinal()];
+  if (smem > smem_set) {
     CHG_CUDA(cudaFuncSetAttribute(readout_bwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_smem_set = smem;
+    smem_set = smem;
   }
   const int blocks = max(1, min((n_atoms + 7) / 8, sm_count() * 2));
   readout_bwd2_kernel<<<blocks, 256, smem, as_stream(stream)>>>(x, xd, n_atoms, ln, mlp_wt, mlp_w, mlp_b, n_hidden, w_last,

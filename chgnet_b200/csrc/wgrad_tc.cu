@@ -180,10 +180,11 @@ int wgrad_tc(const float* x, const float* x2, int ldx, const int32_t* x_rows, in
   dim3 grid(n_chunks, col_blocks);
 #define CHG_WT(ACT_, GG_)                                                                                                   \
   do {                                                                                                                      \
-    static bool attr = false;                                                                                               \
-    if (!attr) {                                                                                                            \
+    static bool attr[MAX_DEVICES] = {}; /* per device: the attribute belongs to its context */                            \
+    bool& set = attr[device_ordinal()];                                                                                     \
+    if (!set) {                                                                                                             \
       CHG_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<ACT_, GG_>, cudaFuncAttributeMaxDynamicSharedMemorySize, WT_SMEM));      \
-      attr = true;                                                                                                          \
+      set = true;                                                                                                           \
     }                                                                                                                       \
     wgrad_tc_kernel<ACT_, GG_><<<grid, WT_THREADS, WT_SMEM, stream>>>(x, x2, ldx, x_rows, g, ldg, g_rows, m, n_out, n_block, \
                                                                       partial, cs_partial);                                 \

@@ -37,16 +37,7 @@ def _second_order_recorder():
     from oracle.elastic import ElasticSpecKernels
 
     class Recorder(RecordingKernels, ElasticSpecKernels):
-        def __getattribute__(self, name):
-            attr = super().__getattribute__(name)
-            if name in replay_fp64.SECOND_DERIV_OUT_ARGS:
-                def wrapped(*args):
-                    snap = [a.detach().clone().contiguous() if isinstance(a, torch.Tensor) else a for a in args]
-                    attr(*args)
-                    outs = {i: args[i].detach().clone().contiguous() for i in replay_fp64.SECOND_DERIV_OUT_ARGS[name]}
-                    self.calls.append((name, snap, outs))
-                return wrapped
-            return attr
+        recorded = replay_fp64.ALL_OUT_ARGS
 
     return Recorder()
 

@@ -5,6 +5,7 @@ column as given)."""
 import copy
 import dataclasses
 
+import dense_cells
 import numpy as np
 import pytest
 import torch
@@ -33,10 +34,10 @@ def _cases():
     z, frac, lat = graphgen.limno2_structure((3, 2, 2), 0.02, 4001)
     big = graphgen.make_crystal_graph(z, frac, lat)
     return [graphgen.random_graphs(5, 8, 30, 9100), [g_iso], [g_far], [g_thin], [g_iso, g_far, g_thin] + graphgen.random_graphs(2, 9, 12, 9200),
-            graphgen.random_graphs(40, 10, 30, 1000), [big]]
+            graphgen.random_graphs(40, 10, 30, 1000), [big], dense_cells.dense_graphs()]
 
 
-@pytest.mark.parametrize("case", range(7))
+@pytest.mark.parametrize("case", range(8))
 def test_wire_format_equals_full_format_cpu(case):
     graphs = _cases()[case]
     _assert_same(build_batch(graphs, "cpu", wire=True), build_batch(graphs, "cpu", wire=False))

@@ -33,21 +33,12 @@ SD_OUT_ARGS = {"bond_basis_hvp": [12], "angle_basis_hvp": [7], "edge_tangent_bwd
 
 
 def _recording_kernels():
-    from kernel_replay import RecordingKernels
+    from kernel_replay import OUT_ARGS, RecordingKernels
 
     from oracle.elastic import ElasticSpecKernels
 
     class SdRecordingKernels(RecordingKernels, ElasticSpecKernels):
-        def __getattribute__(self, name):
-            attr = super().__getattribute__(name)
-            if name in SD_OUT_ARGS:
-                def wrapped(*args):
-                    snap = [a.detach().clone().contiguous() if isinstance(a, torch.Tensor) else a for a in args]
-                    attr(*args)
-                    outs = {i: args[i].detach().clone().contiguous() for i in SD_OUT_ARGS[name]}
-                    self.calls.append((name, snap, outs))
-                return wrapped
-            return attr
+        recorded = {**OUT_ARGS, **SD_OUT_ARGS}
 
     return SdRecordingKernels()
 

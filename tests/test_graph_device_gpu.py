@@ -6,6 +6,7 @@ undirected2directed, bond_graph - on the cases of the reference's own graph test
 5 / 3, 672 / 744 / 336 at 6 / 3, the 2 x 2 x 6 supercell's 9216 / 17856 / 4608: reference
 tests/test_crystal_graph.py:22-42, 256-278), random cells, cells thinner than the cutoff, fractional coordinates outside
 [0, 1), isolated atoms, an empty bond graph - and the model must give the same answer through either path."""
+import dense_cells
 import numpy as np
 import pytest
 import torch
@@ -73,6 +74,12 @@ def test_edge_cases():
     assert len(g.atom_graph) > 0 and len(g.bond_graph) == 0
     # a single atom whose only neighbours are its own images
     _check([26], np.zeros((1, 3)), np.eye(3) * 2.5)
+    # hundreds of neighbours per centre: rattled diamond (158 edges per atom), and the 3.3 A simple cubic H/Li cell,
+    # thinner than the cutoff, with about 700 edges and 6 800 angles per atom
+    g = _check(*dense_cells.diamond())
+    assert int(np.bincount(g.atom_graph[:, 0].numpy()).max()) > 128
+    g = _check(*dense_cells.simple_cubic_hli())
+    assert int(np.bincount(g.atom_graph[:, 0].numpy()).max()) > 512 and int(np.bincount(g.bond_graph[:, 0].numpy()).max()) > 4096
 
 
 def test_c4_sized_cell_and_time(builder):

@@ -29,21 +29,12 @@ HVP_OUT_ARGS = {"bond_basis_hvp": [12], "angle_basis_hvp": [7], "edge_tangent_bw
 
 
 def _recording_kernels():
-    from kernel_replay import RecordingKernels
+    from kernel_replay import OUT_ARGS, RecordingKernels
 
     from oracle.hessian import HessianSpecKernels
 
     class HvpRecordingKernels(RecordingKernels, HessianSpecKernels):
-        def __getattribute__(self, name):
-            attr = super().__getattribute__(name)
-            if name in HVP_OUT_ARGS:
-                def wrapped(*args):
-                    snap = [a.detach().clone().contiguous() if isinstance(a, torch.Tensor) else a for a in args]
-                    attr(*args)
-                    outs = {i: args[i].detach().clone().contiguous() for i in HVP_OUT_ARGS[name]}
-                    self.calls.append((name, snap, outs))
-                return wrapped
-            return attr
+        recorded = {**OUT_ARGS, **HVP_OUT_ARGS}
 
     return HvpRecordingKernels()
 

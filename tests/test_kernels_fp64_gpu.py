@@ -4,8 +4,13 @@ dispatch and checked against an fp64 evaluation of its specification (tests/repl
 The mixed batch puts two rattled LiMnO2 supercells (144 and 480 atoms, 84-88 neighbours per atom) between random cells
 and a cell without edges, so that the persistent kernels run several tiles per CTA, segments span several 16-row
 strips and the virial reduction sees blocks inside one graph and across graphs; ``test_mixed_batch_covers_the_edges``
-asserts these properties of the batch itself.  The inference recording and its fp64 references are cached for the
-module (five implementation slots replay it); the other runs are checked call by call as they are recorded."""
+asserts these properties of the batch itself.  The high-coordination batch of tests/dense_cells.py (rattled diamond
+and a 1.1 A simple cubic H/Li cell: segments of 704 edges, 163 bond-graph rows and 6 806 angles per atom, longer than
+a tile and than a persistent CTA's share) runs through the same tests: the inference recording is parametrized over
+both batches, and the coverage, training and determinism tests check one batch after the other.  The inference
+recording and its fp64 references are cached per batch (five implementation slots replay it); the other runs are
+checked call by call as they are recorded."""
+import dense_cells
 import numpy as np
 import pytest
 import torch
@@ -19,6 +24,7 @@ pytestmark = pytest.mark.gpu
 
 N_SM = 132  # H100 SXM
 WS_TILE, FFMA_TILE, STRIP, VIRIAL_BLOCK = 128, 64, 16, 256  # csrc/gated_ws.cu, gated.cu, geometry.cu
+WS_MIN_ROWS = 4096  # default ws_min_rows: the fused warp-specialised kernels run from this many rows
 
 
 def _mixed_graphs(**cut):
@@ -74,16 +80,48 @@ def mixed_graphs():
 
 
 @pytest.fixture(scope="module")
-def inference(weights030, mixed_graphs):
+def dense_graphs():
+    return dense_cells.dense_graphs()
+
+
+def _inference_calls(weights, graphs, calls=None):
+    """The kernel calls of an inference run (forces, stress, magmoms, features) on ``graphs``."""
     from kernel_replay import RecordingKernels
 
     rec = RecordingKernels()
-    Engine(_packed(weights030), rec).run(build_batch(mixed_graphs, "cpu"), need_grad=True, need_magmom=True,
-                                         need_atom_fea=True, need_crystal_fea=True)
-    return _with_refs(rec.calls)
+    if calls is not None:
+        rec.calls = calls
+    Engine(_packed(weights), rec).run(build_batch(graphs, "cpu"), need_grad=True, need_magmom=True,
+                                      need_atom_fea=True, need_crystal_fea=True)
+    return rec.calls
 
 
-def test_mixed_batch_covers_the_edges(mixed_graphs):
+@pytest.fixture(scope="module", params=["mixed", "dense"])
+def inference(request, weights030):
+    return _with_refs(_inference_calls(weights030, request.getfixturevalue(f"{request.param}_graphs")))
+
+
+def _longest(ptr):
+    ptr = ptr.long()
+    return int((ptr[1:] - ptr[:-1]).max())
+
+
+def test_mixed_batch_covers_the_edges(mixed_graphs, dense_graphs):
+    """Both batches: ragged last tiles; the mixed batch several tiles per persistent CTA, segments across strips and
+    virial blocks inside and across graphs; the dense batch segments longer than a tile."""
+    b = build_batch(dense_graphs, "cpu")
+    ed, a = b.n_edges, b.n_angles
+    assert ed % WS_TILE and a % WS_TILE, (ed, a)
+    assert ed >= WS_MIN_ROWS and a >= WS_MIN_ROWS, (ed, a)  # the default dispatch runs the gated_ws kernels
+    assert _longest(b.ptr_c) > 2 * WS_TILE, "an AtomConv segment longer than 256 rows"
+    assert _longest(b.ptr_is) > WS_TILE, "a BondConv segment longer than a tile"
+    lo, hi = b.ptr_is.long()[:-1], b.ptr_is.long()[1:]
+    assert int(((hi - 1) // STRIP - lo // STRIP + 1)[hi > lo].max()) >= 3, "a BondConv segment spanning 3 strips"
+    assert _longest(b.ptr_x) > 4096, "angles of one atom: more than 4096 items"
+    assert bool((b.ptr_c.long()[1:] == b.ptr_c.long()[:-1]).any()), "an atom without edges"
+    print(f"dense batch: {b.n_atoms} atoms, {ed} edges, {a} angles; longest ptr_c {_longest(b.ptr_c)}, "
+          f"ptr_is {_longest(b.ptr_is)}, ptr_x {_longest(b.ptr_x)}")
+
     b = build_batch(mixed_graphs, "cpu")
     ed, a = b.n_edges, b.n_angles
     assert ed % WS_TILE and a % WS_TILE, (ed, a)
@@ -115,23 +153,25 @@ def test_inference_at_size_matches_fp64(inference, linear_impl, gated_impl):
     assert chk.kernels == INFER_KERNELS, sorted(chk.kernels)
 
 
-def test_training_step_at_size_matches_fp64(weights030, mixed_graphs):
-    """Energy / magmom step, then a step with force and stress seeds: every training and second-order kernel."""
+def test_training_step_at_size_matches_fp64(weights030, mixed_graphs, dense_graphs):
+    """Energy / magmom step, then a step with force and stress seeds: every training and second-order kernel, on the
+    mixed and on the dense batch."""
     from kernel_replay import TRAIN_KERNELS, RecordingKernels
 
-    rec = RecordingKernels()
-    chk = _streamed(rec)
-    eng = Engine(_packed(weights030), rec)
-    n, nb = sum(g.atomic_number.shape[0] for g in mixed_graphs), len(mixed_graphs)
-    gen = torch.Generator().manual_seed(12)
-    out = eng.run(build_batch(mixed_graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
-    eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen))
-    out = eng.run(build_batch(mixed_graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
-    eng.input_grads(out, record=True)
-    eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen),
-                    torch.randn(n, 3, generator=gen), torch.randn(nb, 3, 3, generator=gen))
-    chk.assert_ok("training step")
-    assert TRAIN_KERNELS <= chk.kernels, sorted(TRAIN_KERNELS - chk.kernels)
+    for title, graphs in (("mixed", mixed_graphs), ("dense", dense_graphs)):
+        rec = RecordingKernels()
+        chk = _streamed(rec)
+        eng = Engine(_packed(weights030), rec)
+        n, nb = sum(g.atomic_number.shape[0] for g in graphs), len(graphs)
+        gen = torch.Generator().manual_seed(12)
+        out = eng.run(build_batch(graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
+        eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen))
+        out = eng.run(build_batch(graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
+        eng.input_grads(out, record=True)
+        eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen),
+                        torch.randn(n, 3, generator=gen), torch.randn(nb, 3, 3, generator=gen))
+        chk.assert_ok(f"training step, {title} batch")
+        assert TRAIN_KERNELS <= chk.kernels, (title, sorted(TRAIN_KERNELS - chk.kernels))
 
 
 def test_without_layernorm_at_size_matches_fp64(weights030):
@@ -162,16 +202,7 @@ def _second_order_recorder():
     from oracle.elastic import ElasticSpecKernels
 
     class Recorder(RecordingKernels, ElasticSpecKernels):
-        def __getattribute__(self, name):
-            attr = super().__getattribute__(name)
-            if name in replay_fp64.SECOND_DERIV_OUT_ARGS:
-                def wrapped(*args):
-                    snap = [a.detach().clone().contiguous() if isinstance(a, torch.Tensor) else a for a in args]
-                    attr(*args)
-                    outs = {i: args[i].detach().clone().contiguous() for i in replay_fp64.SECOND_DERIV_OUT_ARGS[name]}
-                    self.calls.append((name, snap, outs))
-                return wrapped
-            return attr
+        recorded = replay_fp64.ALL_OUT_ARGS
 
     return Recorder()
 
@@ -202,9 +233,10 @@ def test_second_derivatives_at_size_match_fp64(weights030, kind):
     assert want <= chk.kernels, sorted(chk.kernels)
 
 
-def test_fused_and_wgrad_are_deterministic_at_size(inference, weights030, mixed_graphs):
+def test_fused_and_wgrad_are_deterministic_at_size(weights030, mixed_graphs, dense_graphs):
     """The header's "fixed order: deterministic": the fused message + aggregation kernels under the default dispatch,
-    and chg_wgrad under both implementations, give bitwise equal results on a second call."""
+    and chg_wgrad under both implementations, give bitwise equal results on a second call, on both batches."""
+    import replay_fp64
     from kernel_replay import RecordingKernels
 
     from chgnet_b200._lib import CudaKernels
@@ -212,19 +244,18 @@ def test_fused_and_wgrad_are_deterministic_at_size(inference, weights030, mixed_
     def twice(K, name, snap, outs):
         res = []
         for _ in range(2):
-            args = [a.cuda() if isinstance(a, torch.Tensor) else a for a in snap]
+            args = replay_fp64.place(snap)[0]
             getattr(K, name)(*args)
             torch.cuda.synchronize()
             res.append([args[i] for i in outs])
         for i, x, y in zip(outs, *res):
             assert torch.equal(x, y), f"{name} out[{i}] differs between two identical calls"
 
-    K = CudaKernels()
-    calls, _ = inference
-    fused = [c for c in calls if c[0] in ("atom_conv_fused", "bond_conv_fused")]
-    assert {c[0] for c in fused} == {"atom_conv_fused", "bond_conv_fused"}
-    for name, snap, outs in fused:
-        twice(K, name, snap, outs)
+    class Fused(list):  # keeps only the fused message + aggregation calls
+        def append(self, call):
+            if call[0] in ("atom_conv_fused", "bond_conv_fused"):
+                super().append(call)
+
     def rows(snap):  # m of chg_wgrad: x_rows, else g_rows, else the rows of x
         return next(t.shape[0] for t in (snap[4], snap[5], snap[0]) if t is not None)
 
@@ -233,19 +264,26 @@ def test_fused_and_wgrad_are_deterministic_at_size(inference, weights030, mixed_
             if call[0] == "wgrad" and rows(call[1]) >= 4096:
                 super().append(call)
 
-    rec = RecordingKernels()
-    rec.calls = LargeWgrad()
-    eng = Engine(_packed(weights030), rec)
-    n, nb = sum(g.atomic_number.shape[0] for g in mixed_graphs), len(mixed_graphs)
-    gen = torch.Generator().manual_seed(14)
-    out = eng.run(build_batch(mixed_graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
-    eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen))
-    wgrad = list(rec.calls)
-    assert wgrad
-    try:
-        for impl in (1, 0):
-            K.set_option("wgrad_impl", impl)
-            for name, snap, outs in wgrad:
-                twice(K, name, snap, outs)
-    finally:
-        K.set_option("wgrad_impl", 1)
+    K = CudaKernels()
+    for graphs in (mixed_graphs, dense_graphs):
+        fused = _inference_calls(weights030, graphs, Fused())
+        assert {c[0] for c in fused} == {"atom_conv_fused", "bond_conv_fused"}
+        for name, snap, outs in fused:
+            twice(K, name, snap, outs)
+        del fused
+        rec = RecordingKernels()
+        rec.calls = LargeWgrad()
+        eng = Engine(_packed(weights030), rec)
+        n, nb = sum(g.atomic_number.shape[0] for g in graphs), len(graphs)
+        gen = torch.Generator().manual_seed(14)
+        out = eng.run(build_batch(graphs, "cpu"), need_grad=True, need_magmom=True, train=True)
+        eng.param_grads(out, torch.randn(nb, generator=gen), torch.randn(n, generator=gen))
+        wgrad = list(rec.calls)
+        assert wgrad
+        try:
+            for impl in (1, 0):
+                K.set_option("wgrad_impl", impl)
+                for name, snap, outs in wgrad:
+                    twice(K, name, snap, outs)
+        finally:
+            K.set_option("wgrad_impl", 1)

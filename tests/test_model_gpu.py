@@ -96,6 +96,19 @@ def test_against_fp64_oracle_on_larger_batch(model, weights030):
     print("max |cuda - oracle64|:", {k: f"{v:.2e}" for k, v in worst.items()})
     for k, tol in TOL.items():
         assert worst[k] < tol, (k, worst[k])
+    # rattled diamond, 158 edges per atom (segments longer than a tile): the native forward of predict_graph and the
+    # device graph builder of predict_structure
+    import dense_cells
+
+    z, frac, lat = dense_cells.diamond()
+    g = graphgen.make_crystal_graph(z, frac, lat, graph_id="diamond")
+    want = orc.predict_graph(weights030, [g], "efsm", dtype=torch.float64)[0]
+    for path, got in (("predict_graph", model.predict_graph(g, task="efsm")),
+                      ("predict_structure", model.predict_structure((z, frac, lat), task="efsm"))):
+        err = {k: _maxabs(got[k], want[k]) for k in TOL}
+        print(f"diamond {path}: max |cuda - oracle64|:", {k: f"{v:.2e}" for k, v in err.items()})
+        for k, tol in TOL.items():
+            assert err[k] < tol, (path, k, err[k])
 
 
 def test_rotation_and_supercell_invariance(model):
@@ -265,3 +278,19 @@ def test_static_evaluator_replays_one_cuda_graph():
     one = model.static_evaluator(graphs[0], task="ef")
     r = [one() for _ in range(3)]
     assert set(r[0]) == {"e", "f"} and np.allclose(r[0]["f"], r[2]["f"]) and np.allclose(r[0]["f"], base[0]["f"], atol=1e-6)
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two CUDA devices")
+def test_same_answer_on_a_second_device_in_one_process():
+    """The large-shared-memory kernels set their launch attributes per device: a model moved to cuda:1 after cuda:0
+    has run (the warp-specialised message kernels included, above 4096 edges and angles) gives the same numbers."""
+    import dense_cells
+
+    from chgnet_b200.model import CHGNet
+
+    gold = os.path.join(os.path.dirname(__file__), "golden", "chgnet_0.3.0_weights.npz")
+    g = graphgen.make_crystal_graph(*dense_cells.diamond())
+    assert g.atom_graph.shape[0] >= 4096 and g.bond_graph.shape[0] >= 4096
+    out = [CHGNet.from_file(gold, version="0.3.0").to(dev).predict_graph(g, task="efsm") for dev in ("cuda:0", "cuda:1")]
+    for k in "efsm":
+        assert np.array_equal(np.asarray(out[0][k]), np.asarray(out[1][k])), k

@@ -139,14 +139,18 @@ def test_c5_slice_parameter_gradients_efsm(model, weights030):
 def test_device_csr_build_is_bit_identical_to_the_torch_build():
     """chg_build_csr (counting sorts + boundary searches, csrc/batch_csr.cu) against the torch sorts it replaces:
     every int32 field of the batch descriptor, exactly - random cells, a batch with isolated atoms and an empty
-    bond graph, the c2 batch, with and without the reverse structures, with and without bond compaction."""
+    bond graph, the c2 batch, the high-coordination batch, with and without the reverse structures, with and without
+    bond compaction."""
+    import dense_cells
+
     from chgnet_b200.batch import build_batch
 
     g_far = graphgen.make_crystal_graph([3, 8], np.array([[0.0, 0, 0], [0.5, 0.5, 0.5]]), np.eye(3) * 5.5)
     g_iso = graphgen.make_crystal_graph([1, 1], np.array([[0.0, 0, 0], [0.5, 0.5, 0.5]]), np.eye(3) * 20.0)
     z, frac, lat = graphgen.limno2_structure((4, 3, 3), 0.02, 4001)
     cases = [graphgen.random_graphs(5, 8, 30, 9100), [g_iso], [g_far], [g_iso, g_far] + graphgen.random_graphs(2, 9, 12, 9200),
-             graphgen.random_graphs(64, 40, 60, 1000), [graphgen.make_crystal_graph(z, frac, lat)]]
+             graphgen.random_graphs(64, 40, 60, 1000), [graphgen.make_crystal_graph(z, frac, lat)],
+             dense_cells.dense_graphs()]  # segments of thousands of items (segment_sort_kernel)
     fields = ("z", "owner", "center", "nbr", "d2u", "u2d", "ptr_c", "perm_n", "ptr_n", "perm_u", "ptr_u", "ang_atom", "ang_i",
               "ang_j", "ang_di", "ang_dj", "ptr_i", "perm_j", "ptr_j", "perm_x", "ptr_x", "short_ids", "ang_is", "ang_js",
               "ptr_is", "perm_js", "ptr_js")
