@@ -74,11 +74,10 @@ SIGNATURES: dict[str, list] = {
     "chg_joint_dos": [P, I, I, I, I, P, P, I, P, I, P, I, D, P, P, P],
 }
 
-# CHG_DOS_MAX_CHUNKS of include/chgnet_b200.h: chg_tetrahedron_dos needs this many (2 + n_proj) x n_freq scratch rows
+# CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
+# chg_thermal_displacements and chg_joint_dos may fill (tests/test_abi_symbols.py ties the copies to the header)
 DOS_MAX_CHUNKS = 512
-# CHG_TD_MAX_CHUNKS: chg_thermal_displacements needs this many n_t x n_prim x 6 scratch blocks
 TD_MAX_CHUNKS = 128
-# CHG_JDOS_MAX_CHUNKS: chg_joint_dos needs this many n_target x (1 + n_t) x 2 x n_freq scratch blocks
 JDOS_MAX_CHUNKS = 64
 
 _lib = None
@@ -86,6 +85,23 @@ _lib = None
 
 class ChgnetB200Error(RuntimeError):
     pass
+
+
+def _mesh_args(name, mesh, freqs, tetrahedra, f64_names, f64_tensors):
+    """(n1, n2, n3) of ``mesh``, checking f64_tensors (None skipped), tetrahedra [6, 4, 3] int32 and freqs."""
+    n1, n2, n3 = (int(n) for n in mesh)
+    if any(t is not None and t.dtype != torch.float64 for t in f64_tensors):
+        raise ChgnetB200Error(f"{name}: {f64_names} must be float64")
+    if tetrahedra.dtype != torch.int32 or tuple(tetrahedra.shape) != (6, 4, 3):
+        raise ChgnetB200Error(f"{name}: tetrahedra must be int32 [6, 4, 3]")
+    if freqs.shape[0] != n1 * n2 * n3:
+        raise ChgnetB200Error(f"{name}: freqs must be [{n1 * n2 * n3}, n_band]")
+    return n1, n2, n3
+
+
+def _chunk_scratch(max_chunks, per_chunk, device):
+    """fp64 scratch for at most ``max_chunks`` chunks of ``per_chunk`` partial sums."""
+    return torch.empty(max_chunks * max(per_chunk, 1), dtype=torch.float64, device=device)
 
 
 def load_library(path: str | None = None) -> ctypes.CDLL:
@@ -398,22 +414,18 @@ class CudaKernels:
         (ascending per q), tetrahedra [6, 4, 3] int32 corner offsets, omega [F] fp64; writes dos [F], idos [F] and,
         with proj [n1 n2 n3, n_band, S], pdos [S, F] (all fp64)."""
         self._chk(freqs, tetrahedra, omega, dos, idos, proj, pdos)
-        n1, n2, n3 = (int(n) for n in mesh)
+        n1, n2, n3 = _mesh_args("tetrahedron_dos", mesh, freqs, tetrahedra, "freqs, omega, proj and the outputs",
+                                (freqs, omega, dos, idos, proj, pdos))
         n_q, n_band = freqs.shape
-        f64 = torch.float64
-        if any(t is not None and t.dtype != f64 for t in (freqs, omega, dos, idos, proj, pdos)):
-            raise ChgnetB200Error("tetrahedron_dos: freqs, omega, proj and the outputs must be float64")
-        if tetrahedra.dtype != torch.int32 or tuple(tetrahedra.shape) != (6, 4, 3):
-            raise ChgnetB200Error("tetrahedron_dos: tetrahedra must be int32 [6, 4, 3]")
         n_f = omega.shape[0]
-        if n_q != n1 * n2 * n3 or tuple(dos.shape) != (n_f,) or tuple(idos.shape) != (n_f,):
-            raise ChgnetB200Error(f"tetrahedron_dos: freqs must be [{n1 * n2 * n3}, n_band], dos and idos [{n_f}]")
+        if tuple(dos.shape) != (n_f,) or tuple(idos.shape) != (n_f,):
+            raise ChgnetB200Error(f"tetrahedron_dos: dos and idos must be [{n_f}]")
         n_proj = 0
         if proj is not None:
             n_proj = proj.shape[2]
             if tuple(proj.shape[:2]) != (n_q, n_band) or pdos is None or tuple(pdos.shape) != (n_proj, n_f):
                 raise ChgnetB200Error(f"tetrahedron_dos: proj must be [{n_q}, {n_band}, S] and pdos [S, {n_f}]")
-        work = torch.empty(DOS_MAX_CHUNKS * (2 + n_proj) * max(n_f, 1), dtype=f64, device=freqs.device)
+        work = _chunk_scratch(DOS_MAX_CHUNKS, (2 + n_proj) * n_f, freqs.device)
         self._call("chg_tetrahedron_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(proj), n_proj, _p(omega),
                    n_f, _p(dos), _p(idos), _p(pdos if proj is not None else None), _p(work))
 
@@ -434,7 +446,7 @@ class CudaKernels:
                 or tuple(acc.shape) != (n_t, n3 // 3, 6)):
             raise ChgnetB200Error(f"thermal_displacements: freqs must be [Q, 3n], eigvecs [{n_q}, {n3}, {n3}], "
                                   f"temperatures [T] and acc [T, {n3 // 3}, 6]")
-        work = torch.empty(TD_MAX_CHUNKS * max(n_t * (n3 // 3) * 6, 1), dtype=f64, device=freqs.device)
+        work = _chunk_scratch(TD_MAX_CHUNKS, n_t * (n3 // 3) * 6, freqs.device)
         self._call("chg_thermal_displacements", _p(freqs), _p(eigvecs), n_q, n3 // 3, _p(temperatures), n_t,
                    float(cutoff_thz), _p(work), _p(acc))
 
@@ -444,25 +456,21 @@ class CudaKernels:
         fp64 THz (the frequency points of each target), temperatures [T] fp64 K or None; writes out [Q, 1 + T, 2, F]
         fp64 (slot 0: D2 classes 1 and 2; slot 1 + t: N2 at temperatures[t]), modes below cutoff_thz left out."""
         self._chk(freqs, tetrahedra, targets, omega, temperatures, out)
-        n1, n2, n3 = (int(n) for n in mesh)
-        f64 = torch.float64
-        if any(t is not None and t.dtype != f64 for t in (freqs, omega, temperatures, out)):
-            raise ChgnetB200Error("joint_dos: freqs, omega, temperatures and out must be float64")
-        if tetrahedra.dtype != torch.int32 or tuple(tetrahedra.shape) != (6, 4, 3):
-            raise ChgnetB200Error("joint_dos: tetrahedra must be int32 [6, 4, 3]")
+        n1, n2, n3 = _mesh_args("joint_dos", mesh, freqs, tetrahedra, "freqs, omega, temperatures and out",
+                                (freqs, omega, temperatures, out))
         if targets.dtype != torch.int32 or targets.dim() != 1:
             raise ChgnetB200Error("joint_dos: targets must be int32 [Q]")
-        n_q, n_band = freqs.shape
+        n_band = freqs.shape[1]
         n_target = targets.shape[0]
         n_t = 0 if temperatures is None else temperatures.shape[0]
         if temperatures is not None and temperatures.dim() != 1:
             raise ChgnetB200Error("joint_dos: temperatures must be [T]")
-        if n_q != n1 * n2 * n3 or omega.dim() != 2 or omega.shape[0] != n_target:
-            raise ChgnetB200Error(f"joint_dos: freqs must be [{n1 * n2 * n3}, n_band] and omega [{n_target}, F]")
+        if omega.dim() != 2 or omega.shape[0] != n_target:
+            raise ChgnetB200Error(f"joint_dos: omega must be [{n_target}, F]")
         n_f = omega.shape[1]
         if tuple(out.shape) != (n_target, 1 + n_t, 2, n_f):
             raise ChgnetB200Error(f"joint_dos: out must be [{n_target}, {1 + n_t}, 2, {n_f}]")
-        work = torch.empty(JDOS_MAX_CHUNKS * max(n_target * (1 + n_t) * 2 * n_f, 1), dtype=f64, device=freqs.device)
+        work = _chunk_scratch(JDOS_MAX_CHUNKS, n_target * (1 + n_t) * 2 * n_f, freqs.device)
         self._call("chg_joint_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(targets), n_target, _p(omega),
                    n_f, _p(temperatures), n_t, float(cutoff_thz), _p(out), _p(work))
 

@@ -177,10 +177,42 @@ __device__ __forceinline__ bool tetra_weights(double w, const double (&e)[4], do
   return true;
 }
 
+// corner(v, a, b, c) for the four corners v of tetrahedron tt % 6 of mesh cell tt / 6, (a, b, c) wrapped onto the mesh
+template <class Corner>
+__device__ __forceinline__ void tetrahedron_corners(const int32_t* __restrict__ tet, int64_t tt, int n1, int n2, int n3,
+                                                    Corner corner) {
+  const int it = (int)(tt % 6);
+  const int64_t cell = tt / 6;
+  const int ci = (int)(cell / ((int64_t)n2 * n3)), cj = (int)((cell / n3) % n2), ck = (int)(cell % n3);
+#pragma unroll
+  for (int v = 0; v < 4; ++v) {
+    const int32_t* o = tet + (it * 4 + v) * 3;
+    int a = ci + __ldg(o), b = cj + __ldg(o + 1), c = ck + __ldg(o + 2);
+    a -= a >= n1 ? n1 : 0;
+    b -= b >= n2 ? n2 : 0;
+    c -= c >= n3 ? n3 : 0;
+    corner(v, a, b, c);
+  }
+}
+
+// Sorting network: the corner values ascending, each carrying its payload (ties keep a fixed, data-determined order)
+template <class T>
+__device__ __forceinline__ void sort4(double (&e)[4], T (&x)[4]) {
+  const auto cswap = [&](int i, int j) {
+    if (e[j] < e[i]) {
+      const double te = e[i];
+      e[i] = e[j], e[j] = te;
+      const T tx = x[i];
+      x[i] = x[j], x[j] = tx;
+    }
+  };
+  cswap(0, 1), cswap(2, 3), cswap(0, 2), cswap(1, 3), cswap(1, 2);
+}
+
 // One thread per frequency point; block x owns a contiguous range of (tetrahedron, band) pairs, z a group of
 // DOS_PROJ projection columns.  Each tile of pairs is staged, sorted, in shared memory by the block and then read
 // by every thread (broadcasts).  The block's sums go to work[chunk][row][F] (row 0 g, 1 n, 2 + s the projection s),
-// each element written by exactly one thread: no atomics, and dos_reduce_kernel adds the chunks in a fixed order.
+// each element written by exactly one thread: no atomics, and chunk_reduce_kernel adds the chunks in a fixed order.
 __global__ void __launch_bounds__(DOS_MAX_THREADS)
 tetrahedron_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
                        const int32_t* __restrict__ tet, const double* __restrict__ proj, int n_proj,
@@ -204,32 +236,13 @@ tetrahedron_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int
     __syncthreads();  // the previous tile has been read
     if (p < n_pairs) {
       const int band = (int)(p % n_band);
-      const int64_t tt = p / n_band;
-      const int it = (int)(tt % 6);
-      const int64_t cell = tt / 6;
-      const int ci = (int)(cell / ((int64_t)n2 * n3)), cj = (int)((cell / n3) % n2), ck = (int)(cell % n3);
       double e[4];
       int32_t q[4];
-#pragma unroll
-      for (int v = 0; v < 4; ++v) {
-        const int32_t* o = tet + (it * 4 + v) * 3;
-        int a = ci + __ldg(o), b = cj + __ldg(o + 1), c = ck + __ldg(o + 2);
-        a -= a >= n1 ? n1 : 0;
-        b -= b >= n2 ? n2 : 0;
-        c -= c >= n3 ? n3 : 0;
+      tetrahedron_corners(tet, p / n_band, n1, n2, n3, [&](int v, int a, int b, int c) {
         q[v] = (a * n2 + b) * n3 + c;
         e[v] = __ldg(freqs + (int64_t)q[v] * n_band + band);
-      }
-      // sorting network, ascending (ties keep a fixed, data-determined order)
-#define CHG_CSWAP(i, j)                      \
-  if (e[j] < e[i]) {                         \
-    const double te = e[i];                  \
-    e[i] = e[j], e[j] = te;                  \
-    const int32_t tq = q[i];                 \
-    q[i] = q[j], q[j] = tq;                  \
-  }
-      CHG_CSWAP(0, 1) CHG_CSWAP(2, 3) CHG_CSWAP(0, 2) CHG_CSWAP(1, 3) CHG_CSWAP(1, 2)
-#undef CHG_CSWAP
+      });
+      sort4(e, q);
 #pragma unroll
       for (int v = 0; v < 4; ++v) se[threadIdx.x][v] = e[v], sq[threadIdx.x][v] = q[v];
       sb[threadIdx.x] = band;
@@ -266,17 +279,16 @@ tetrahedron_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int
     if (s < ns) out[(size_t)(2 + s0 + s) * n_freq] = acc_p[s];
 }
 
-// out[row][f] = scale * sum over chunks (in chunk order) of work[chunk][row][f]
-__global__ void dos_reduce_kernel(const double* __restrict__ work, int n_chunks, int rows, int n_freq, double scale,
-                                  double* __restrict__ dos, double* __restrict__ idos, double* __restrict__ pdos) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)rows * n_freq) return;
-  const int r = (int)(idx / n_freq), f = (int)(idx % n_freq);
-  double acc = 0.0;
-  for (int c = 0; c < n_chunks; ++c) acc += work[((size_t)c * rows + r) * n_freq + f];
-  double* out = r == 0 ? dos : (r == 1 ? idos : pdos + (size_t)(r - 2) * n_freq);
-  out[f] = acc * scale;
-}
+struct DosStore {  // work[chunk][row][f]: scale * the sum, row 0 to dos, 1 to idos, 2 + s to pdos[s]
+  double *dos, *idos, *pdos;
+  int n_freq;
+  double scale;
+  __device__ void operator()(int64_t o, double s) const {
+    const int r = (int)(o / n_freq), f = (int)(o % n_freq);
+    double* out = r == 0 ? dos : (r == 1 ? idos : pdos + (size_t)(r - 2) * n_freq);
+    out[f] = s * scale;
+  }
+};
 
 // ---------------------------------------------------------------------------------------------------------------
 // Thermal displacements.  acc[t][k][c] += sum over (q, mode) of w(nu, T_t) Re(e e^H)_c, e the 3-component block of
@@ -286,7 +298,7 @@ __global__ void dos_reduce_kernel(const double* __restrict__ work, int n_chunks,
 // takes the q-points q_begin + qi, q_begin + qi + n_qi, ... of its block's range at temperature t0 + ti, reads the
 // eigenvector blocks of the group's atoms (the same addresses for every ti of one q) and keeps 6 TD_ATOMS sums in
 // registers.  The block adds them over qi in a fixed order in shared memory and writes work[chunk][t][k][6];
-// td_reduce_kernel adds the chunks in chunk order to acc.  No atomics, and neither the (q, mode) products nor the
+// chunk_reduce_kernel adds the chunks in chunk order to acc.  No atomics, and neither the (q, mode) products nor the
 // weights ever reach global memory.
 constexpr int TD_THREADS = 256;  // (q, temperature) slots per block
 constexpr int TD_ATOMS = 4;      // atoms per block (grid y)
@@ -351,15 +363,10 @@ thermal_displacements_kernel(const double* __restrict__ freqs, const double2* __
   }
 }
 
-// acc[o] += sum over chunks (in chunk order) of work[chunk][o]
-__global__ void td_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out,
-                                 double* __restrict__ acc) {
-  const int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= n_out) return;
-  double s = 0.0;
-  for (int c = 0; c < n_chunks; ++c) s += work[(size_t)c * n_out + o];
-  acc[o] += s;
-}
+struct AccumulateStore {  // work[chunk][t][k][6]: acc += the sum
+  double* acc;
+  __device__ void operator()(int64_t o, double s) const { acc[o] += s; }
+};
 
 // ---------------------------------------------------------------------------------------------------------------
 // Joint densities of states.  For a target q and an item (cell, tetrahedron, l1, l2) the corners are q1_i of the
@@ -369,7 +376,7 @@ __global__ void td_reduce_kernel(const double* __restrict__ work, int n_chunks, 
 //   class 2: f_i = nu1_i + nu2_i,                                   c_i = m_i           or m_i (n1_i + n2_i + 1)
 // m_i = [nu1_i >= cutoff and nu2_i >= cutoff], n = 1 / expm1(h nu / k T) (0 at T = 0).  The other class-1 term,
 // delta(w - nu1 + nu2), is the same sum mapped by q1 -> q - q1, l1 <-> l2 (the 6-tetrahedron set is inversion
-// symmetric): jdos_reduce_kernel doubles class 1, which also gives N2(1)'s difference.  The contribution at w is
+// symmetric): the reduction doubles class 1, which also gives N2(1)'s difference.  The contribution at w is
 // sum_i wt_i(w) c_i with tetra_weights' corner weights, each tetrahedron weighted 1 / (6 N).
 //
 // Block (x, y): JDOS_THREADS threads as blockDim.y target slots of blockDim.x (a multiple of 32) frequency points.
@@ -377,25 +384,12 @@ __global__ void td_reduce_kernel(const double* __restrict__ work, int n_chunks, 
 // z: the slot (0: D2, 1 + t: N2 at temperatures[t]).  Each warp of a target slot stages one sorted tile of
 // blockDim.x items of its own target in shared memory (values and corner factors of both classes), then every
 // thread of that slot evaluates the tile at its own frequency point (shared-memory broadcasts).  The block writes
-// work[chunk][target][slot][class][f], each element by exactly one thread; jdos_reduce_kernel adds the chunks in a
+// work[chunk][target][slot][class][f], each element by exactly one thread; chunk_reduce_kernel adds the chunks in a
 // fixed order.  No atomics, and no per-item value leaves the SM.
 constexpr int JDOS_THREADS = 256;
 
 __device__ __forceinline__ double bose(double nu, double temp) {
   return temp > 0.0 ? 1.0 / expm1(TD_H_OVER_K * nu / temp) : 0.0;
-}
-
-// sort the corner values ascending, carrying their factors (ties keep a fixed, data-determined order)
-__device__ __forceinline__ void sort4(double (&e)[4], double (&c)[4]) {
-#define CHG_CSWAP(i, j)        \
-  if (e[j] < e[i]) {           \
-    const double te = e[i];    \
-    e[i] = e[j], e[j] = te;    \
-    const double tc = c[i];    \
-    c[i] = c[j], c[j] = tc;    \
-  }
-  CHG_CSWAP(0, 1) CHG_CSWAP(2, 3) CHG_CSWAP(0, 2) CHG_CSWAP(1, 3) CHG_CSWAP(1, 2)
-#undef CHG_CSWAP
 }
 
 __global__ void __launch_bounds__(JDOS_THREADS)
@@ -429,19 +423,9 @@ joint_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, i
       const int l2 = (int)(p % n_band);
       const int64_t r = p / n_band;
       const int l1 = (int)(r % n_band);
-      const int64_t tt = r / n_band;
-      const int it = (int)(tt % 6);
-      const int64_t cell = tt / 6;
-      const int ci = (int)(cell / ((int64_t)n2 * n3)), cj = (int)((cell / n3) % n2), ck = (int)(cell % n3);
       double e1[4], c1[4], e2[4], c2[4];
       bool any = false;
-#pragma unroll
-      for (int v = 0; v < 4; ++v) {
-        const int32_t* o = tet + (it * 4 + v) * 3;
-        int a = ci + __ldg(o), b = cj + __ldg(o + 1), c = ck + __ldg(o + 2);
-        a -= a >= n1 ? n1 : 0;
-        b -= b >= n2 ? n2 : 0;
-        c -= c >= n3 ? n3 : 0;
+      tetrahedron_corners(tet, r / n_band, n1, n2, n3, [&](int v, int a, int b, int c) {
         int a2 = qa - a, b2 = qb - b, c2i = qc - c;
         a2 += a2 < 0 ? n1 : 0;
         b2 += b2 < 0 ? n2 : 0;
@@ -461,7 +445,7 @@ joint_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, i
           c1[v] = b1 - b2v;
           c2[v] = b1 + b2v + 1.0;
         }
-      }
+      });
       sort4(e1, c1);
       sort4(e2, c2);
       if (!any) e1[0] = e2[0] = CUDART_INF;  // every corner masked: no frequency point is evaluated
@@ -498,15 +482,32 @@ joint_dos_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, i
   out[n_freq] = acc2;
 }
 
-// out[o] = scale_class * sum over chunks (in chunk order) of work[chunk][o], o = ((target, slot), class, f); class 1
-// carries both of its terms (x 2)
-__global__ void jdos_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out, int n_freq,
-                                   double scale, double* __restrict__ out) {
+struct JointDosStore {  // work[chunk][target][slot][class][f]: scale * the sum, x 2 for class 1 (both its terms)
+  double* out;
+  int n_freq;
+  double scale;
+  __device__ void operator()(int64_t o, double s) const { out[o] = s * ((o / n_freq) % 2 == 0 ? 2.0 * scale : scale); }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
+// The chunk reduction of the three kernels above: store(o, sum over chunks c, in chunk order, of work[c * n_out + o])
+template <class Store>
+__global__ void chunk_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out, Store store) {
   const int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= n_out) return;
   double s = 0.0;
   for (int c = 0; c < n_chunks; ++c) s += work[(size_t)c * n_out + o];
-  out[o] = s * ((o / n_freq) % 2 == 0 ? 2.0 * scale : scale);
+  store(o, s);
+}
+
+// Checks the launch of the kernel that filled work, then launches chunk_reduce_kernel after it on the same stream
+template <class Store>
+cudaError_t reduce_chunks(const double* work, int n_chunks, int64_t n_out, Store store, cudaStream_t stream) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  count_launch();
+  chunk_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, stream>>>(work, n_chunks, n_out, store);
+  return cudaSuccess;
 }
 
 }  // namespace
@@ -564,12 +565,9 @@ extern "C" int chg_tetrahedron_dos(const double* freqs, int32_t n_band, int32_t 
   const int rows = 2 + (proj ? n_proj : 0);
   tetrahedron_dos_kernel<<<dim3(chunks, (unsigned)f_blocks, groups), threads, 0, as_stream(stream)>>>(
       freqs, n_band, n1, n2, n3, tetrahedra, proj, n_proj, omega, n_freq, n_pairs, work);
-  CHG_CUDA(cudaGetLastError());
-  chg::count_launch();
-  const int64_t n_out = (int64_t)rows * n_freq;
   const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
-  dos_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, rows, n_freq, scale,
-                                                                                      dos, idos, pdos);
+  CHG_CUDA(reduce_chunks(work, chunks, (int64_t)rows * n_freq, DosStore{dos, idos, pdos, n_freq, scale},
+                         as_stream(stream)));
   CHG_LAUNCH_END();
 }
 
@@ -588,10 +586,7 @@ extern "C" int chg_thermal_displacements(const double* freqs, const double* eigv
   thermal_displacements_kernel<<<dim3(chunks, (unsigned)groups, (unsigned)t_tiles), n_qi * t_tile, 0,
                                  as_stream(stream)>>>(freqs, reinterpret_cast<const double2*>(eigvecs), n_q, n_prim,
                                                       temperatures, n_t, t_tile, cutoff_thz, work);
-  CHG_CUDA(cudaGetLastError());
-  chg::count_launch();
-  const int64_t n_out = (int64_t)n_t * n_prim * 6;
-  td_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, n_out, acc);
+  CHG_CUDA(reduce_chunks(work, chunks, (int64_t)n_t * n_prim * 6, AccumulateStore{acc}, as_stream(stream)));
   CHG_LAUNCH_END();
 }
 
@@ -618,11 +613,8 @@ extern "C" int chg_joint_dos(const double* freqs, int32_t n_band, int32_t n1, in
   joint_dos_kernel<<<dim3(chunks, (unsigned)groups, n_slots), dim3(threads, per_block), 0, as_stream(stream)>>>(
       freqs, n_band, n1, n2, n3, tetrahedra, targets, n_target, omega, n_freq, temperatures, cutoff_thz,
       n_items, work);
-  CHG_CUDA(cudaGetLastError());
-  chg::count_launch();
-  const int64_t n_out = (int64_t)n_target * n_slots * 2 * n_freq;
   const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
-  jdos_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, as_stream(stream)>>>(work, chunks, n_out, n_freq,
-                                                                                       scale, out);
+  CHG_CUDA(reduce_chunks(work, chunks, (int64_t)n_target * n_slots * 2 * n_freq, JointDosStore{out, n_freq, scale},
+                         as_stream(stream)));
   CHG_LAUNCH_END();
 }

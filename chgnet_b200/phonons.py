@@ -253,6 +253,24 @@ def cif_displacement_matrices(u_cart, prim_lattice) -> np.ndarray:
     return m @ np.asarray(u_cart, dtype=np.float64) @ m.T
 
 
+def _signed_thz(lam: torch.Tensor) -> torch.Tensor:
+    """Frequencies (THz) of the eigenvalues of D (eV/(A^2 amu)), imaginary modes negative."""
+    return torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+
+
+def _temperatures(temperatures) -> np.ndarray:
+    """``temperatures`` (K) as a 1-D fp64 array; ValueError unless every one is finite and >= 0."""
+    temps = np.asarray(temperatures, dtype=np.float64).reshape(-1)
+    if not np.all(np.isfinite(temps)) or np.any(temps < 0):
+        raise ValueError(f"temperatures must be finite and non-negative, got {temps.tolist()}")
+    return temps
+
+
+def _zero_gamma_acoustic(nu: torch.Tensor) -> None:
+    """Sets the three modes of smallest |nu| of row 0 (Gamma on a Gamma-centred mesh) to 0, in place."""
+    nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0
+
+
 class Phonons:
     """Harmonic phonons of a crystal from its compact supercell force constants (``CHGNet.phonons``).
 
@@ -304,6 +322,16 @@ class Phonons:
         self.kernels.dynamical_matrices(self._fc, self._img_ptr, self._img_vec, self._s2p, self._inv_sqrt_m, q, d)
         return d
 
+    def _eigh_chunks(self, q, *, eigenvectors: bool, matrices_per_q: int = 1, eigh_batch=math.inf):
+        """Yields ``(slice, nu, e or None)`` per chunk of ``q``: frequencies (THz) and eigenvectors of D on the device,
+        at most ``eigh_batch`` q keeping ``matrices_per_q`` complex128 [3n, 3n] per q below ``chunk_bytes``."""
+        n3 = 3 * len(self.p2s)
+        chunk = max(1, min(self.chunk_bytes // (matrices_per_q * 16 * n3 * n3), eigh_batch))
+        for s in range(0, len(q), chunk):
+            d = self.dynamical_matrices(q[s : s + chunk])
+            lam, e = torch.linalg.eigh(d) if eigenvectors else (torch.linalg.eigvalsh(d), None)
+            yield slice(s, s + chunk), _signed_thz(lam), e
+
     def frequencies(self, qpoints, *, eigenvectors: bool = False):
         """Frequencies ``[Q, 3 n_prim]`` in THz at the reduced ``qpoints`` (``[Q,3]`` or ``[3]``), ascending per q;
         an imaginary mode (negative eigenvalue of D) is given as a negative number, nu = sign(lambda) sqrt|lambda|
@@ -316,17 +344,12 @@ class Phonons:
         single = q.ndim == 1
         q = q.reshape(-1, 3)
         n3 = 3 * len(self.p2s)
-        chunk = max(1, self.chunk_bytes // (16 * n3 * n3))
         freqs = np.empty((len(q), n3))
         vecs = np.empty((len(q), n3, n3), dtype=np.complex128) if eigenvectors else None
-        for s in range(0, len(q), chunk):
-            d = self.dynamical_matrices(q[s : s + chunk])
+        for s, nu, e in self._eigh_chunks(q, eigenvectors=eigenvectors):
+            freqs[s] = nu.cpu().numpy()
             if eigenvectors:
-                w, v = torch.linalg.eigh(d)
-                vecs[s : s + chunk] = v.cpu().numpy()
-            else:
-                w = torch.linalg.eigvalsh(d)
-            freqs[s : s + chunk] = (torch.sign(w) * torch.sqrt(torch.abs(w)) * THZ_PER_SQRT_EV_A2_AMU).cpu().numpy()
+                vecs[s] = e.cpu().numpy()
         if single:
             freqs = freqs[0]
             vecs = None if vecs is None else vecs[0]
@@ -353,19 +376,15 @@ class Phonons:
         single = q.ndim == 1
         q = np.ascontiguousarray(q.reshape(-1, 3))
         n3 = 3 * len(self.p2s)
-        chunk = max(1, min(self.chunk_bytes // (4 * 16 * n3 * n3), self.eigh_batch))  # D and its three derivatives
         dev, c2 = self.device, THZ_PER_SQRT_EV_A2_AMU**2
         out = np.empty((len(q), n3, 3))
-        for s in range(0, len(q), chunk):
-            qd = torch.as_tensor(q[s : s + chunk]).to(dev)
+        # D and its three derivatives per q
+        for s, nu, e in self._eigh_chunks(q, eigenvectors=True, matrices_per_q=4, eigh_batch=self.eigh_batch):
+            qd = torch.as_tensor(q[s]).to(dev)
             nq = qd.shape[0]
-            d = torch.empty(nq, n3, n3, dtype=torch.complex128, device=dev)
-            self.kernels.dynamical_matrices(self._fc, self._img_ptr, self._img_vec, self._s2p, self._inv_sqrt_m, qd, d)
             dd = torch.empty(nq, 3, n3, n3, dtype=torch.complex128, device=dev)
             self.kernels.dynamical_matrix_derivatives(self._fc, self._img_ptr, self._img_vec, self._s2p,
                                                       self._inv_sqrt_m, qd, self._lattice, dd)
-            lam, e = torch.linalg.eigh(d)
-            nu = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
             m = e.conj().transpose(1, 2)[:, None] @ dd @ e[:, None]  # [nq, 3, n3, n3]
             dlam = torch.diagonal(m, dim1=-2, dim2=-1).real.clone()  # [nq, 3, n3]
             # degenerate sets: set ids ascending along the (ascending) modes
@@ -383,7 +402,7 @@ class Phonons:
                 dlam[idx] = ev - shift
             anu = nu.abs()[:, None, :]
             v = torch.where(anu >= THERMAL_CUTOFF_THZ, c2 * dlam / (2 * anu.clamp_min(THERMAL_CUTOFF_THZ)), 0.0)
-            out[s : s + chunk] = v.transpose(1, 2).cpu().numpy()
+            out[s] = v.transpose(1, 2).cpu().numpy()
         return out[0] if single else out
 
     def _mesh_frequencies(self, mesh, *, projected: bool = False):
@@ -396,15 +415,10 @@ class Phonons:
         n3, dev = 3 * n_prim, self.device
         nu = torch.empty(len(q), n3, dtype=torch.float64, device=dev)
         proj = torch.empty(len(q), n3, n_prim, dtype=torch.float64, device=dev) if projected else None
-        chunk = max(1, min(self.chunk_bytes // (16 * n3 * n3), self.eigh_batch))
-        for s in range(0, len(q), chunk):
-            d = self.dynamical_matrices(q[s : s + chunk])
+        for s, nu_s, e in self._eigh_chunks(q, eigenvectors=projected, eigh_batch=self.eigh_batch):
             if projected:
-                lam, e = torch.linalg.eigh(d)
-                proj[s : s + chunk] = (e.abs() ** 2).view(-1, n_prim, 3, n3).sum(dim=2).transpose(1, 2)
-            else:
-                lam = torch.linalg.eigvalsh(d)
-            nu[s : s + chunk] = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+                proj[s] = (e.abs() ** 2).view(-1, n_prim, 3, n3).sum(dim=2).transpose(1, 2)
+            nu[s] = nu_s
         return nu, proj
 
     def dos(self, mesh, frequency_points=None, *, projected: bool = False) -> dict:
@@ -455,22 +469,16 @@ class Phonons:
         the mesh, as in ``thermal_properties``: U is not meaningful when it is not 0.  D(q), the eigenvectors and the
         sums (``chg_thermal_displacements``) stay on the device, in chunks of at most ``eigh_batch`` q; only the
         [T, n_prim, 6] sums are copied back."""
-        temps = np.asarray(temperatures, dtype=np.float64).reshape(-1)
-        if not np.all(np.isfinite(temps)) or np.any(temps < 0):
-            raise ValueError(f"temperatures must be finite and non-negative, got {temps.tolist()}")
+        temps = _temperatures(temperatures)
         q = gamma_mesh(mesh)
-        n_prim = len(self.p2s)
-        n3, dev = 3 * n_prim, self.device
+        n_prim, dev = len(self.p2s), self.device
         t = torch.as_tensor(temps).to(dev)
         acc = torch.zeros(len(temps), n_prim, 6, dtype=torch.float64, device=dev)
         n_imaginary = torch.zeros((), dtype=torch.int64, device=dev)
-        chunk = max(1, min(self.chunk_bytes // (16 * n3 * n3), self.eigh_batch))
-        for s in range(0, len(q), chunk):
-            lam, e = torch.linalg.eigh(self.dynamical_matrices(q[s : s + chunk]))
-            nu = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
+        for s, nu, e in self._eigh_chunks(q, eigenvectors=True, eigh_batch=self.eigh_batch):
             n_imaginary += (nu < -THERMAL_CUTOFF_THZ).sum()
-            if s == 0:  # q index 0 is Gamma
-                nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0
+            if s.start == 0:  # q index 0 is Gamma
+                _zero_gamma_acoustic(nu)
             # eigh returns column-major matrices: e.mT is the mode-major layout of the kernel, without a copy
             self.kernels.thermal_displacements(nu, e.mT.contiguous(), t, THERMAL_CUTOFF_THZ, acc)
         v = acc.cpu().numpy() * (DISPLACEMENT_A2_AMU_THZ / len(q)) / self.masses[None, :, None]
@@ -482,15 +490,11 @@ class Phonons:
         """The mesh, its frequencies on the device with the three modes of smallest |nu| at Gamma set to 0 (still
         ascending), ``n_imaginary`` (counted before that), the tetrahedra and the temperatures (None or [T] on the
         device) for ``joint_dos`` and ``phase_space``."""
-        temps = None
-        if temperatures is not None:
-            temps = np.asarray(temperatures, dtype=np.float64).reshape(-1)
-            if not np.all(np.isfinite(temps)) or np.any(temps < 0):
-                raise ValueError(f"temperatures must be finite and non-negative, got {temps.tolist()}")
+        temps = None if temperatures is None else _temperatures(temperatures)
         mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
         nu = self._mesh_frequencies(mesh)[0]
         n_imaginary = (nu < -THERMAL_CUTOFF_THZ).sum()
-        nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0  # q index 0 is Gamma
+        _zero_gamma_acoustic(nu)
         tets = torch.as_tensor(tetrahedra(mesh, self.cell.prim_lattice)).to(self.device)
         t = None if temps is None else torch.as_tensor(temps).to(self.device)
         return mesh, nu, n_imaginary, tets, temps, t

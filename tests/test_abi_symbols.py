@@ -50,6 +50,17 @@ def test_binding_table_matches_header(lib):
         assert len(proto.split(",")) == len(argtypes), name
 
 
+def test_scratch_chunk_counts_match_header():
+    """The wrappers size the kernels' scratch from copies of the header's chunk limits: a copy smaller than its
+    #define would let the kernels write past the scratch."""
+    from chgnet_b200 import _lib
+
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "chgnet_b200.h")).read(), flags=re.S)
+    for name in ("DOS_MAX_CHUNKS", "TD_MAX_CHUNKS", "JDOS_MAX_CHUNKS"):
+        value = int(re.search(rf"#define CHG_{name}\s+(\d+)", src).group(1))
+        assert getattr(_lib, name) == value, name
+
+
 def test_library_metadata(lib):
     assert lib.chg_abi_version() == 3
     assert lib.chg_launch_count() >= 0

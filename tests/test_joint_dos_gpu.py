@@ -1,24 +1,21 @@
 """-m gpu: two-phonon joint densities of states on the device (Phonons.joint_dos, Phonons.phase_space).
 
-* ``chg_joint_dos`` against its fp64 specification (oracle/joint_dos.py, run with torch on the same device) on random
+* ``chg_joint_dos`` against its fp64 specification (oracle/phonons.py, run with torch on the same device) on random
   ascending frequencies with negative values, values below and on the cutoff: 24 bands on a 16^3 mesh with 256
   targets at their own 24 mode frequencies (n_t = 0 and n_t = 31), 93 bands (31 atoms) on 4^3 with a 201-point grid,
   and frequencies on a coarse grid (tied corner values, frequency points on corner values); bitwise reproducible;
 * the device force constants of LiMnO2 2x2x2: ``joint_dos`` and ``phase_space`` on a 10^3 mesh against the
   specification path on the same force constants."""
-import os
-
 import numpy as np
+import phonon_cells
 import pytest
 import torch
 
-from chgnet_b200 import graphgen
 from chgnet_b200.phonons import THERMAL_CUTOFF_THZ, Phonons, tetrahedra
-from oracle.joint_dos import JointDosSpecKernels
+from oracle.phonons import PhononSpecKernels
 
 pytestmark = pytest.mark.gpu
 
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
 TEMPS = np.linspace(0.0, 1500.0, 31)
 
 
@@ -51,7 +48,7 @@ def _compare(case, nu, mesh, targets, omega, temps, spec_every=1):
         return out
 
     got, again = run(kern, tg, omega), run(kern, tg, omega)
-    spec = JointDosSpecKernels()
+    spec = PhononSpecKernels()
     spec.jdos_chunk_items = 1 << 20
     sub = slice(None, None, spec_every)
     want = run(spec, tg[sub].contiguous(), omega[sub].contiguous())
@@ -93,16 +90,13 @@ def test_kernel_matches_spec_ties_and_vertices():
 
 @pytest.fixture(scope="module")
 def limno2_222():
-    from chgnet_b200.model import CHGNet
-
-    model = CHGNet.from_file(os.path.join(GOLD, "chgnet_0.3.0_weights.npz"), version="0.3.0").to("cuda")
-    return model.phonons(graphgen.limno2_structure(), [2, 2, 2])
+    return phonon_cells.limno2_222(phonon_cells.model030())
 
 
 def test_device_path_matches_spec_path(limno2_222):
     ph = limno2_222
     mesh = (10, 10, 10)
-    spec = Phonons(ph.force_constants, ph.cell, device="cuda", kernels=JointDosSpecKernels())
+    spec = Phonons(ph.force_constants, ph.cell, device="cuda", kernels=PhononSpecKernels())
     spec.kernels.jdos_chunk_items = 1 << 20
     # away from Gamma: there the class-1 tetrahedra of l1 = l2 are flat to rounding and D2(1) at w = 0 is ~1/ulp
     q = np.array([[0.3, 0.3, 0.0], [0.5, 0.0, 0.0], [0.1, 0.2, 0.3], [-0.4, 0.5, 0.7]])

@@ -1,5 +1,5 @@
 """CPU (fp64): two-phonon joint densities of states of chgnet_b200.phonons (``Phonons.joint_dos``,
-``Phonons.phase_space``) with the specification of ``chg_joint_dos`` (oracle/joint_dos.py).
+``Phonons.phase_space``) with the specification of ``chg_joint_dos`` (oracle/phonons.py).
 
 * the specification against a plain loop over (q1, tetrahedron, band pair, term), with negative frequencies, values
   below and on the cutoff, tied corner values, frequency points on corner values and T = 0;
@@ -15,11 +15,10 @@ import pytest
 import torch
 
 from chgnet_b200 import graphgen
-from chgnet_b200.phonons import (H_OVER_KB_K_PER_THZ, THERMAL_CUTOFF_THZ, Phonons, gamma_mesh, make_supercell,
-                                 tetrahedra)
-from oracle.joint_dos import JointDosSpecKernels
+from chgnet_b200.phonons import H_OVER_KB_K_PER_THZ, THERMAL_CUTOFF_THZ, gamma_mesh, tetrahedra
 from oracle.phonon_dos import tetrahedron_weights
-from oracle.phonons import oracle_compact_fcs
+from oracle.phonons import PhononSpecKernels
+from phonon_cells import limno2_211_spec, spec_phonons
 
 CUT = THERMAL_CUTOFF_THZ
 f64 = torch.float64
@@ -81,7 +80,7 @@ def _random_freqs(n_q, nb, rng, grid=None):
 def _terms(freqs, mesh, targets, omega, temps, tets=None):
     tets = tetrahedra(mesh, np.eye(3)) if tets is None else tets
     om = torch.as_tensor(np.broadcast_to(omega, (len(targets), len(omega))).copy())
-    return JointDosSpecKernels().joint_dos_terms(
+    return PhononSpecKernels().joint_dos_terms(
         torch.as_tensor(freqs), mesh, torch.as_tensor(tets), torch.as_tensor(np.asarray(targets, dtype=np.int32)), om,
         None if temps is None else torch.as_tensor(np.asarray(temps, dtype=np.float64)), CUT).numpy()
 
@@ -101,10 +100,10 @@ def test_spec_matches_plain_loop(grid):
         err = np.abs(got[i] - want).max() / np.abs(want).max()
         assert err <= 1e-13, (tq, err)
     out = torch.empty(len(targets), 1 + len(temps), 2, len(omega), dtype=f64)
-    JointDosSpecKernels().joint_dos(torch.as_tensor(freqs), mesh, torch.as_tensor(tets),
-                                    torch.as_tensor(np.asarray(targets, dtype=np.int32)),
-                                    torch.as_tensor(np.broadcast_to(omega, (3, len(omega))).copy()),
-                                    torch.as_tensor(temps), CUT, out)
+    PhononSpecKernels().joint_dos(torch.as_tensor(freqs), mesh, torch.as_tensor(tets),
+                                  torch.as_tensor(np.asarray(targets, dtype=np.int32)),
+                                  torch.as_tensor(np.broadcast_to(omega, (3, len(omega))).copy()),
+                                  torch.as_tensor(temps), CUT, out)
     assert np.array_equal(out[:, :, 0].numpy(), got[:, :, 0] + got[:, :, 1])
     assert np.array_equal(out[:, :, 1].numpy(), got[:, :, 2])
     # the two class-1 terms are one sum mapped by q1 -> q - q1, l1 <-> l2 (the kernel evaluates one and doubles it)
@@ -168,24 +167,6 @@ def test_time_reversal():
     b = _terms(freqs, mesh, [int(minus[t]) for t in targets], omega, [0.0, 300.0])
     assert all(minus[t] != t for t in targets)
     assert np.abs(a - b).max() <= 1e-12 * np.abs(a).max()
-
-
-# one atom per simple cubic cell, nearest-neighbour springs: three 1D chains, nu_a = NU_MAX |sin pi q_a|
-A, K, Z = 2.7, 3.0, 13
-
-
-def _sc_springs(m, ks=(K, K, K)):
-    sc = make_supercell([Z], np.zeros((1, 3)), A * np.eye(3), m)
-    fc = np.zeros((1, len(sc.z), 3, 3))
-    for a in range(3):
-        for sgn in (1, -1):
-            d = np.zeros(3)
-            d[a] = sgn
-            x = (d @ np.linalg.inv(sc.matrix.astype(np.float64))) % 1.0
-            j = int(np.argmin(np.abs((sc.frac - x + 0.5) % 1.0 - 0.5).sum(1)))
-            fc[0, j, a, a] -= ks[a]
-        fc[0, 0, a, a] += 2 * ks[a]
-    return Phonons(fc, sc, device="cpu", kernels=JointDosSpecKernels())
 
 
 def _chain_freqs(q, nu0=0.0):
@@ -272,9 +253,7 @@ def test_classical_limit():
 
 @pytest.fixture(scope="module")
 def limno2_211(weights030):
-    sc = make_supercell(*graphgen.limno2_structure(), [2, 1, 1])
-    g = graphgen.make_crystal_graph(sc.z, sc.frac, sc.lattice)
-    return Phonons(oracle_compact_fcs(weights030, g, sc.p2s), sc, device="cpu", kernels=JointDosSpecKernels())
+    return limno2_211_spec(weights030)
 
 
 def test_phase_space_equals_joint_dos_at_the_modes(limno2_211):
@@ -313,7 +292,7 @@ def test_host_path(limno2_211):
     assert jd["jdos"].shape == (3, 2, 201) and jd["weighted_jdos"].shape == (3, 3, 2, 201)
     w = jd["frequency_points"]
     assert w[0] == 0 and w[-1] == 2 * ps["frequencies"].max()
-    small = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=JointDosSpecKernels())
+    small = spec_phonons(ph.force_constants, ph.cell)
     small.eigh_batch = 5
     small.jdos_chunk_bytes = 1  # one target per call
     jd2, ps2 = small.joint_dos(mesh, q, temperatures=temps), small.phase_space(mesh, temps)

@@ -1,25 +1,22 @@
 """-m gpu: phonon group velocities and densities of states on the device (Phonons.group_velocities, Phonons.dos).
 
-* ``chg_dynamical_matrix_derivatives`` against its fp64 specification (oracle/phonon_dos.py) with synthetic force
+* ``chg_dynamical_matrix_derivatives`` against its fp64 specification (oracle/phonons.py) with synthetic force
   constants at the sizes of test_phonons_gpu.py: LiMnO2 4x4x4 on a 16^3 mesh, a 31-atom random cell 3x3x3, a
   non-diagonal supercell; bitwise reproducible and written Hermitian;
 * ``chg_tetrahedron_dos`` with projections on a 24^3 mesh against its specification, with tied vertex values and
   frequency points on vertices; bitwise reproducible;
 * the device force constants of LiMnO2 2x2x2: ``group_velocities`` and ``dos`` against the specification path on the
   same force constants, and the acoustic velocities near Gamma."""
-import os
-
 import numpy as np
+import phonon_cells
 import pytest
 import torch
 
 from chgnet_b200 import graphgen
-from chgnet_b200.phonons import Phonons, gamma_mesh, make_supercell, tetrahedra
-from oracle.phonon_dos import PhononDosSpecKernels
+from chgnet_b200.phonons import gamma_mesh, make_supercell, tetrahedra
+from oracle.phonons import PhononSpecKernels
 
 pytestmark = pytest.mark.gpu
-
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
 @pytest.mark.parametrize("case", ["limno2_444_mesh16", "random31_333", "limno2_nondiagonal"])
@@ -48,7 +45,7 @@ def test_derivative_kernel_matches_spec(case):
     again = torch.empty_like(got)
     kern.dynamical_matrix_derivatives(*args, again)
     want = torch.empty_like(got)
-    PhononDosSpecKernels().dynamical_matrix_derivatives(*args, want)
+    PhononSpecKernels().dynamical_matrix_derivatives(*args, want)
     scale = float(want.abs().max())
     err = float((got - want).abs().max()) / scale
     print(case, f"max|dD/dQ - spec| / max|dD/dQ| = {err:.2e} (max {scale:.3e})")
@@ -79,7 +76,7 @@ def test_tetrahedron_dos_kernel_matches_spec():
         k.tetrahedron_dos(f, mesh, tets, w, out[0], out[1], p if with_proj else None, pd)
         return out + ([pd] if with_proj else [])
 
-    got, again, want = run(kern), run(kern), run(PhononDosSpecKernels())
+    got, again, want = run(kern), run(kern), run(PhononSpecKernels())
     plain = run(kern, with_proj=False)
     for name, a, b, c in zip(("dos", "idos", "pdos"), got, again, want):
         scale = float(c.abs().max())
@@ -92,12 +89,8 @@ def test_tetrahedron_dos_kernel_matches_spec():
 
 @pytest.fixture(scope="module")
 def limno2_222():
-    from chgnet_b200.model import CHGNet
-
-    model = CHGNet.from_file(os.path.join(GOLD, "chgnet_0.3.0_weights.npz"), version="0.3.0").to("cuda")
-    ph = model.phonons(graphgen.limno2_structure(), [2, 2, 2])
-    spec = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=PhononDosSpecKernels())
-    return ph, spec
+    ph = phonon_cells.limno2_222(phonon_cells.model030())
+    return ph, phonon_cells.spec_phonons(ph.force_constants, ph.cell)
 
 
 def test_group_velocities_and_dos_match_spec_path(limno2_222):

@@ -1,5 +1,5 @@
 """CPU (fp64): group velocities and the linear tetrahedron density of states of chgnet_b200.phonons, with the
-specifications of ``chg_dynamical_matrix_derivatives`` and ``chg_tetrahedron_dos`` (oracle/phonon_dos.py).
+specifications of ``chg_dynamical_matrix_derivatives`` and ``chg_tetrahedron_dos`` (oracle/phonons.py).
 
 * single-tetrahedron identities of the closed forms, and a Monte-Carlo histogram;
 * a one-atom simple cubic crystal with nearest-neighbour central springs (three independent 1D chains): group
@@ -11,9 +11,10 @@ import pytest
 import torch
 
 from chgnet_b200 import graphgen
-from chgnet_b200.phonons import (THZ_PER_SQRT_EV_A2_AMU, Phonons, gamma_mesh, make_supercell, tetrahedra)
-from oracle.phonon_dos import PhononDosSpecKernels, tetrahedron_weights
-from oracle.phonons import oracle_compact_fcs
+from chgnet_b200.phonons import gamma_mesh, tetrahedra
+from oracle.phonon_dos import tetrahedron_weights
+from oracle.phonons import PhononSpecKernels
+from phonon_cells import A, limno2_211_spec, springs
 
 
 def _vertex_sets():
@@ -88,24 +89,11 @@ def test_single_tetrahedron_monte_carlo():
     assert np.abs(w_mc - want_w).max() <= 5 * sigma_n.max()
 
 
-# one atom per simple cubic cell (lattice constant A), nearest-neighbour central springs K: nu_a = NU_MAX |sin pi q_a|
-A, K, Z = 2.7, 3.0, 13
-
-
 def _sc_springs(m):
-    sc = make_supercell([Z], np.zeros((1, 3)), A * np.eye(3), m)
-    n = len(sc.z)
-    fc = np.zeros((1, n, 3, 3))
-    for a in range(3):
-        for sgn in (1, -1):
-            d = np.zeros(3)
-            d[a] = sgn
-            x = (d @ np.linalg.inv(sc.matrix.astype(np.float64))) % 1.0  # supercell fractional position of r0 + d
-            j = int(np.argmin(np.abs((sc.frac - x + 0.5) % 1.0 - 0.5).sum(1)))
-            fc[0, j, a, a] -= K
-        fc[0, 0, a, a] += 2 * K
-    ph = Phonons(fc, sc, device="cpu", kernels=PhononDosSpecKernels())
-    return ph, THZ_PER_SQRT_EV_A2_AMU * np.sqrt(4 * K / ph.masses[0])
+    """One atom per simple cubic cell (lattice constant A), nearest-neighbour central springs: nu_a = nu_max
+    |sin pi q_a|."""
+    ph, nu_max = springs(m)
+    return ph, nu_max[0]
 
 
 @pytest.mark.parametrize("m", [[3, 3, 3], [2, 2, 2]])
@@ -158,9 +146,7 @@ def test_spring_crystal_dos_converges_to_the_chain():
 
 @pytest.fixture(scope="module")
 def limno2_211_fc(weights030):
-    sc = make_supercell(*graphgen.limno2_structure(), [2, 1, 1])
-    g = graphgen.make_crystal_graph(sc.z, sc.frac, sc.lattice)
-    return Phonons(oracle_compact_fcs(weights030, g, sc.p2s), sc, device="cpu", kernels=PhononDosSpecKernels())
+    return limno2_211_spec(weights030)
 
 
 def test_limno2_group_velocities_match_finite_differences(limno2_211_fc):
@@ -197,7 +183,7 @@ def test_limno2_dos_sum_rules_and_diagonal(limno2_211_fc):
     assert (np.diff(out["integrated_dos"]) >= -1e-12).all()
     # the body diagonal of the tetrahedra changes the result only by the discretisation
     nu = torch.as_tensor(ph.frequencies(gamma_mesh(mesh)))
-    kern = PhononDosSpecKernels()
+    kern = PhononSpecKernels()
     dos = []
     for d in range(4):
         tot, idos = torch.empty(201, dtype=torch.float64), torch.empty(201, dtype=torch.float64)
@@ -218,7 +204,7 @@ def test_tetrahedron_diagonals_agree_within_discretisation():
     """A band with no mirror symmetry: the four diagonals give different tetrahedra and agree to the discretisation
     error, which falls with the mesh."""
     lat = graphgen.limno2_structure()[2]
-    kern = PhononDosSpecKernels()
+    kern = PhononSpecKernels()
     w = torch.linspace(-1.2, 1.2, 49, dtype=torch.float64)
     spreads = []
     for n in (12, 24):

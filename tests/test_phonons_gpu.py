@@ -9,17 +9,17 @@
 import os
 
 import numpy as np
+import phonon_cells
 import pytest
 import torch
 
 from chgnet_b200 import graphgen
-from chgnet_b200.phonons import (THZ_PER_SQRT_EV_A2_AMU, Phonons, gamma_mesh, make_supercell,
+from chgnet_b200.phonons import (THZ_PER_SQRT_EV_A2_AMU, gamma_mesh, make_supercell,
                                  thermal_properties_from_frequencies)
 from oracle.phonons import PhononSpecKernels, oracle_compact_fcs
 
 pytestmark = pytest.mark.gpu
 
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
 # the fp32 device force constants against the fp64 oracle, as fractions of max|Phi| (TOL of test_hessian_gpu.py)
 TOL = 2e-3
 
@@ -32,14 +32,12 @@ def _eigenvalues(nu):
 
 @pytest.fixture(scope="module")
 def model030():
-    from chgnet_b200.model import CHGNet
-
-    return CHGNet.from_file(os.path.join(GOLD, "chgnet_0.3.0_weights.npz"), version="0.3.0").to("cuda")
+    return phonon_cells.model030()
 
 
 @pytest.fixture(scope="module")
 def limno2_222(model030):
-    return model030.phonons(graphgen.limno2_structure(), [2, 2, 2])
+    return phonon_cells.limno2_222(model030)
 
 
 @pytest.mark.parametrize("case", ["limno2_444_mesh16", "random31_333", "limno2_nondiagonal"])
@@ -104,7 +102,7 @@ def test_device_force_constants_match_oracle(model030, weights030, limno2_222, c
 
 
 def test_gamma_matches_live_reference(limno2_222):
-    with np.load(os.path.join(GOLD, "chgnet_0.3.0_hessian.npz")) as f:
+    with np.load(os.path.join(phonon_cells.GOLD, "chgnet_0.3.0_hessian.npz")) as f:
         h = f["limno2.hessian"]
     mw = 1.0 / np.sqrt(np.repeat(limno2_222.masses, 3))
     d = mw[:, None] * h * mw[None, :]
@@ -139,7 +137,7 @@ def test_commensurate_q_match_supercell_hessian(model030, limno2_222):
 def test_thermal_properties_match_host_formula(limno2_222):
     mesh, temps = (6, 6, 6), [0.0, 50.0, 300.0, 1000.0]
     got = limno2_222.thermal_properties(mesh, temps)
-    spec = Phonons(limno2_222.force_constants, limno2_222.cell, device="cpu", kernels=PhononSpecKernels())
+    spec = phonon_cells.spec_phonons(limno2_222.force_constants, limno2_222.cell)
     d = spec.dynamical_matrices(gamma_mesh(mesh)).numpy()
     lam = np.linalg.eigvalsh(d)
     want = thermal_properties_from_frequencies(np.sign(lam) * np.sqrt(np.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU, temps)

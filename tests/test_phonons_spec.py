@@ -7,6 +7,7 @@ The force constants come from the kernel schedule with the torch specifications 
 import itertools
 
 import numpy as np
+import phonon_cells
 import pytest
 import torch
 
@@ -14,16 +15,14 @@ from chgnet_b200 import graphgen
 from chgnet_b200.batch import build_batch
 from chgnet_b200.dynamics import KB
 from chgnet_b200.engine import Engine
-from chgnet_b200.phonons import (H_EV_PER_THZ, THZ_PER_SQRT_EV_A2_AMU, Phonons, compact_force_constants,
-                                 make_supercell, thermal_properties_from_frequencies)
+from chgnet_b200.phonons import (H_EV_PER_THZ, THZ_PER_SQRT_EV_A2_AMU, compact_force_constants, make_supercell,
+                                 thermal_properties_from_frequencies)
 from chgnet_b200.weights import pack_weights
 from oracle.hessian import HessianSpecKernels, oracle_hessian
-from oracle.phonons import PhononSpecKernels, oracle_compact_fcs
+from oracle.phonons import oracle_compact_fcs
 
 SKEWED = [[1, 3, 0], [0, 1, 0], [0, 0, 2]]
 NONDIAG = [[1, 1, 0], [-1, 1, 0], [0, 0, 1]]
-# one atom per cell: fcc Cu, primitive lattice
-CU = (np.array([29]), np.zeros((1, 3)), 1.805 * (np.ones((3, 3)) - np.eye(3)))
 
 
 def spec_hvp(weights):
@@ -106,10 +105,8 @@ def test_bad_supercell_matrix(m):
 
 @pytest.fixture(scope="module")
 def limno2_211(weights030):
-    z, frac, lat = graphgen.limno2_structure()
-    sc = make_supercell(z, frac, lat, [2, 1, 1])
-    g = graphgen.make_crystal_graph(sc.z, sc.frac, sc.lattice)
-    return sc, g, oracle_hessian(weights030, g), oracle_compact_fcs(weights030, g, sc.p2s)
+    sc, g, fc = phonon_cells.limno2_211(weights030)
+    return sc, g, oracle_hessian(weights030, g), fc
 
 
 def test_translation_identity_of_oracle_supercell_hessian(limno2_211):
@@ -135,7 +132,7 @@ def test_spec_engine_force_constants_match_oracle(weights030, limno2_211):
     got = compact_force_constants(lambda v: hvp(g, v), sc)
     assert got.shape == (8, 16, 3, 3)
     assert np.abs(got - want).max() <= 1e-6 * np.abs(want).max()
-    sc1 = make_supercell(*CU, [2, 2, 2])
+    sc1 = make_supercell(*phonon_cells.CU, [2, 2, 2])
     g1 = graphgen.make_crystal_graph(sc1.z, sc1.frac, sc1.lattice)
     want1 = oracle_compact_fcs(weights030, g1, sc1.p2s)
     got1 = compact_force_constants(lambda v: hvp(g1, v), sc1)
@@ -144,7 +141,7 @@ def test_spec_engine_force_constants_match_oracle(weights030, limno2_211):
 
 
 def _spec_dyn(fc, sc, q):
-    ph = Phonons(fc, sc, device="cpu", kernels=PhononSpecKernels())
+    ph = phonon_cells.spec_phonons(fc, sc)
     ph._fc = torch.as_tensor(fc)  # the identities hold for the force constants as computed (no ASR correction)
     return ph.dynamical_matrices(q).numpy(), ph.masses
 
@@ -175,7 +172,7 @@ def test_exact_identities_of_the_dynamical_matrix(weights030, limno2_211, m):
 
 def test_frequencies_path_with_spec_kernels(limno2_211):
     sc, _, _, fc = limno2_211
-    ph = Phonons(fc, sc, device="cpu", kernels=PhononSpecKernels())
+    ph = phonon_cells.spec_phonons(fc, sc)
     assert ph.supercell[0].shape == (16,) and ph.asr_correction < 1e-9 * np.abs(fc).max()
     rng = np.random.default_rng(3)
     q = np.vstack([np.zeros(3), rng.uniform(-0.5, 0.5, size=(6, 3))])

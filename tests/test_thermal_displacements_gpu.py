@@ -1,27 +1,23 @@
 """-m gpu: thermal displacement matrices on the device (Phonons.thermal_displacement_matrices).
 
-* ``chg_thermal_displacements`` against its fp64 specification (oracle/thermal_displacements.py) at production sizes:
+* ``chg_thermal_displacements`` against its fp64 specification (oracle/phonons.py) at production sizes:
   4 096 q x 24 modes x 31 temperatures, the 31-atom cell's 93 modes, one temperature, one atom, 300 temperatures (two
   temperature tiles); bitwise reproducible, exact doubling on a second accumulation, and the Einstein identity;
 * the device force constants of LiMnO2 2x2x2 on a 20^3 mesh (two eigh chunks): the device path against the
   specification path on the same force constants;
 * fcc Cu 4x4x4 (0.3.0 weights): U at 300 K on 8^3, 16^3 and 24^3 meshes, cubic isotropy and the CIF form."""
-import os
-
 import numpy as np
+import phonon_cells
 import pytest
 import torch
 
-from chgnet_b200 import graphgen
-from chgnet_b200.phonons import H_OVER_KB_K_PER_THZ, THERMAL_CUTOFF_THZ, Phonons
-from oracle.thermal_displacements import ThermalDisplacementSpecKernels
+from chgnet_b200.phonons import H_OVER_KB_K_PER_THZ, THERMAL_CUTOFF_THZ
+from oracle.phonons import PhononSpecKernels
+from phonon_cells import CU
 
 pytestmark = pytest.mark.gpu
 
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
 TEMPS = np.linspace(0.0, 1500.0, 31)
-# fcc Cu, one atom per rhombohedral primitive cell
-CU = (np.array([29]), np.zeros((1, 3)), 1.805 * (np.ones((3, 3)) - np.eye(3)))
 
 
 def _random_modes(n_q, n_prim, seed, equal=None):
@@ -60,7 +56,7 @@ def test_kernel_matches_spec(case):
         k.thermal_displacements(nu, e, t, THERMAL_CUTOFF_THZ, acc)
         return acc
 
-    got, want = run(kern), run(ThermalDisplacementSpecKernels())
+    got, want = run(kern), run(PhononSpecKernels())
     again = run(kern)
     twice = run(kern, got.clone())
     scale = float(want.abs().max())
@@ -88,13 +84,11 @@ def test_kernel_einstein_identity():
 
 @pytest.fixture(scope="module")
 def model030():
-    from chgnet_b200.model import CHGNet
-
-    return CHGNet.from_file(os.path.join(GOLD, "chgnet_0.3.0_weights.npz"), version="0.3.0").to("cuda")
+    return phonon_cells.model030()
 
 
 def test_device_path_matches_spec_path(model030):
-    ph = model030.phonons(graphgen.limno2_structure(), [2, 2, 2])
+    ph = phonon_cells.limno2_222(model030)
     mesh = (20, 20, 20)  # 8 000 q: two eigh chunks of at most 4 096
     assert 20**3 > ph.eigh_batch
     d = ph.dynamical_matrices(np.zeros((2, 3)))
@@ -102,7 +96,7 @@ def test_device_path_matches_spec_path(model030):
     print("eigh eigenvectors on the device: strides", e.stride(), "; e.mT contiguous:", e.mT.is_contiguous())
     got = ph.thermal_displacement_matrices(mesh, TEMPS)
     again = ph.thermal_displacement_matrices(mesh, TEMPS)
-    spec = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=ThermalDisplacementSpecKernels())
+    spec = phonon_cells.spec_phonons(ph.force_constants, ph.cell)
     want = spec.thermal_displacement_matrices(mesh, TEMPS)
     scale = np.abs(want["cartesian"]).max()
     err = np.abs(got["cartesian"] - want["cartesian"]).max() / scale

@@ -1,5 +1,5 @@
 """CPU (fp64): thermal displacement matrices of chgnet_b200.phonons (Phonons.thermal_displacement_matrices), with the
-specification of ``chg_thermal_displacements`` (oracle/thermal_displacements.py).
+specification of ``chg_thermal_displacements`` (oracle/phonons.py).
 
 * the specification against a plain triple loop, and the Einstein identity;
 * simple cubic and orthorhombic crystals of nearest-neighbour central springs (three independent 1D chains): the exact
@@ -14,12 +14,12 @@ import numpy as np
 import pytest
 import torch
 
-from chgnet_b200 import graphgen
 from chgnet_b200.phonons import (DISPLACEMENT_A2_AMU_THZ, H_OVER_KB_K_PER_THZ, THERMAL_CUTOFF_THZ,
-                                 THZ_PER_SQRT_EV_A2_AMU, Phonons, acoustic_sum_rule, cif_displacement_matrices,
-                                 gamma_mesh, make_supercell)
-from oracle.phonons import oracle_compact_fcs
-from oracle.thermal_displacements import VOIGT, ThermalDisplacementSpecKernels
+                                 THZ_PER_SQRT_EV_A2_AMU, acoustic_sum_rule, cif_displacement_matrices, gamma_mesh,
+                                 make_supercell)
+from oracle.phonons import PhononSpecKernels
+from oracle.thermal_displacements import VOIGT
+from phonon_cells import CU, K, limno2_211_spec, spec_phonons, springs
 
 C = DISPLACEMENT_A2_AMU_THZ
 TEMPS = np.array([0.0, 10.0, 300.0, 1500.0])
@@ -37,8 +37,8 @@ def _coth_over_nu(nu, t):
 
 def _spec_sums(freqs, vecs, temps):
     acc = torch.zeros(len(temps), freqs.shape[1] // 3, 6, dtype=torch.float64)
-    ThermalDisplacementSpecKernels().thermal_displacements(torch.as_tensor(freqs), torch.as_tensor(vecs),
-                                                           torch.as_tensor(temps), THERMAL_CUTOFF_THZ, acc)
+    PhononSpecKernels().thermal_displacements(torch.as_tensor(freqs), torch.as_tensor(vecs), torch.as_tensor(temps),
+                                              THERMAL_CUTOFF_THZ, acc)
     return acc.numpy()
 
 
@@ -77,33 +77,6 @@ def test_einstein_identity():
         assert np.abs(got[t] - want).max() <= 1e-13 * np.abs(want).max()
 
 
-# nearest-neighbour central springs along the axes of an orthorhombic lattice diag(a) with constants ks:
-# branch c has nu_c(q) = nu_max,c |sin pi q_c|
-A, K, Z = 2.7, 3.0, 13
-
-
-def _springs(m, ks=(K, K, K), a=(A, A, A), frac=((0.0, 0.0, 0.0),), cell=(1, 1, 1), noise=0.0, seed=0):
-    """A spring crystal whose primitive cell is ``cell`` simple orthorhombic cells (atoms at ``frac``)."""
-    lat = np.diag(np.asarray(a, dtype=np.float64) * cell)
-    frac = np.asarray(frac, dtype=np.float64)
-    sc = make_supercell([Z] * len(frac), frac, lat, m)
-    n = len(sc.z)
-    cart = sc.frac @ sc.lattice
-    inv = np.linalg.inv(sc.lattice)
-    fc = np.zeros((len(frac), n, 3, 3))
-    for k, k0 in enumerate(sc.p2s):
-        for c in range(3):
-            for sgn in (1, -1):
-                x = ((cart[k0] + sgn * a[c] * np.eye(3)[c]) @ inv) % 1.0
-                j = int(np.argmin(np.abs((sc.frac - x + 0.5) % 1.0 - 0.5).sum(1)))
-                fc[k, j, c, c] -= ks[c]
-            fc[k, k0, c, c] += 2 * ks[c]
-    if noise:
-        fc += noise * np.random.default_rng(seed).normal(size=fc.shape)  # not symmetric
-    ph = Phonons(fc, sc, device="cpu", kernels=ThermalDisplacementSpecKernels())
-    return ph, THZ_PER_SQRT_EV_A2_AMU * np.sqrt(4 * np.asarray(ks) / ph.masses[0])
-
-
 def _chain_sum(nu_max, n, t):
     """(1/n) sum_{j=1}^{n-1} coth(h nu_j / 2 k T) / nu_j, nu_j = nu_max sin(pi j / n)."""
     return _coth_over_nu(nu_max * np.sin(np.pi * np.arange(1, n) / n), t).sum() / n
@@ -113,9 +86,9 @@ def _chain_sum(nu_max, n, t):
 @pytest.mark.parametrize("n", [4, 7, 8])
 def test_spring_crystal_exact_mesh_sums(crystal, n):
     if crystal == "orthorhombic_333":
-        ph, nu_max = _springs([3, 3, 3], ks=(3.0, 1.7, 4.4), a=(2.7, 3.1, 2.4))
+        ph, nu_max = springs([3, 3, 3], ks=(3.0, 1.7, 4.4), a=(2.7, 3.1, 2.4))
     else:
-        ph, nu_max = _springs([3, 3, 3] if crystal == "cubic_333" else [2, 2, 2])
+        ph, nu_max = springs([3, 3, 3] if crystal == "cubic_333" else [2, 2, 2])
     out = ph.thermal_displacement_matrices((n, n, n), TEMPS)
     u = out["cartesian"]
     assert u.shape == (4, 1, 3, 3) and out["cif"].shape == (4, 1, 3, 3) and out["n_imaginary"] == 0
@@ -191,15 +164,12 @@ def _supercell_displacements(ph, temps):
 
 @pytest.fixture(scope="module")
 def limno2_211(weights030):
-    sc = make_supercell(*graphgen.limno2_structure(), [2, 1, 1])
-    g = graphgen.make_crystal_graph(sc.z, sc.frac, sc.lattice)
-    return Phonons(oracle_compact_fcs(weights030, g, sc.p2s), sc, device="cpu",
-                   kernels=ThermalDisplacementSpecKernels())
+    return limno2_211_spec(weights030)
 
 
 @pytest.mark.parametrize("crystal", ["limno2_211", "springs_333"])
 def test_commensurate_identity(crystal, request):
-    ph = request.getfixturevalue("limno2_211") if crystal == "limno2_211" else _springs([3, 3, 3])[0]
+    ph = request.getfixturevalue("limno2_211") if crystal == "limno2_211" else springs([3, 3, 3])[0]
     mesh = np.diag(ph.cell.matrix)
     temps = np.array([0.0, 300.0, 1000.0])
     out = ph.thermal_displacement_matrices(mesh, temps)
@@ -219,7 +189,7 @@ def test_commensurate_identity(crystal, request):
 def _fcc_springs(m, doubled=False, noise=0.0, seed=0):
     """One atom per fcc primitive cell (a = 3.61 A), nearest-neighbour central springs K; with ``doubled`` the primitive
     cell is two fcc cells (lattice rows 2 a1, a2, a3), and ``noise`` adds Gaussian noise that is not symmetric."""
-    lat1 = 1.805 * (np.ones((3, 3)) - np.eye(3))
+    lat1 = CU[2]
     lat, frac = (lat1 * [[2], [1], [1]], [[0.0, 0, 0], [0.5, 0, 0]]) if doubled else (lat1, [[0.0, 0, 0]])
     sc = make_supercell([29] * len(frac), np.asarray(frac), lat, m)
     n = len(sc.z)
@@ -236,7 +206,7 @@ def _fcc_springs(m, doubled=False, noise=0.0, seed=0):
             fc[k, k0] += phi
     if noise:
         fc += noise * np.random.default_rng(seed).normal(size=fc.shape)
-    return Phonons(fc, sc, device="cpu", kernels=ThermalDisplacementSpecKernels())
+    return spec_phonons(fc, sc)
 
 
 def test_limits():
@@ -255,7 +225,7 @@ def test_limits():
     assert diffs[1] < 0.6 * diffs[0] and diffs[1] <= 1.2e-4
 
     # classical limit: U / T -> (k / N_q m) sum e e^H / omega^2, relative gap ~ (h nu / k T)^2 / 12
-    ph, nu_max = _springs([3, 3, 3], ks=(3.0, 1.7, 4.4), a=(2.7, 3.1, 2.4))
+    ph, nu_max = springs([3, 3, 3], ks=(3.0, 1.7, 4.4), a=(2.7, 3.1, 2.4))
     mesh = (5, 5, 5)
     temps = np.array([2000.0, 4000.0, 8000.0])
     u = ph.thermal_displacement_matrices(mesh, temps)["cartesian"][:, 0]
@@ -317,7 +287,7 @@ def test_chunking_n_imaginary_and_bad_temperatures(limno2_211):
     ph = limno2_211
     mesh, temps = (3, 4, 2), np.array([0.0, 150.0, 300.0, 1200.0])
     whole = ph.thermal_displacement_matrices(mesh, temps)
-    chunked = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=ThermalDisplacementSpecKernels())
+    chunked = spec_phonons(ph.force_constants, ph.cell)
     chunked.eigh_batch = 5  # Gamma in the first chunk, a short last chunk
     small = chunked.thermal_displacement_matrices(mesh, temps)
     assert np.abs(small["cartesian"] - whole["cartesian"]).max() <= 1e-13 * np.abs(whole["cartesian"]).max()

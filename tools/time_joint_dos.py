@@ -5,8 +5,8 @@
 With the force constants of LiMnO2 3x3x3 (0.3.0 weights): ``joint_dos`` at 4 q-points of a jdos-mesh^3 mesh with 201
 frequency points, without temperatures and with 31 from 0 to 1500 K; ``phase_space`` on each mesh^3 mesh at 0, 300
 and 1000 K (wall clock, ending in a synchronise), and the ``chg_joint_dos`` kernel alone over the same target chunks
-(CUDA events, on the frequencies the call uses).  Then ``phase_space`` with ``oracle/joint_dos.py``'s specification
-on the host (``Phonons(..., device="cpu", kernels=JointDosSpecKernels())``) on a host-mesh^3 mesh, with the largest
+(CUDA events, on the frequencies the call uses).  Then ``phase_space`` with ``oracle/phonons.py``'s specification
+on the host (``Phonons(..., device="cpu", kernels=PhononSpecKernels())``) on a host-mesh^3 mesh, with the largest
 difference from the device.  Prints the GPU name and power limit first: the times belong to that card.  Times are the
 fastest of ``repeats`` after a warm-up call.  Needs a CUDA device; there is no CPU fallback.
 """
@@ -27,7 +27,7 @@ sys.path.insert(0, ROOT)
 from chgnet_b200 import graphgen  # noqa: E402
 from chgnet_b200.model import CHGNet  # noqa: E402
 from chgnet_b200.phonons import Phonons  # noqa: E402
-from oracle.joint_dos import JointDosSpecKernels  # noqa: E402
+from oracle.phonons import PhononSpecKernels  # noqa: E402
 from tools.time_phonons import gpu_card, timed  # noqa: E402
 from tools.time_thermal_displacements import event_ms  # noqa: E402
 
@@ -88,7 +88,7 @@ def main() -> None:
                           "n_imaginary": out["n_imaginary"], "average_jdos": out["average_jdos"].tolist(),
                           "average_weighted_jdos": out["average_weighted_jdos"].tolist()}), flush=True)
 
-    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=JointDosSpecKernels())
+    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=PhononSpecKernels())
     hm = (a.host_mesh,) * 3
     dev = device_out.get(a.host_mesh) or ph.phase_space(hm, temps)
     t0 = time.perf_counter()

@@ -4,8 +4,8 @@
 
 With the force constants of LiMnO2 3x3x3 (0.3.0 weights): ``dos(projected=True)`` on a mesh^3 Gamma-centred mesh
 (201 points), the ``chg_tetrahedron_dos`` kernel alone on the same frequencies and projections (CUDA events), and
-``group_velocities`` on a gv-mesh^3 mesh.  Then the same calls with ``oracle/phonon_dos.py``'s specifications on the
-host (``Phonons(..., device="cpu", kernels=PhononDosSpecKernels())``), on a host-mesh^3 mesh, with the largest
+``group_velocities`` on a gv-mesh^3 mesh.  Then the same calls with ``oracle/phonons.py``'s specifications on the
+host (``Phonons(..., device="cpu", kernels=PhononSpecKernels())``), on a host-mesh^3 mesh, with the largest
 difference from the device.  Prints the GPU name and power limit first: the times belong to that card.  Wall-clock
 times are synchronised, the fastest of ``repeats`` after a warm-up call.  Needs a CUDA device; there is no CPU
 fallback.
@@ -26,8 +26,8 @@ sys.path.insert(0, ROOT)
 
 from chgnet_b200 import graphgen  # noqa: E402
 from chgnet_b200.model import CHGNet  # noqa: E402
-from chgnet_b200.phonons import THZ_PER_SQRT_EV_A2_AMU, Phonons, gamma_mesh, tetrahedra  # noqa: E402
-from oracle.phonon_dos import PhononDosSpecKernels  # noqa: E402
+from chgnet_b200.phonons import Phonons, gamma_mesh, tetrahedra  # noqa: E402
+from oracle.phonons import PhononSpecKernels  # noqa: E402
 from tools.time_phonons import gpu_card, timed  # noqa: E402
 
 
@@ -57,12 +57,7 @@ def main() -> None:
 
     # the kernel alone, on the frequencies and projections dos() builds
     q = gamma_mesh(mesh)
-    nu = torch.empty(len(q), n3, dtype=torch.float64, device="cuda")
-    proj = torch.empty(len(q), n3, n_prim, dtype=torch.float64, device="cuda")
-    for s in range(0, len(q), ph.eigh_batch):
-        lam, e = torch.linalg.eigh(ph.dynamical_matrices(q[s : s + ph.eigh_batch]))
-        nu[s : s + ph.eigh_batch] = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
-        proj[s : s + ph.eigh_batch] = (e.abs() ** 2).view(-1, n_prim, 3, n3).sum(dim=2).transpose(1, 2)
+    nu, proj = ph._mesh_frequencies(mesh, projected=True)
     omega = torch.as_tensor(out["frequency_points"]).cuda()
     tets = torch.as_tensor(tetrahedra(mesh, ph.cell.prim_lattice)).cuda()
     dos, idos = torch.empty_like(omega), torch.empty_like(omega)
@@ -89,7 +84,7 @@ def main() -> None:
     print(json.dumps({"gv_mesh": [a.gv_mesh] * 3, "n_q": len(qg), "device_group_velocities_s": round(t_gv, 4),
                       "max_abs_v_THz_A": float(np.abs(v).max())}), flush=True)
 
-    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=PhononDosSpecKernels())
+    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=PhononSpecKernels())
     hm = (a.host_mesh,) * 3
     dev_dos = ph.dos(hm, projected=True)
     host_dos, t_host_dos = host_timed(lambda: host.dos(hm, projected=True))

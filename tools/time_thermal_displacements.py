@@ -5,8 +5,8 @@
 With the force constants of LiMnO2 3x3x3 (0.3.0 weights) and 31 temperatures from 0 to 1500 K:
 ``thermal_displacement_matrices`` on each mesh^3 Gamma-centred mesh (wall clock, ending in a synchronise), and, on the
 same eigenvectors, the ``chg_thermal_displacements`` kernel alone and D(q) + ``torch.linalg.eigh`` alone (CUDA events
-around the loop over the eigh chunks).  Then the same call with ``oracle/thermal_displacements.py``'s specification on
-the host (``Phonons(..., device="cpu", kernels=ThermalDisplacementSpecKernels())``) on a host-mesh^3 mesh, with the
+around the loop over the eigh chunks).  Then the same call with ``oracle/phonons.py``'s specification on
+the host (``Phonons(..., device="cpu", kernels=PhononSpecKernels())``) on a host-mesh^3 mesh, with the
 largest difference from the device.  Prints the GPU name and power limit first: the times belong to that card.  Times
 are the fastest of ``repeats`` after a warm-up call.  Needs a CUDA device; there is no CPU fallback.
 """
@@ -26,9 +26,9 @@ sys.path.insert(0, ROOT)
 
 from chgnet_b200 import graphgen  # noqa: E402
 from chgnet_b200.model import CHGNet  # noqa: E402
-from chgnet_b200.phonons import (DISPLACEMENT_A2_AMU_THZ, THERMAL_CUTOFF_THZ, THZ_PER_SQRT_EV_A2_AMU, Phonons,  # noqa: E402
-                                 gamma_mesh)
-from oracle.thermal_displacements import ThermalDisplacementSpecKernels  # noqa: E402
+from chgnet_b200.phonons import DISPLACEMENT_A2_AMU_THZ, THERMAL_CUTOFF_THZ, Phonons, gamma_mesh  # noqa: E402
+from chgnet_b200.phonons import _zero_gamma_acoustic  # noqa: E402
+from oracle.phonons import PhononSpecKernels  # noqa: E402
 from tools.time_phonons import gpu_card, timed  # noqa: E402
 
 
@@ -69,11 +69,9 @@ def main() -> None:
         # zeroed as there)
         q = gamma_mesh(mesh)
         chunks = []
-        for s in range(0, len(q), ph.eigh_batch):
-            lam, e = torch.linalg.eigh(ph.dynamical_matrices(q[s : s + ph.eigh_batch]))
-            nu = torch.sign(lam) * torch.sqrt(torch.abs(lam)) * THZ_PER_SQRT_EV_A2_AMU
-            if s == 0:
-                nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0
+        for s, nu, e in ph._eigh_chunks(q, eigenvectors=True, eigh_batch=ph.eigh_batch):
+            if s.start == 0:
+                _zero_gamma_acoustic(nu)
             chunks.append((nu, e.mT.contiguous()))
         acc = torch.zeros(len(temps), n_prim, 6, dtype=torch.float64, device="cuda")
 
@@ -83,8 +81,7 @@ def main() -> None:
                 ph.kernels.thermal_displacements(nu, e, t_dev, THERMAL_CUTOFF_THZ, acc)
 
         kernel_ms = event_ms(kernels, a.repeats)
-        eigh_ms = event_ms(lambda: [torch.linalg.eigh(ph.dynamical_matrices(q[s : s + ph.eigh_batch]))
-                                    for s in range(0, len(q), ph.eigh_batch)], a.repeats)
+        eigh_ms = event_ms(lambda: list(ph._eigh_chunks(q, eigenvectors=True, eigh_batch=ph.eigh_batch)), a.repeats)
         v = acc.cpu().numpy() * (DISPLACEMENT_A2_AMU_THZ / len(q)) / ph.masses[None, :, None]
         same = bool(np.array_equal(v, out["cartesian"][..., [0, 1, 2, 1, 0, 0], [0, 1, 2, 2, 2, 1]]))
         del chunks
@@ -97,7 +94,7 @@ def main() -> None:
                           "U_300K_diag_A2": np.diagonal(out["cartesian"][6], axis1=1, axis2=2).round(6).tolist(),
                           "kernel_loop_equals_call": same}), flush=True)
 
-    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=ThermalDisplacementSpecKernels())
+    host = Phonons(ph.force_constants, ph.cell, device="cpu", kernels=PhononSpecKernels())
     hm = (a.host_mesh,) * 3
     dev = device_out.get(a.host_mesh) or ph.thermal_displacement_matrices(hm, temps)
     t0 = time.perf_counter()
