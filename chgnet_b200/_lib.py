@@ -72,6 +72,8 @@ SIGNATURES: dict[str, list] = {
     "chg_tetrahedron_dos": [P, I, I, I, I, P, P, I, P, I, P, P, P, P, P],
     "chg_thermal_displacements": [P, P, I, I, P, I, D, P, P, P],
     "chg_joint_dos": [P, I, I, I, I, P, P, I, P, I, P, I, D, P, P, P],
+    "chg_structure_factors": [P, P, P, P, P, P, P, P, I, I, I, D, P, P],
+    "chg_broadened_spectrum": [P, P, I, I, I, I64, I, I64, P, I, D, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -79,6 +81,20 @@ SIGNATURES: dict[str, list] = {
 DOS_MAX_CHUNKS = 512
 TD_MAX_CHUNKS = 128
 JDOS_MAX_CHUNKS = 64
+# CHG_SQW_MAX_CHUNKS: the most chunks chg_broadened_spectrum uses (tests/test_structure_factor_spec.py ties it to the
+# header); the call also uses no more chunks than its work argument holds
+SQW_MAX_CHUNKS = 64
+
+
+def sqw_scratch_doubles(n_rows, n_modes, n_t, row0, group_size, n_freq):
+    """The scratch ``CudaKernels.broadened_spectrum`` allocates for one call: n_t x (groups the rows [row0, row0 +
+    n_rows) touch) x n_freq doubles per chunk, for at most one chunk per 32 items of the largest group (the kernel's
+    smallest tile) and at most ``SQW_MAX_CHUNKS``."""
+    if n_rows <= 0:
+        return 0
+    groups = (row0 + n_rows - 1) // group_size - row0 // group_size + 1
+    chunks = max(1, min(SQW_MAX_CHUNKS, -(-min(group_size, n_rows) * n_modes // 32)))
+    return chunks * n_t * groups * n_freq
 
 _lib = None
 
@@ -473,6 +489,51 @@ class CudaKernels:
         work = _chunk_scratch(JDOS_MAX_CHUNKS, n_target * (1 + n_t) * 2 * n_f, freqs.device)
         self._call("chg_joint_dos", _p(freqs), n_band, n1, n2, n3, _p(tetrahedra), _p(targets), n_target, _p(omega),
                    n_f, _p(temperatures), n_t, float(cutoff_thz), _p(out), _p(work))
+
+    def structure_factors(self, freqs, eigvecs, kcart, gvec, frac, coef, u, temperatures, cutoff_thz, out):
+        """out [T, Q, 3n, 2] fp64 (overwritten) = (S+, S-) of every row and mode, coherent one-phonon structure
+        factors in A^2 x coef^2 (``chg_structure_factors``): freqs [Q, 3n] THz (signed), eigvecs [Q, mode, 3n]
+        complex128 (mode-major: ``e.mT`` of eigh's eigenvectors), kcart [Q, 3] Cartesian K (1/A, 2 pi included), gvec
+        [Q, 3] reduced G, frac [n, 3] fractional positions, coef [n] = b / sqrt(m), u [T, n, 6] Voigt U (A^2) or None
+        for no Debye-Waller factor, temperatures [T] K (all fp64); modes below cutoff_thz get 0."""
+        self._chk(freqs, eigvecs, kcart, gvec, frac, coef, u, temperatures, out)
+        f64 = torch.float64
+        if (any(t is not None and t.dtype != f64 for t in (freqs, kcart, gvec, frac, coef, u, temperatures, out))
+                or eigvecs.dtype != torch.complex128):
+            raise ChgnetB200Error("structure_factors: eigvecs must be complex128 and every other tensor float64")
+        n_q, n3 = freqs.shape
+        n_prim, n_t = n3 // 3, temperatures.shape[0]
+        if (n3 % 3 or tuple(eigvecs.shape) != (n_q, n3, n3) or tuple(kcart.shape) != (n_q, 3)
+                or tuple(gvec.shape) != (n_q, 3) or tuple(frac.shape) != (n_prim, 3) or tuple(coef.shape) != (n_prim,)
+                or temperatures.dim() != 1 or (u is not None and tuple(u.shape) != (n_t, n_prim, 6))
+                or tuple(out.shape) != (n_t, n_q, n3, 2)):
+            raise ChgnetB200Error(f"structure_factors: freqs must be [Q, 3n], eigvecs [{n_q}, {n3}, {n3}], kcart and "
+                                  f"gvec [{n_q}, 3], frac [{n_prim}, 3], coef [{n_prim}], temperatures [T], u None or "
+                                  f"[T, {n_prim}, 6] and out [T, {n_q}, {n3}, 2]")
+        self._call("chg_structure_factors", _p(freqs), _p(eigvecs), _p(kcart), _p(gvec), _p(frac), _p(coef), _p(u),
+                   _p(temperatures), n_t, n_q, n_prim, float(cutoff_thz), _p(out))
+
+    def broadened_spectrum(self, freqs, weights, row0, group_size, omega, sigma, out):
+        """out [T, n_groups, F] fp64 += (1 / group_size) sum over the rows of each group and their modes of
+        S+ g(omega - nu) + S- g(omega + nu), g the normalised Gaussian of standard deviation sigma (THz) cut at
+        8 sigma (``chg_broadened_spectrum``): freqs [Q, 3n] THz are the rows [row0, row0 + Q) of the map, row r in group
+        r // group_size; weights [T, Q, 3n, 2] (S+, S-) as ``structure_factors`` writes them; omega [F] THz."""
+        self._chk(freqs, weights, omega, out)
+        if any(t.dtype != torch.float64 for t in (freqs, weights, omega, out)):
+            raise ChgnetB200Error("broadened_spectrum: freqs, weights, omega and out must be float64")
+        n_q, n3 = freqs.shape
+        n_t, n_f = weights.shape[0], omega.shape[0]
+        row0, group_size = int(row0), int(group_size)
+        if (tuple(weights.shape) != (n_t, n_q, n3, 2) or omega.dim() != 1 or out.dim() != 3
+                or tuple(out.shape[::2]) != (n_t, n_f)):
+            raise ChgnetB200Error(f"broadened_spectrum: weights must be [T, {n_q}, {n3}, 2], omega [F] and out "
+                                  f"[T, n_groups, F]")
+        if n_q == 0:
+            return
+        work = torch.empty(max(1, sqw_scratch_doubles(n_q, n3, n_t, row0, group_size, n_f)), dtype=torch.float64,
+                           device=freqs.device)
+        self._call("chg_broadened_spectrum", _p(freqs), _p(weights), n_q, n3, n_t, row0, group_size, out.shape[1],
+                   _p(omega), n_f, float(sigma), _p(work), work.numel(), _p(out))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

@@ -18,6 +18,8 @@
 // displacement matrices, see below.
 // chg_joint_dos: the two-phonon joint densities of states D2 and their occupation-weighted forms N2 at target q-points,
 // by the same tetrahedron method, see below.
+// chg_structure_factors and chg_broadened_spectrum: coherent one-phonon neutron structure factors S(Q, omega) per mode
+// and their Gaussian-broadened spectra, averaged over groups of rows (powder directions), see below.
 #include <math_constants.h>
 
 #include <algorithm>
@@ -490,6 +492,151 @@ struct JointDosStore {  // work[chunk][target][slot][class][f]: scale * the sum,
 };
 
 // ---------------------------------------------------------------------------------------------------------------
+// Coherent one-phonon structure factors.  For row r (a scattering vector Q = q + G) and mode m,
+//   F_t = sum_k coef_k exp(-W_k,t) (K . e_km) exp(-2 pi i G . x_k),  W_k,t = K^T U_k,t K / 2,
+//   S+ = C (n + 1) / nu |F_t|^2,  S- = C n / nu |F_t|^2,  n = 1 / expm1(h nu / k T) (0 at T = 0),
+// and S+- = 0 for nu < cutoff; C = h / (8 pi^2 amu THz) in A^2 (phonons.DISPLACEMENT_A2_AMU_THZ), applied here.
+// One thread per (row, mode), grid y over tiles of SQW_T_TILE temperatures.  The thread walks the atoms once per tile:
+// it reads e_km (three complex128 values), forms K . e and the phase in registers and keeps one complex F per
+// temperature of its tile.  Without U (no Debye-Waller factor) F does not depend on T and one tile covers every
+// temperature.  No per-(row, atom) tensor reaches global memory.
+constexpr int SQW_THREADS = 256;
+constexpr int SQW_T_TILE = 8;
+// h / (8 pi^2 amu 1 THz) / A^2: chgnet_b200.phonons.DISPLACEMENT_A2_AMU_THZ, the same expression in the same order
+constexpr double SQW_C = 6.62607015e-34 / (8 * (3.141592653589793 * 3.141592653589793) * 1.66053906660e-27 * 1e12) /
+                         (1e-10 * 1e-10);
+
+__global__ void __launch_bounds__(SQW_THREADS)
+structure_factors_kernel(const double* __restrict__ freqs, const double2* __restrict__ eigvecs,
+                         const double* __restrict__ kcart, const double* __restrict__ gvec,
+                         const double* __restrict__ frac, const double* __restrict__ coef, const double* __restrict__ u,
+                         const double* __restrict__ temps, int n_t, int n_q, int n_prim, double cutoff,
+                         double* __restrict__ out) {
+  const int n3 = 3 * n_prim;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_q * n3) return;
+  const int row = (int)(i / n3);
+  const int t0 = u ? blockIdx.y * SQW_T_TILE : 0;
+  const int t_here = u ? min(SQW_T_TILE, n_t - t0) : n_t;
+  const double nu = __ldg(freqs + i);
+  double2* o = reinterpret_cast<double2*>(out) + (size_t)t0 * n_q * n3 + i;
+  if (!(nu >= cutoff)) {
+    for (int t = 0; t < t_here; ++t) o[(size_t)t * n_q * n3] = make_double2(0.0, 0.0);
+    return;
+  }
+  const double kx = __ldg(kcart + row * 3), ky = __ldg(kcart + row * 3 + 1), kz = __ldg(kcart + row * 3 + 2);
+  const double g0 = __ldg(gvec + row * 3), g1 = __ldg(gvec + row * 3 + 1), g2 = __ldg(gvec + row * 3 + 2);
+  // K K^T in Voigt order with the off-diagonal terms doubled: W = acc . u / 2
+  const double kk[6] = {kx * kx, ky * ky, kz * kz, 2.0 * ky * kz, 2.0 * kx * kz, 2.0 * kx * ky};
+  double fr[SQW_T_TILE], fi[SQW_T_TILE];
+#pragma unroll
+  for (int t = 0; t < SQW_T_TILE; ++t) fr[t] = fi[t] = 0.0;
+  const double2* e = eigvecs + i * n3;
+  for (int k = 0; k < n_prim; ++k) {
+    const double2 ex = __ldg(e + 3 * k), ey = __ldg(e + 3 * k + 1), ez = __ldg(e + 3 * k + 2);
+    const double dr = fma(kx, ex.x, fma(ky, ey.x, kz * ez.x)), di = fma(kx, ex.y, fma(ky, ey.y, kz * ez.y));
+    double sn, cs;  // exp(-2 pi i G . x_k) = cs - i sn
+    sincospi(2.0 * fma(g0, __ldg(frac + 3 * k), fma(g1, __ldg(frac + 3 * k + 1), g2 * __ldg(frac + 3 * k + 2))), &sn,
+             &cs);
+    const double c = __ldg(coef + k);
+    const double tr = c * fma(dr, cs, di * sn), ti = c * fma(di, cs, -dr * sn);
+    if (!u) {
+      fr[0] += tr;
+      fi[0] += ti;
+      continue;
+    }
+#pragma unroll
+    for (int t = 0; t < SQW_T_TILE; ++t) {
+      if (t >= t_here) break;
+      const double* uk = u + ((size_t)(t0 + t) * n_prim + k) * 6;
+      double w = 0.0;
+#pragma unroll
+      for (int c6 = 0; c6 < 6; ++c6) w = fma(kk[c6], __ldg(uk + c6), w);
+      const double dw = exp(-0.5 * w);
+      fr[t] = fma(dw, tr, fr[t]);
+      fi[t] = fma(dw, ti, fi[t]);
+    }
+  }
+  for (int t = 0; t < t_here; ++t) {
+    const int tf = u ? t : 0;
+    double f2 = 0.0;
+#pragma unroll
+    for (int j = 0; j < SQW_T_TILE; ++j)  // registers, not local memory: the index is a compile-time constant
+      if (j == tf) f2 = fma(fr[j], fr[j], fi[j] * fi[j]);
+    const double temp = __ldg(temps + t0 + t);
+    const double n = bose(nu, temp);
+    const double s = SQW_C * f2 / nu;
+    o[(size_t)t * n_q * n3] = make_double2(s * (n + 1.0), s * n);
+  }
+}
+
+// Broadening.  For the rows [row0, row0 + n_q) of a map whose rows form groups of group_size (row r in group
+// r / group_size), out[t][g][f] += (1 / group_size) sum over the group's rows in this call and their modes of
+//   S+ g(omega_f - nu) + S- g(omega_f + nu),  g(x) = exp(-x^2 / 2 sigma^2) / (sigma sqrt(2 pi)),  |x| <= 8 sigma.
+// One thread per frequency point; block x = chunk + n_chunks (g - g_first + n_groups_here t), one chunk of the items
+// of group g at temperature t, and block y a frequency tile.  Each tile of (row, mode) items is staged in shared memory as (nu, S+, S-) and read by every
+// thread (broadcasts).  The block's sums go to work[chunk][t][g - g_first][f], each element written by exactly one
+// thread: no atomics, and chunk_reduce_kernel adds the chunks in a fixed order.  No [row, mode, f] tensor exists.
+constexpr int SQW_BROAD_THREADS = 256;
+
+__global__ void __launch_bounds__(SQW_BROAD_THREADS)
+broadened_spectrum_kernel(const double* __restrict__ freqs, const double2* __restrict__ weights, int n_q, int n3,
+                          int n_t, int64_t row0, int group_size, int n_groups_here, const double* __restrict__ omega,
+                          int n_freq, double sigma, int n_chunks, double* __restrict__ work) {
+  __shared__ double st[SQW_BROAD_THREADS][3];
+  const int chunk = (int)(blockIdx.x % n_chunks);
+  const int gt = (int)(blockIdx.x / n_chunks);
+  const int gl = gt % n_groups_here, t = gt / n_groups_here;
+  const int f = blockIdx.y * blockDim.x + threadIdx.x;
+  const bool active = f < n_freq;
+  const double w = active ? omega[f] : 0.0;
+  // the rows of group g_first + gl inside this call, relative to row0
+  const int64_t g = row0 / group_size + gl;
+  const int r_begin = (int)(max(g * group_size, row0) - row0);
+  const int r_end = (int)(min((g + 1) * group_size, row0 + n_q) - row0);
+  const int64_t n_items = (int64_t)(r_end - r_begin) * n3;
+  const double2* wt = weights + (size_t)t * n_q * n3 + (size_t)r_begin * n3;
+  const double* nu_g = freqs + (size_t)r_begin * n3;
+  const double inv2s2 = 0.5 / (sigma * sigma), reach = 8.0 * sigma;
+  const double norm = 1.0 / (sigma * 2.5066282746310002);  // sqrt(2 pi)
+  double acc = 0.0;
+  const int64_t tile = blockDim.x;
+  const int64_t n_tiles = (n_items + tile - 1) / tile;
+  const int64_t t_end = n_tiles * (chunk + 1) / n_chunks;
+  for (int64_t tt = n_tiles * chunk / n_chunks; tt < t_end; ++tt) {
+    const int64_t p = tt * tile + threadIdx.x;
+    __syncthreads();  // the previous tile has been read
+    if (p < n_items) {
+      const double2 s = __ldg(wt + p);
+      st[threadIdx.x][0] = __ldg(nu_g + p), st[threadIdx.x][1] = s.x, st[threadIdx.x][2] = s.y;
+    }
+    __syncthreads();
+    if (!active) continue;
+    const int n_here = (int)min(tile, n_items - tt * tile);
+    for (int j = 0; j < n_here; ++j) {
+      const double nu = st[j][0];
+      const double xp = w - nu, xm = w + nu;
+      if (fabs(xp) <= reach) acc = fma(st[j][1], exp(-xp * xp * inv2s2), acc);
+      if (fabs(xm) <= reach) acc = fma(st[j][2], exp(-xm * xm * inv2s2), acc);
+    }
+  }
+  if (!active) return;
+  work[(((size_t)chunk * n_t + t) * n_groups_here + gl) * n_freq + f] = acc * norm;
+}
+
+struct SpectrumStore {  // work[chunk][t][g - g_first][f]: out[t][g][f] += scale * the sum
+  double* out;
+  int n_freq, n_groups_here;
+  int64_t g_first, n_groups;
+  double scale;
+  __device__ void operator()(int64_t o, double s) const {
+    const int64_t f = o % n_freq, r = o / n_freq;
+    const int64_t gl = r % n_groups_here, t = r / n_groups_here;
+    out[(t * n_groups + g_first + gl) * n_freq + f] += s * scale;
+  }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
 // The chunk reduction of the three kernels above: store(o, sum over chunks c, in chunk order, of work[c * n_out + o])
 template <class Store>
 __global__ void chunk_reduce_kernel(const double* __restrict__ work, int n_chunks, int64_t n_out, Store store) {
@@ -615,6 +762,59 @@ extern "C" int chg_joint_dos(const double* freqs, int32_t n_band, int32_t n1, in
       n_items, work);
   const double scale = 1.0 / (6.0 * (double)n1 * n2 * n3);
   CHG_CUDA(reduce_chunks(work, chunks, (int64_t)n_target * n_slots * 2 * n_freq, JointDosStore{out, n_freq, scale},
+                         as_stream(stream)));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_structure_factors(const double* freqs, const double* eigvecs, const double* kcart,
+                                     const double* gvec, const double* frac, const double* coef, const double* u,
+                                     const double* temperatures, int32_t n_t, int32_t n_q, int32_t n_prim,
+                                     double cutoff_thz, double* out, void* stream) {
+  CHG_CHECK_ARG(n_t >= 0 && n_q >= 0 && n_prim >= 0, "negative size");
+  if (n_t == 0 || n_q == 0 || n_prim == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && eigvecs && kcart && gvec && frac && coef && temperatures && out, "null pointer");
+  const int64_t n_items = (int64_t)n_q * 3 * n_prim;
+  const int64_t blocks = (n_items + SQW_THREADS - 1) / SQW_THREADS;
+  const int64_t t_tiles = u ? ((int64_t)n_t + SQW_T_TILE - 1) / SQW_T_TILE : 1;
+  CHG_CHECK_ARG(blocks < (1ll << 31) && t_tiles <= 65535, "too many rows or temperatures in one call");
+  structure_factors_kernel<<<dim3((unsigned)blocks, (unsigned)t_tiles), SQW_THREADS, 0, as_stream(stream)>>>(
+      freqs, reinterpret_cast<const double2*>(eigvecs), kcart, gvec, frac, coef, u, temperatures, n_t, n_q, n_prim,
+      cutoff_thz, out);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_broadened_spectrum(const double* freqs, const double* weights, int32_t n_q, int32_t n_modes,
+                                      int32_t n_t, int64_t row0, int32_t group_size, int64_t n_groups,
+                                      const double* omega, int32_t n_freq, double sigma, double* work,
+                                      int64_t work_doubles, double* out, void* stream) {
+  CHG_CHECK_ARG(n_q >= 0 && n_modes >= 0 && n_t >= 0 && n_freq >= 0 && row0 >= 0 && group_size > 0, "bad size");
+  if (n_q == 0 || n_modes == 0 || n_t == 0 || n_freq == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && weights && omega && work && out, "null pointer");
+  CHG_CHECK_ARG(sigma > 0.0, "sigma must be positive");
+  const int64_t g_first = row0 / group_size, g_last = (row0 + n_q - 1) / group_size;
+  CHG_CHECK_ARG(g_last < n_groups, "rows beyond the last group");
+  const int n_groups_here = (int)(g_last - g_first + 1);
+  const int threads = (int)std::min<int64_t>(SQW_BROAD_THREADS, ((int64_t)n_freq + 31) / 32 * 32);
+  const int64_t f_blocks = ((int64_t)n_freq + threads - 1) / threads;
+  CHG_CHECK_ARG(f_blocks <= 65535, "too many frequency points in one call");
+  // scratch of one chunk: every (t, group, f) of the call
+  const int64_t per_chunk = (int64_t)n_t * n_groups_here * n_freq;
+  CHG_CHECK_ARG(work_doubles >= per_chunk, "work holds less than one chunk (n_t x groups in the call x n_freq)");
+  // enough chunks for about 4 096 blocks in all, at most CHG_SQW_MAX_CHUNKS, one tile of the largest group each, and
+  // no more than work holds
+  const int64_t most = (int64_t)std::min(group_size, n_q) * n_modes;
+  const int64_t n_tiles = (most + threads - 1) / threads;
+  const int64_t others = f_blocks * n_groups_here * n_t;
+  const int64_t want = (4096 + others - 1) / others;
+  const int chunks = (int)std::max<int64_t>(
+      1, std::min<int64_t>({(int64_t)CHG_SQW_MAX_CHUNKS, n_tiles, want, work_doubles / per_chunk}));
+  const int64_t x_blocks = (int64_t)chunks * n_groups_here * n_t;
+  CHG_CHECK_ARG(x_blocks < (1ll << 31), "too many groups or temperatures in one call");
+  broadened_spectrum_kernel<<<dim3((unsigned)x_blocks, (unsigned)f_blocks), threads, 0, as_stream(stream)>>>(
+      freqs, reinterpret_cast<const double2*>(weights), n_q, n_modes, n_t, row0, group_size, n_groups_here, omega,
+      n_freq, sigma, chunks, work);
+  CHG_CUDA(reduce_chunks(work, chunks, (int64_t)n_t * n_groups_here * n_freq,
+                         SpectrumStore{out, n_freq, n_groups_here, g_first, n_groups, 1.0 / group_size},
                          as_stream(stream)));
   CHG_LAUNCH_END();
 }

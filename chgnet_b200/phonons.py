@@ -12,11 +12,14 @@
   atoms (``chg_tetrahedron_dos``); anisotropic thermal displacement matrices U(T) on a mesh
   (``chg_thermal_displacements``), Cartesian and in the CIF convention (``cif_displacement_matrices``); two-phonon
   joint densities of states and their occupation-weighted forms at mesh q-points, and per mode as the three-phonon
-  phase space (``chg_joint_dos``).
+  phase space (``chg_joint_dos``); coherent one-phonon neutron structure factors S(Q, omega) per mode at scattering
+  vectors and their broadened spectra, per Q (``dynamic_structure_factor``) and averaged over directions for powders
+  (``powder_spectrum``), with ``chg_structure_factors`` and ``chg_broadened_spectrum``.
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
-primitive cell for densities of states, A^2 for thermal displacement matrices, 1/THz for joint densities of states.
+primitive cell for densities of states, A^2 for thermal displacement matrices, 1/THz for joint densities of states,
+b^2 per primitive cell for structure factors (b the caller's scattering lengths) and b^2/THz for their spectra.
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from chgnet_b200._lib import JDOS_MAX_CHUNKS
+from chgnet_b200._lib import JDOS_MAX_CHUNKS, sqw_scratch_doubles
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -271,6 +274,36 @@ def _zero_gamma_acoustic(nu: torch.Tensor) -> None:
     nu[0, torch.argsort(nu[0].abs(), stable=True)[:3]] = 0.0
 
 
+def _zero_gamma_rows(nu: torch.Tensor, q: np.ndarray) -> None:
+    """Sets the three modes of smallest |nu| to 0, in place, in every row of ``nu`` whose reduced wave vector ``q``
+    (the same rows, [Q, 3]) is Gamma: every component within 1e-9 of an integer."""
+    rows = np.nonzero(np.all(np.abs(q - np.round(q)) <= 1e-9, axis=1))[0]
+    if len(rows):
+        r = torch.as_tensor(rows).to(nu.device)
+        nu[r[:, None], torch.argsort(nu[r].abs(), dim=1, stable=True)[:, :3]] = 0.0
+
+
+def _gaussian_sigma(width) -> float | None:
+    """The standard deviation (THz) of a Gaussian of FWHM ``width``, width / (2 sqrt(2 ln 2)); None for None, and
+    ValueError unless it is finite and > 0."""
+    if width is None:
+        return None
+    w = float(width)
+    if not (np.isfinite(w) and w > 0):
+        raise ValueError(f"width must be finite and positive, got {width!r}")
+    return w / (2.0 * math.sqrt(2.0 * math.log(2.0)))
+
+
+def fibonacci_directions(n: int) -> np.ndarray:
+    """[n, 3] unit vectors of a Fibonacci sphere: d_i = (r cos phi_i, r sin phi_i, z_i), z_i = 1 - (2 i + 1) / n,
+    r = sqrt(1 - z_i^2), phi_i = i pi (3 - sqrt 5)."""
+    i = np.arange(n, dtype=np.float64)
+    z = 1.0 - (2.0 * i + 1.0) / n
+    r = np.sqrt(1.0 - z * z)
+    phi = i * (math.pi * (3.0 - math.sqrt(5.0)))
+    return np.stack([r * np.cos(phi), r * np.sin(phi), z], axis=1)
+
+
 class Phonons:
     """Harmonic phonons of a crystal from its compact supercell force constants (``CHGNet.phonons``).
 
@@ -290,6 +323,9 @@ class Phonons:
     eigh_batch = 4096
     # joint_dos and phase_space: targets per chg_joint_dos call keep its output and scratch below this many bytes
     jdos_chunk_bytes = 1 << 28
+    # dynamic_structure_factor and powder_spectrum: rows per chg_broadened_spectrum call keep its scratch below this
+    # many bytes (or at one group of rows, when a group alone needs more)
+    sqw_chunk_bytes = 1 << 28
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -583,4 +619,172 @@ class Phonons:
             res["temperatures"] = temps
             res["weighted_jdos"] = out[1:].cpu().numpy()
             res["average_weighted_jdos"] = avg[1:].cpu().numpy()
+        return res
+
+    def _scattering_coefficients(self, scattering_lengths) -> np.ndarray:
+        """[n_prim] b_k / sqrt(m_k) from the mapping {atomic number: coherent scattering length}; ValueError if a
+        species of the primitive cell is missing or its length is not finite."""
+        coef = np.empty(len(self.p2s))
+        for k, z in enumerate(self.cell.prim_z):
+            b = scattering_lengths.get(int(z)) if hasattr(scattering_lengths, "get") else None
+            if b is None or not np.isfinite(float(b)):
+                raise ValueError(f"scattering_lengths needs a finite coherent scattering length for atomic number "
+                                 f"{int(z)}, got {b!r}")
+            coef[k] = float(b) / math.sqrt(self.masses[k])
+        return coef
+
+    def _debye_waller(self, debye_waller_mesh, temps):
+        """U [T, n_prim, 6] (Voigt, A^2) on the device from ``thermal_displacement_matrices`` on ``debye_waller_mesh``
+        and that call's ``n_imaginary``, or (None, None) for no Debye-Waller factor."""
+        if debye_waller_mesh is None:
+            return None, None
+        td = self.thermal_displacement_matrices(debye_waller_mesh, temps)
+        u = td["cartesian"][..., [0, 1, 2, 1, 0, 0], [0, 1, 2, 2, 2, 1]]
+        return torch.as_tensor(np.ascontiguousarray(u)).to(self.device), td["n_imaginary"]
+
+    def _structure_factor_chunks(self, q_red, g, u, t, coef):
+        """Yields ``(slice, nu, weights, n_imaginary)`` per eigh chunk of the rows (scattering vectors Q = q_red + g):
+        the frequencies at q_red (THz, the three modes of smallest |nu| set to 0 where q_red is Gamma), the
+        ``chg_structure_factors`` output [T, rows, 3n, 2] and the chunk's modes below -``THERMAL_CUTOFF_THZ`` (counted
+        before the Gamma rule), all on the device.  ``g`` [Q, 3] is any integer vector: |F| does not depend on it."""
+        dev = self.device
+        n3 = 3 * len(self.p2s)
+        q_red = np.ascontiguousarray(q_red, dtype=np.float64)
+        g = np.ascontiguousarray(g, dtype=np.float64)
+        kcart = 2 * math.pi * (q_red + g) @ np.linalg.inv(self.cell.prim_lattice).T
+        frac = torch.as_tensor(np.ascontiguousarray(self.cell.prim_frac, dtype=np.float64)).to(dev)
+        coef = torch.as_tensor(coef).to(dev)
+        for s, nu, e in self._eigh_chunks(q_red, eigenvectors=True, eigh_batch=self.eigh_batch):
+            n_imaginary = (nu < -THERMAL_CUTOFF_THZ).sum()
+            _zero_gamma_rows(nu, q_red[s])
+            out = torch.empty(len(t), nu.shape[0], n3, 2, dtype=torch.float64, device=dev)
+            # eigh returns column-major matrices: e.mT is the mode-major layout of the kernel, without a copy
+            self.kernels.structure_factors(nu, e.mT.contiguous(), torch.as_tensor(kcart[s]).to(dev),
+                                           torch.as_tensor(g[s]).to(dev), frac, coef, u, t, THERMAL_CUTOFF_THZ, out)
+            yield s, nu, out, n_imaginary
+
+    def _broaden(self, nu, w, row0, group_size, omega, sigma, out) -> None:
+        """``chg_broadened_spectrum`` of the rows [row0, row0 + len(nu)) of nu [R, 3n] and w [T, R, 3n, 2] into out
+        [T, n_groups, F], in calls of as many rows as keep the call's scratch (``sqw_scratch_doubles``) within
+        ``sqw_chunk_bytes``: whole groups where two fit (a call may straddle one group more than it holds), else a
+        part of a group, at least one row (whose scratch, one [T, F] map, is the least a call can have)."""
+        n_rows, n3 = nu.shape
+        n_t, n_f = w.shape[0], omega.shape[0]
+        per_group = 8 * sqw_scratch_doubles(min(group_size, n_rows), n3, n_t, 0, group_size, n_f)
+        n_fit = self.sqw_chunk_bytes // per_group
+        if n_fit >= 2:
+            rows = (n_fit - 1) * group_size
+        else:  # r < group_size rows over two groups take ceil(r 3n / 32) chunks of 2 T F doubles
+            rows = max(1, min(group_size, self.sqw_chunk_bytes // (16 * n_t * n_f) * 32 // n3))
+        for a in range(0, n_rows, rows):
+            b = min(a + rows, n_rows)
+            self.kernels.broadened_spectrum(nu[a:b], w[:, a:b].contiguous(), row0 + a, group_size, omega, sigma, out)
+
+    def dynamic_structure_factor(self, qpoints, temperatures, scattering_lengths, *, debye_waller_mesh=None,
+                                 frequency_points=None, width=None) -> dict:
+        """Coherent one-phonon neutron scattering S(Q, omega) per mode at the scattering vectors ``qpoints`` ([Q, 3]
+        or [3], reduced in the primitive reciprocal basis; the result drops the Q axis for one [3] vector):
+
+            F_nu(Q, T) = sum_k b_k m_k^-1/2 exp(-W_k) (K . e_k,nu(q)) exp(-2 pi i G . x_k),  W_k = K^T U_k(T) K / 2
+            S+_nu = C (n + 1) / nu |F_nu|^2  (energy loss, omega = +nu),  S-_nu = C n / nu |F_nu|^2  (gain, -nu)
+
+        with K = 2 pi Q inv(prim_lattice)^T the Cartesian scattering vector (1/A, 2 pi included), G = floor(Q + 1/2),
+        q = Q - G, e_k,nu(q) atom k's block of the eigenvector of ``frequencies`` (phonopy's phase convention), x_k
+        the fractional positions, m_k in amu, n = 1 / expm1(h nu / k T) (0 at T = 0) and C = h / (8 pi^2 amu THz)
+        (``DISPLACEMENT_A2_AMU_THZ``).  The phase exp(-2 pi i G . x_k) makes |F| independent of the G that reduces Q.
+        ``scattering_lengths`` maps every atomic number of the primitive cell to its coherent scattering length b
+        (finite, else ValueError); S is in units of b^2 per primitive cell, e.g. fm^2 for b in fm (fcc Cu:
+        ``{29: 7.718}``).  U_k(T) is ``thermal_displacement_matrices(debye_waller_mesh, temperatures)``, or W = 0
+        without ``debye_waller_mesh``.  Modes with nu < ``THERMAL_CUTOFF_THZ`` get S = 0, and where q is Gamma so do
+        the three modes of smallest |nu| (the Bragg peak is elastic).
+
+        Returns ``qpoints`` (q = Q - G), ``frequencies`` [Q, 3n] (THz, with those Gamma modes set to 0), ``stokes``
+        (S+) and ``anti_stokes`` (S-) [T, Q, 3n], ``temperatures`` and ``n_imaginary`` (the modes below
+        -``THERMAL_CUTOFF_THZ`` over the Q evaluated); with ``debye_waller_mesh`` also ``debye_waller_n_imaginary``;
+        with ``frequency_points`` (THz, may be negative; needs ``width``) also ``spectrum`` [T, Q, F]
+        = sum_nu [S+ g(omega - nu) + S- g(omega + nu)] in b^2/THz per primitive cell, g the normalised Gaussian of
+        FWHM ``width`` (THz) cut at 8 sigma.  Non-finite Q, bad temperatures, width <= 0 and missing species raise
+        ValueError.  D(q), the eigenvectors and the structure factors (``chg_structure_factors``, then
+        ``chg_broadened_spectrum``) stay on the device in chunks of at most ``eigh_batch`` q."""
+        big_q = np.asarray(qpoints, dtype=np.float64)
+        single = big_q.ndim == 1
+        big_q = big_q.reshape(-1, 3)
+        if not np.all(np.isfinite(big_q)):
+            raise ValueError(f"qpoints must be finite, got {big_q.tolist()}")
+        temps = _temperatures(temperatures)
+        if frequency_points is not None and width is None:
+            raise ValueError("frequency_points needs a width (THz)")
+        sigma = _gaussian_sigma(width)
+        coef = self._scattering_coefficients(scattering_lengths)
+        u, dw_imag = self._debye_waller(debye_waller_mesh, temps)
+        g = np.floor(big_q + 0.5)
+        q = big_q - g
+        dev, n3 = self.device, 3 * len(self.p2s)
+        t = torch.as_tensor(temps).to(dev)
+        nu_all = torch.empty(len(q), n3, dtype=torch.float64, device=dev)
+        sqw = torch.empty(len(temps), len(q), n3, 2, dtype=torch.float64, device=dev)
+        spec = omega = None
+        if frequency_points is not None:
+            omega = torch.as_tensor(np.asarray(frequency_points, dtype=np.float64).reshape(-1)).to(dev)
+            spec = torch.zeros(len(temps), len(q), len(omega), dtype=torch.float64, device=dev)
+        n_imaginary = torch.zeros((), dtype=torch.int64, device=dev)
+        for s, nu, w, n_im in self._structure_factor_chunks(q, g, u, t, coef):
+            n_imaginary += n_im
+            nu_all[s], sqw[:, s] = nu, w
+            if spec is not None:
+                self._broaden(nu, w, s.start, 1, omega, sigma, spec)
+        res = {"qpoints": q, "frequencies": nu_all.cpu().numpy(), "stokes": sqw[..., 0].cpu().numpy(),
+               "anti_stokes": sqw[..., 1].cpu().numpy(), "temperatures": temps, "n_imaginary": int(n_imaginary)}
+        if dw_imag is not None:
+            res["debye_waller_n_imaginary"] = dw_imag
+        if spec is not None:
+            res["frequency_points"] = omega.cpu().numpy()
+            res["spectrum"] = spec.cpu().numpy()
+        if single:
+            res["qpoints"], res["frequencies"] = res["qpoints"][0], res["frequencies"][0]
+            for key in ("stokes", "anti_stokes", "spectrum"):
+                if key in res:
+                    res[key] = res[key][:, 0]
+        return res
+
+    def powder_spectrum(self, q_magnitudes, frequency_points, temperatures, scattering_lengths, *, width,
+                        n_directions=500, debye_waller_mesh=None) -> dict:
+        """Powder-averaged coherent one-phonon spectrum S(|Q|, omega) in b^2/THz per primitive cell: the spectrum of
+        ``dynamic_structure_factor`` averaged over the ``n_directions`` unit vectors d_i of ``fibonacci_directions``
+        (a plain mean), K = |Q| d_i in the Cartesian frame of the lattice as given, Q = K prim_lattice^T / 2 pi.
+
+        ``q_magnitudes`` [M] in 1/A (2 pi included; finite and >= 0), ``frequency_points`` [F] in THz (may be
+        negative), ``width`` the FWHM of the Gaussian (THz, > 0), ``n_directions`` >= 1; the other arguments as in
+        ``dynamic_structure_factor``, and the same errors.  Returns ``q_magnitudes``, ``frequency_points``,
+        ``temperatures``, ``spectrum`` [T, M, F] and ``n_imaginary`` (over all M n_directions vectors); with
+        ``debye_waller_mesh`` also ``debye_waller_n_imaginary``.  The M n_directions rows run as contiguous groups of
+        ``n_directions`` through the eigh chunks; frequencies, eigenvectors and weights stay on the device, and
+        ``chg_broadened_spectrum`` adds each chunk's rows to their shells, so only [T, M, F] is copied back."""
+        qm = np.asarray(q_magnitudes, dtype=np.float64).reshape(-1)
+        if not np.all(np.isfinite(qm)) or np.any(qm < 0):
+            raise ValueError(f"q_magnitudes must be finite and non-negative, got {qm.tolist()}")
+        n_dir = int(n_directions)
+        if n_dir != n_directions or n_dir < 1:
+            raise ValueError(f"n_directions must be a positive integer, got {n_directions!r}")
+        temps = _temperatures(temperatures)
+        if width is None:
+            raise ValueError("powder_spectrum needs a width (THz)")
+        sigma = _gaussian_sigma(width)
+        coef = self._scattering_coefficients(scattering_lengths)
+        u, dw_imag = self._debye_waller(debye_waller_mesh, temps)
+        kcart = (qm[:, None, None] * fibonacci_directions(n_dir)[None]).reshape(-1, 3)
+        big_q = kcart @ np.asarray(self.cell.prim_lattice, dtype=np.float64).T / (2 * math.pi)
+        g = np.floor(big_q + 0.5)
+        dev = self.device
+        t = torch.as_tensor(temps).to(dev)
+        omega = torch.as_tensor(np.asarray(frequency_points, dtype=np.float64).reshape(-1)).to(dev)
+        spec = torch.zeros(len(temps), len(qm), len(omega), dtype=torch.float64, device=dev)
+        n_imaginary = torch.zeros((), dtype=torch.int64, device=dev)
+        for s, nu, w, n_im in self._structure_factor_chunks(big_q - g, g, u, t, coef):
+            n_imaginary += n_im
+            self._broaden(nu, w, s.start, n_dir, omega, sigma, spec)
+        res = {"q_magnitudes": qm, "frequency_points": omega.cpu().numpy(), "temperatures": temps,
+               "spectrum": spec.cpu().numpy(), "n_imaginary": int(n_imaginary)}
+        if dw_imag is not None:
+            res["debye_waller_n_imaginary"] = dw_imag
         return res

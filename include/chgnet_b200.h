@@ -603,6 +603,29 @@ int chg_thermal_displacements(const double* freqs, const double* eigvecs, int32_
 int chg_joint_dos(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3, const int32_t* tetrahedra,
                   const int32_t* targets, int32_t n_target, const double* omega, int32_t n_freq,
                   const double* temperatures, int32_t n_t, double cutoff_thz, double* out, double* work, void* stream);
+/* Coherent one-phonon structure factors: out [n_t][n_q][3 n_prim][2] = (S+, S-) per row (scattering vector) and mode,
+ *   F = sum_k coef[k] exp(-W_k) (K . e_k) exp(-2 pi i G . x_k),  W_k = K^T U_k K / 2,
+ *   S+ = C (n + 1) / nu |F|^2,  S- = C n / nu |F|^2,  n = 1 / expm1(h nu / k_B T) (0 at T = 0),
+ * S+- = 0 for nu < cutoff_thz; C = h / (8 pi^2 amu THz) = 0.5053790 A^2 is applied in the kernel.  freqs [n_q][3 n_prim]
+ * fp64 THz (signed); eigvecs [n_q][mode][3 n_prim] interleaved complex128, mode-major (as chg_thermal_displacements);
+ * kcart [n_q][3] Cartesian K (1/A, 2 pi included); gvec [n_q][3] the reciprocal-lattice vector G (reduced); frac
+ * [n_prim][3] fractional positions; coef [n_prim] = b_k / sqrt(m_k); u [n_t][n_prim][6] U in Voigt order (xx, yy, zz,
+ * yz, xz, xy; A^2) or NULL for W = 0; temperatures [n_t] K (fp64).  No atomics.                                      */
+int chg_structure_factors(const double* freqs, const double* eigvecs, const double* kcart, const double* gvec,
+                          const double* frac, const double* coef, const double* u, const double* temperatures,
+                          int32_t n_t, int32_t n_q, int32_t n_prim, double cutoff_thz, double* out, void* stream);
+/* Gaussian broadening of structure factors: for the rows [row0, row0 + n_q) of a map of n_groups groups of group_size
+ * rows (row r in group r / group_size), out [n_t][n_groups][n_freq] +=
+ *   (1 / group_size) sum over the group's rows in this call and their modes of S+ g(omega - nu) + S- g(omega + nu),
+ * g(x) = exp(-x^2 / 2 sigma^2) / (sigma sqrt(2 pi)), terms with |x| > 8 sigma dropped.  freqs [n_q][n_modes] fp64 THz;
+ * weights [n_t][n_q][n_modes][2] (S+, S-) as chg_structure_factors writes them; omega [n_freq] THz.  work: scratch
+ * of work_doubles doubles, at least one chunk of n_t * (groups the call touches) * n_freq; the call uses at most
+ * CHG_SQW_MAX_CHUNKS chunks, and no more than work holds.  Deterministic for given arguments: two kernels, per-block
+ * partial sums added in a fixed order, no atomics.                                                                  */
+#define CHG_SQW_MAX_CHUNKS 64
+int chg_broadened_spectrum(const double* freqs, const double* weights, int32_t n_q, int32_t n_modes, int32_t n_t,
+                           int64_t row0, int32_t group_size, int64_t n_groups, const double* omega, int32_t n_freq,
+                           double sigma, double* work, int64_t work_doubles, double* out, void* stream);
 
 #ifdef __cplusplus
 }
