@@ -74,6 +74,8 @@ SIGNATURES: dict[str, list] = {
     "chg_joint_dos": [P, I, I, I, I, P, P, I, P, I, P, I, D, P, P, P],
     "chg_structure_factors": [P, P, P, P, P, P, P, P, I, I, I, D, P, P],
     "chg_broadened_spectrum": [P, P, I, I, I, I64, I, I64, P, I, D, P, I64, P, P],
+    "chg_phonon_interaction": [P, P, P, P, P, P, I, I, I, I, I, P, P, I, P, I, D, P, I64, P, P],
+    "chg_imag_self_energy": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -95,6 +97,23 @@ def sqw_scratch_doubles(n_rows, n_modes, n_t, row0, group_size, n_freq):
     groups = (row0 + n_rows - 1) // group_size - row0 // group_size + 1
     chunks = max(1, min(SQW_MAX_CHUNKS, -(-min(group_size, n_rows) * n_modes // 32)))
     return chunks * n_t * groups * n_freq
+
+
+# CHG_ISE_MAX_CHUNKS: the most chunks chg_imag_self_energy's partial sums use (tests/test_three_phonon_spec.py ties it
+# to the header)
+ISE_MAX_CHUNKS = 64
+
+
+def ph3_scratch_doubles(n_q1, n_prim, n_super):
+    """The scratch of one ``chg_phonon_interaction`` call: the image averages of q1 and q2, 2 n_q1 n_prim n_super
+    complex, and two [n_q1, 3n, 3n, 3n] complex buffers."""
+    return 4 * n_q1 * (n_prim * n_super + (3 * n_prim) ** 3)
+
+
+def ise_scratch_doubles(n_q1, n_band, n_t):
+    """The scratch of one ``chg_imag_self_energy`` call: the tetrahedron weights [n_q1, n_band^3, 2] and
+    ``ISE_MAX_CHUNKS`` chunks of [n_t, n_band] partial sums."""
+    return 2 * n_q1 * n_band**3 + ISE_MAX_CHUNKS * n_t * n_band
 
 _lib = None
 
@@ -534,6 +553,53 @@ class CudaKernels:
                            device=freqs.device)
         self._call("chg_broadened_spectrum", _p(freqs), _p(weights), n_q, n3, n_t, row0, group_size, out.shape[1],
                    _p(omega), n_f, float(sigma), _p(work), work.numel(), _p(out))
+
+    def phonon_interaction(self, fc3, img_ptr, img_vec, s2p, inv_sqrt_m, frac, mesh, freqs, eigvecs, target, q1,
+                           cutoff_thz, out):
+        """out [n_q1, 3n, 3n, 3n] fp64 (overwritten) = the interaction strengths P (eV^2) of the target q (mesh index)
+        with the q1 of the mesh indices ``q1`` [n_q1] int32 and q2 = q - q1 (``chg_phonon_interaction``): fc3 [n, N, N,
+        3, 3, 3] eV/A^3, img_ptr, img_vec, s2p and inv_sqrt_m as ``dynamical_matrices`` (the supercell atom-major),
+        frac [n, 3] fractional positions, freqs [n1 n2 n3, 3n] THz and eigvecs [n1 n2 n3, mode, 3n] complex128 (mode-
+        major) of the full Gamma-centred ``mesh``; modes below cutoff_thz give 0."""
+        self._chk(fc3, img_ptr, img_vec, s2p, inv_sqrt_m, frac, freqs, eigvecs, q1, out)
+        f64 = torch.float64
+        if (any(t.dtype != f64 for t in (fc3, img_vec, inv_sqrt_m, frac, freqs, out))
+                or eigvecs.dtype != torch.complex128 or q1.dtype != torch.int32 or s2p.dtype != torch.int32):
+            raise ChgnetB200Error("phonon_interaction: eigvecs must be complex128, q1 and s2p int32 and every other "
+                                  "tensor float64")
+        n1, n2, n3 = (int(n) for n in mesh)
+        n_prim, n_super = fc3.shape[0], fc3.shape[1]
+        nb, n_q1 = 3 * n_prim, q1.shape[0]
+        if (tuple(fc3.shape) != (n_prim, n_super, n_super, 3, 3, 3) or tuple(frac.shape) != (n_prim, 3)
+                or tuple(freqs.shape) != (n1 * n2 * n3, nb) or tuple(eigvecs.shape) != (n1 * n2 * n3, nb, nb)
+                or q1.dim() != 1 or tuple(out.shape) != (n_q1, nb, nb, nb)):
+            raise ChgnetB200Error(f"phonon_interaction: fc3 must be [n, N, N, 3, 3, 3], frac [{n_prim}, 3], freqs "
+                                  f"[{n1 * n2 * n3}, {nb}], eigvecs [{n1 * n2 * n3}, {nb}, {nb}], q1 [Q1] and out "
+                                  f"[Q1, {nb}, {nb}, {nb}]")
+        if n_prim and (n_super % n_prim or not torch.equal(
+                s2p, torch.arange(n_super, device=s2p.device, dtype=torch.int32) // (n_super // n_prim))):
+            raise ChgnetB200Error("phonon_interaction: the supercell must be atom-major (s2p[j] = j // n_cells)")
+        work = torch.empty(max(1, ph3_scratch_doubles(n_q1, n_prim, n_super)), dtype=f64, device=freqs.device)
+        self._call("chg_phonon_interaction", _p(fc3), _p(img_ptr), _p(img_vec), _p(s2p), _p(inv_sqrt_m), _p(frac),
+                   n_prim, n_super, n1, n2, n3, _p(freqs), _p(eigvecs), int(target), _p(q1), n_q1, float(cutoff_thz),
+                   _p(work), work.numel(), _p(out))
+
+    def imag_self_energy(self, freqs, mesh, tetrahedra, target, omega, q1, p, temperatures, cutoff_thz, gamma):
+        """gamma [T, n_band] fp64 += the contribution of the q1 (mesh indices ``q1`` [n_q1] int32) to the imaginary
+        self-energy (half width, THz) of the target's modes at w = omega [n_band] (``chg_imag_self_energy``): freqs
+        [n1 n2 n3, n_band] THz, tetrahedra [6, 4, 3] int32, p [n_q1, n_band, n_band, n_band] the interaction strengths
+        of ``phonon_interaction``, temperatures [T] K; modes below cutoff_thz left out."""
+        self._chk(freqs, tetrahedra, omega, q1, p, temperatures, gamma)
+        n1, n2, n3 = _mesh_args("imag_self_energy", mesh, freqs, tetrahedra, "freqs, omega, p, temperatures and gamma",
+                                (freqs, omega, p, temperatures, gamma))
+        nb, n_q1, n_t = freqs.shape[1], q1.shape[0], temperatures.shape[0]
+        if (q1.dtype != torch.int32 or q1.dim() != 1 or tuple(omega.shape) != (nb,) or temperatures.dim() != 1
+                or tuple(p.shape) != (n_q1, nb, nb, nb) or tuple(gamma.shape) != (n_t, nb)):
+            raise ChgnetB200Error(f"imag_self_energy: q1 must be int32 [Q1], omega [{nb}], p [Q1, {nb}, {nb}, {nb}], "
+                                  f"temperatures [T] and gamma [T, {nb}]")
+        work = torch.empty(max(1, ise_scratch_doubles(n_q1, nb, n_t)), dtype=torch.float64, device=freqs.device)
+        self._call("chg_imag_self_energy", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), _p(q1),
+                   n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(gamma))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

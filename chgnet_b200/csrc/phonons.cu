@@ -657,6 +657,377 @@ cudaError_t reduce_chunks(const double* work, int n_chunks, int64_t n_out, Store
   return cudaSuccess;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Three-phonon interaction strengths.  For a target q (mesh index) and a q1 of the mesh, q2 = q - q1 on the mesh and
+// G = q - q1 - q2 (integer, each component 0 or -1):
+//   R[k a][k' b][k'' c] = e^{-2 pi i G.x_k} / sqrt(m_k m_k' m_k'') sum_{j' in k', j'' in k''} Phi3[k][j'][j''][a][b][c]
+//                         rho_kj'(q1) rho_kj''(q2),   rho_kj(q) = (1/m_kj) sum_images e^{2 pi i q.v}
+//   P[l][l1][l2] = C^3 / (36 N nu nu1 nu2) |sum e*_l(q) e_l1(q1) e_l2(q2) R|^2,   C = h / (8 pi^2 amu THz) (SQW_C),
+// P = 0 when any of the three frequencies is below the cutoff.  Five stages per call, every one over all the q1 of the
+// call: rho_kernel (the image averages, with the phase and the masses folded in), fc3_fourier_kernel (R, each thread one
+// entry for PH3_Q1_TILE q1, so each Phi3 load serves them all), then three complex GEMMs (contract_kernel) that contract
+// the modes of q, q1 and q2 in turn; the last one writes P.  Scratch: rho, and two [n_q1][3n]^3 complex buffers that R,
+// the first and the second contraction take in turn.  No atomics; everything is fp64.
+constexpr int PH3_THREADS = 128;
+constexpr int PH3_Q1_TILE = 4;
+constexpr int PH3_TILE = 32;   // GEMM output tile (both dimensions)
+constexpr int PH3_KTILE = 16;  // GEMM reduction tile
+
+struct MeshTriplet {  // q1 and q2 = target - q1 of the mesh, and G = target - q1 - q2
+  int q1, q2;
+  double g0, g1, g2;
+  double r1[3], r2[3];  // reduced q1, q2
+};
+
+__device__ __forceinline__ MeshTriplet mesh_triplet(int target, int q1, int n1, int n2, int n3) {
+  const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
+  const int a = q1 / (n2 * n3), b = (q1 / n3) % n2, c = q1 % n3;
+  int a2 = ta - a, b2 = tb - b, c2 = tc - c;
+  MeshTriplet m;
+  m.g0 = a2 < 0 ? -1.0 : 0.0, m.g1 = b2 < 0 ? -1.0 : 0.0, m.g2 = c2 < 0 ? -1.0 : 0.0;
+  a2 += a2 < 0 ? n1 : 0;
+  b2 += b2 < 0 ? n2 : 0;
+  c2 += c2 < 0 ? n3 : 0;
+  m.q1 = q1, m.q2 = (a2 * n2 + b2) * n3 + c2;
+  m.r1[0] = (double)a / n1, m.r1[1] = (double)b / n2, m.r1[2] = (double)c / n3;
+  m.r2[0] = (double)a2 / n1, m.r2[1] = (double)b2 / n2, m.r2[2] = (double)c2 / n3;
+  return m;
+}
+
+// rho[q1][side][k][j], side 0: e^{-2 pi i G.x_k} rho_kj(q1) / sqrt(m_k m_s2p[j]), side 1: rho_kj(q2) / sqrt(m_s2p[j])
+__global__ void __launch_bounds__(PH3_THREADS)
+rho_kernel(const int32_t* __restrict__ img_ptr, const double* __restrict__ img_vec, const int32_t* __restrict__ s2p,
+           const double* __restrict__ inv_sqrt_m, const double* __restrict__ frac, int n_prim, int n_super, int n1,
+           int n2, int n3, int target, const int32_t* __restrict__ q1_idx, int n_q1, double2* __restrict__ rho) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t per_side = (int64_t)n_prim * n_super;
+  if (i >= (int64_t)n_q1 * 2 * per_side) return;
+  const int q1l = (int)(i / (2 * per_side)), side = (int)((i / per_side) % 2);
+  const int k = (int)((i % per_side) / n_super), j = (int)(i % n_super);
+  const MeshTriplet m = mesh_triplet(target, __ldg(q1_idx + q1l), n1, n2, n3);
+  const double q0 = side == 0 ? m.r1[0] : m.r2[0], q1 = side == 0 ? m.r1[1] : m.r2[1];
+  const double q2 = side == 0 ? m.r1[2] : m.r2[2];
+  const size_t pair = (size_t)k * n_super + j;
+  const int b = __ldg(img_ptr + pair), e = __ldg(img_ptr + pair + 1);
+  double c = 0.0, s = 0.0;
+  for (int t = b; t < e; ++t) {
+    const double* v = img_vec + (size_t)t * 3;
+    double sn, cs;
+    sincospi(2.0 * fma(q0, __ldg(v), fma(q1, __ldg(v + 1), q2 * __ldg(v + 2))), &sn, &cs);
+    c += cs;
+    s += sn;
+  }
+  double w = __ldg(inv_sqrt_m + __ldg(s2p + j)) / (double)(e > b ? e - b : 1);
+  if (side == 0) {
+    w *= __ldg(inv_sqrt_m + k);
+    double sn, cs;  // e^{-2 pi i G.x_k} = cs - i sn
+    sincospi(2.0 * fma(m.g0, __ldg(frac + 3 * k), fma(m.g1, __ldg(frac + 3 * k + 1), m.g2 * __ldg(frac + 3 * k + 2))),
+             &sn, &cs);
+    const double cr = fma(c, cs, s * sn), ci = fma(s, cs, -c * sn);
+    c = cr, s = ci;
+  }
+  rho[i] = make_double2(w * c, w * s);
+}
+
+// r[q1][k a][k' b][k'' c] (see above); thread: one (k, k', k'', a b c) for the PH3_Q1_TILE q1 of grid y.  Supercell
+// atom j of primitive atom k' is k' n_cells + l (atom-major, as make_supercell orders it).
+__global__ void __launch_bounds__(PH3_THREADS)
+fc3_fourier_kernel(const double* __restrict__ fc3, const double2* __restrict__ rho, int n_prim, int n_super, int n_q1,
+                   double2* __restrict__ r) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_prim * n_prim * n_prim * 27) return;
+  const int abc = (int)(i % 27);
+  const int64_t kkk = i / 27;
+  const int kpp = (int)(kkk % n_prim), kp = (int)((kkk / n_prim) % n_prim), k = (int)(kkk / ((int64_t)n_prim * n_prim));
+  const int n_cells = n_super / n_prim;
+  const int q0 = blockIdx.y * PH3_Q1_TILE;
+  const int nq = min(PH3_Q1_TILE, n_q1 - q0);
+  double ar[PH3_Q1_TILE], ai[PH3_Q1_TILE];
+#pragma unroll
+  for (int t = 0; t < PH3_Q1_TILE; ++t) ar[t] = ai[t] = 0.0;
+  const size_t side = (size_t)n_prim * n_super;
+  const double2* rho_k = rho + (size_t)q0 * 2 * side + (size_t)k * n_super;
+  for (int lp = 0; lp < n_cells; ++lp) {
+    const int jp = kp * n_cells + lp;
+    const double* f = fc3 + (((size_t)k * n_super + jp) * n_super + (size_t)kpp * n_cells) * 27 + abc;
+    double br[PH3_Q1_TILE], bi[PH3_Q1_TILE];
+#pragma unroll
+    for (int t = 0; t < PH3_Q1_TILE; ++t) br[t] = bi[t] = 0.0;
+    for (int lpp = 0; lpp < n_cells; ++lpp) {
+      const double x = __ldg(f + (size_t)lpp * 27);
+#pragma unroll
+      for (int t = 0; t < PH3_Q1_TILE; ++t) {
+        if (t >= nq) break;
+        const double2 p2 = __ldg(rho_k + (size_t)t * 2 * side + side + kpp * n_cells + lpp);
+        br[t] = fma(x, p2.x, br[t]);
+        bi[t] = fma(x, p2.y, bi[t]);
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < PH3_Q1_TILE; ++t) {
+      if (t >= nq) break;
+      const double2 p1 = __ldg(rho_k + (size_t)t * 2 * side + jp);
+      ar[t] = fma(p1.x, br[t], fma(-p1.y, bi[t], ar[t]));
+      ai[t] = fma(p1.x, bi[t], fma(p1.y, br[t], ai[t]));
+    }
+  }
+  const int n3 = 3 * n_prim;
+  const int a = abc / 9, b = (abc / 3) % 3, c = abc % 3;
+  const size_t o = ((size_t)(3 * k + a) * n3 + 3 * kp + b) * n3 + 3 * kpp + c;
+  const size_t n33 = (size_t)n3 * n3 * n3;
+#pragma unroll
+  for (int t = 0; t < PH3_Q1_TILE; ++t) {
+    if (t >= nq) break;
+    r[(size_t)(q0 + t) * n33 + o] = make_double2(ar[t], ai[t]);
+  }
+}
+
+// The three contractions as complex GEMMs C[m][n] = sum_k A(m, k) B(k, n), one q1 per grid z and PH3_TILE^2 outputs per
+// block, e the mode-major eigenvectors (e[q][mode][k a]):
+//   STAGE 0: A = conj(e[target]) [l][k a], B = R [k a][k' b, k'' c]          -> c1 [l][k' b, k'' c]
+//   STAGE 1: per l (sub), A = e[q1] [l1][k' b], B = c1[l] [k' b][k'' c]       -> c2 [l][l1][k'' c]
+//   STAGE 2: A = c2 [l l1][k'' c], B(k, n) = e[q2][n][k], and P = C^3 / (36 N nu nu1 nu2) |C|^2 (0 below the cutoff)
+template <int STAGE>
+__global__ void __launch_bounds__(256)
+contract_kernel(const double2* __restrict__ eig, const double* __restrict__ freqs, int n_prim, int n1, int n2, int n3m,
+                int target, const int32_t* __restrict__ q1_idx, double cutoff, double p_scale,
+                const double2* __restrict__ in, double2* __restrict__ out, double* __restrict__ p) {
+  __shared__ double2 sa[PH3_KTILE][PH3_TILE];
+  __shared__ double2 sb[PH3_KTILE][PH3_TILE + 1];
+  const int n3 = 3 * n_prim;
+  const size_t n33 = (size_t)n3 * n3 * n3;
+  const int q1l = blockIdx.z;
+  const MeshTriplet mt = mesh_triplet(target, __ldg(q1_idx + q1l), n1, n2, n3m);
+  const int big = STAGE == 0 ? n3 * n3 : n3;  // N of stage 0, M of stage 2
+  const int rows = STAGE == 2 ? n3 * n3 : n3, cols = STAGE == 0 ? big : n3;
+  const int tm = (rows + PH3_TILE - 1) / PH3_TILE, tn = (cols + PH3_TILE - 1) / PH3_TILE;
+  const int sub = blockIdx.x / (tm * tn);
+  const int m0 = (blockIdx.x % (tm * tn)) / tn * PH3_TILE, c0 = blockIdx.x % tn * PH3_TILE;
+  const double2* a_base;
+  const double2* b_base;
+  if constexpr (STAGE == 0) {
+    a_base = eig + (size_t)target * n3 * n3;
+    b_base = in + (size_t)q1l * n33;
+  } else if constexpr (STAGE == 1) {
+    a_base = eig + (size_t)mt.q1 * n3 * n3;
+    b_base = in + (size_t)q1l * n33 + (size_t)sub * n3 * n3;
+  } else {
+    a_base = in + (size_t)q1l * n33;
+    b_base = eig + (size_t)mt.q2 * n3 * n3;
+  }
+  const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
+  double cr[2][2] = {{0.0, 0.0}, {0.0, 0.0}}, ci[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
+  for (int k0 = 0; k0 < n3; k0 += PH3_KTILE) {
+    __syncthreads();  // the previous tiles have been read
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int e = threadIdx.x + 256 * r;
+      const int am = e / PH3_KTILE, ak = e % PH3_KTILE;  // A(m0 + am, k0 + ak), k fastest
+      double2 x = make_double2(0.0, 0.0);
+      if (m0 + am < rows && k0 + ak < n3) {
+        x = __ldg(a_base + (size_t)(m0 + am) * n3 + k0 + ak);
+        if constexpr (STAGE == 0) x.y = -x.y;
+      }
+      sa[ak][am] = x;
+      double2 y = make_double2(0.0, 0.0);
+      if constexpr (STAGE == 2) {  // B(k, n) = e[q2][n][k]: k fastest
+        const int bn = e / PH3_KTILE, bk = e % PH3_KTILE;
+        if (c0 + bn < cols && k0 + bk < n3) y = __ldg(b_base + (size_t)(c0 + bn) * n3 + k0 + bk);
+        sb[bk][bn] = y;
+      } else {
+        const int bk = e / PH3_TILE, bn = e % PH3_TILE;
+        if (c0 + bn < cols && k0 + bk < n3) y = __ldg(b_base + (size_t)(k0 + bk) * cols + c0 + bn);
+        sb[bk][bn] = y;
+      }
+    }
+    __syncthreads();
+    const int kn = min(PH3_KTILE, n3 - k0);
+    for (int kk = 0; kk < kn; ++kk) {
+      const double2 a0 = sa[kk][ty], a1 = sa[kk][ty + 16];
+      const double2 b0 = sb[kk][tx], b1 = sb[kk][tx + 16];
+      cr[0][0] = fma(a0.x, b0.x, fma(-a0.y, b0.y, cr[0][0]));
+      ci[0][0] = fma(a0.x, b0.y, fma(a0.y, b0.x, ci[0][0]));
+      cr[0][1] = fma(a0.x, b1.x, fma(-a0.y, b1.y, cr[0][1]));
+      ci[0][1] = fma(a0.x, b1.y, fma(a0.y, b1.x, ci[0][1]));
+      cr[1][0] = fma(a1.x, b0.x, fma(-a1.y, b0.y, cr[1][0]));
+      ci[1][0] = fma(a1.x, b0.y, fma(a1.y, b0.x, ci[1][0]));
+      cr[1][1] = fma(a1.x, b1.x, fma(-a1.y, b1.y, cr[1][1]));
+      ci[1][1] = fma(a1.x, b1.y, fma(a1.y, b1.x, ci[1][1]));
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int m = m0 + ty + 16 * i, c = c0 + tx + 16 * j;
+      if (m >= rows || c >= cols) continue;
+      if constexpr (STAGE == 0) {
+        out[(size_t)q1l * n33 + (size_t)m * cols + c] = make_double2(cr[i][j], ci[i][j]);
+      } else if constexpr (STAGE == 1) {
+        out[(size_t)q1l * n33 + ((size_t)sub * n3 + m) * n3 + c] = make_double2(cr[i][j], ci[i][j]);
+      } else {
+        const double nu = __ldg(freqs + (size_t)target * n3 + m / n3);
+        const double nu1 = __ldg(freqs + (size_t)mt.q1 * n3 + m % n3);
+        const double nu2 = __ldg(freqs + (size_t)mt.q2 * n3 + c);
+        const bool keep = nu >= cutoff && nu1 >= cutoff && nu2 >= cutoff;
+        p[(size_t)q1l * n33 + (size_t)m * n3 + c] =
+            keep ? p_scale * fma(cr[i][j], cr[i][j], ci[i][j] * ci[i][j]) / (nu * nu1 * nu2) : 0.0;
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Imaginary self-energy.  For the target q and an item (q1, l1, l2) of the call, vertex q1 enters the tetrahedron
+// averages of the three deltas with the weights
+//   g(w) = 1/6 sum over the 24 (tetrahedron, corner) with that corner at q1 of tetra_weights' corner weight,
+// for the corner values f = nu1 + nu2 (g2: d(w - nu1 - nu2)), nu2 - nu1 (g1+: d(w + nu1 - nu2)) and nu1 - nu2 (g1-:
+// d(w - nu1 + nu2)), nu1 = freqs[q1'][l1], nu2 = freqs[q - q1'][l2] at each corner q1'.  (1/N) sum_q1 g reproduces the
+// tetrahedron sums of chg_joint_dos.  An item with nu1 or nu2 below the cutoff has weight 0.
+// ise_weights_kernel: one thread per item; it sorts the three corner sets of each of the 24 tetrahedra once and
+// evaluates them at every band frequency w_l (>= cutoff) inside their range, writing (g2, g1+ - g1-) to
+// wts[q1][l][l1][l2] (the layout of P), each element by its own thread.  ise_accumulate_kernel: block (chunk, l, tile
+// of ISE_T_TILE temperatures) adds 18 pi / h^2 P [(1 + n1 + n2) g2 + (n1 - n2) (g1+ - g1-)] over its chunk of items in
+// a fixed order and writes work[chunk][t][l]; chunk_reduce_kernel adds the chunks in chunk order to gamma.  The
+// weights depend on the frequencies only and are formed once per call for every temperature.  No atomics.
+constexpr int ISE_THREADS = 256;
+constexpr int ISE_T_TILE = 8;
+// 18 pi / h^2 with h in eV/THz: chgnet_b200.phonons.H_EV_PER_THZ, the same expression in the same order
+constexpr double ISE_H = 6.62607015e-34 / 1.602176634e-19 * 1e12;
+
+// wt[p] for a run-time index p, from registers
+__device__ __forceinline__ double corner_weight(const double (&wt)[4], int p) {
+  return p == 0 ? wt[0] : (p == 1 ? wt[1] : (p == 2 ? wt[2] : wt[3]));
+}
+
+__global__ void __launch_bounds__(ISE_THREADS)
+ise_weights_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
+                   const int32_t* __restrict__ tet, int target, const double* __restrict__ omega,
+                   const int32_t* __restrict__ q1_idx, int n_q1, double cutoff, double2* __restrict__ wts) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nb2 = (int64_t)n_band * n_band;
+  if (i >= (int64_t)n_q1 * nb2) return;
+  const int q1l = (int)(i / nb2), l1 = (int)((i / n_band) % n_band), l2 = (int)(i % n_band);
+  double2* w_out = wts + (size_t)q1l * n_band * nb2 + (size_t)(i % nb2);
+  for (int l = 0; l < n_band; ++l) w_out[(size_t)l * nb2] = make_double2(0.0, 0.0);
+  const int q1 = __ldg(q1_idx + q1l);
+  const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
+  const auto nu_pair = [&](int a, int b, int c, double& nu1, double& nu2) {
+    int a2 = ta - a, b2 = tb - b, c2 = tc - c;
+    a2 += a2 < 0 ? n1 : 0;
+    b2 += b2 < 0 ? n2 : 0;
+    c2 += c2 < 0 ? n3 : 0;
+    nu1 = __ldg(freqs + (int64_t)((a * n2 + b) * n3 + c) * n_band + l1);
+    nu2 = __ldg(freqs + (int64_t)((a2 * n2 + b2) * n3 + c2) * n_band + l2);
+  };
+  const int qa = q1 / (n2 * n3), qb = (q1 / n3) % n2, qc = q1 % n3;
+  double nu1, nu2;
+  nu_pair(qa, qb, qc, nu1, nu2);
+  if (!(nu1 >= cutoff && nu2 >= cutoff)) return;
+  for (int tv = 0; tv < 24; ++tv) {
+    const int it = tv / 4, v = tv % 4;
+    const int32_t* o = tet + (it * 4 + v) * 3;
+    // the cell whose corner v of tetrahedron it is q1
+    int ca = qa - __ldg(o), cb = qb - __ldg(o + 1), cc = qc - __ldg(o + 2);
+    ca += ca < 0 ? n1 : 0;
+    cb += cb < 0 ? n2 : 0;
+    cc += cc < 0 ? n3 : 0;
+    double e2[4], ep[4], em[4];
+    int x2[4], xp[4], xm[4];
+    tetrahedron_corners(tet, ((int64_t)(ca * n2 + cb) * n3 + cc) * 6 + it, n1, n2, n3, [&](int u, int a, int b, int c) {
+      double v1, v2;
+      nu_pair(a, b, c, v1, v2);
+      e2[u] = v1 + v2, ep[u] = v2 - v1, em[u] = v1 - v2;
+      x2[u] = xp[u] = xm[u] = u;
+    });
+    sort4(e2, x2);
+    sort4(ep, xp);
+    sort4(em, xm);
+    int p2 = 0, pp = 0, pm = 0;
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      p2 = x2[u] == v ? u : p2;
+      pp = xp[u] == v ? u : pp;
+      pm = xm[u] == v ? u : pm;
+    }
+    for (int l = 0; l < n_band; ++l) {
+      const double w = __ldg(omega + l);
+      if (!(w >= cutoff)) continue;
+      const bool h2 = w >= e2[0] && w < e2[3], hp = w >= ep[0] && w < ep[3], hm = w >= em[0] && w < em[3];
+      if (!(h2 || hp || hm)) continue;
+      double n, g, wt[4], d2 = 0.0, d1 = 0.0;
+      if (h2) {
+        tetra_weights(w, e2, n, g, wt);
+        d2 = corner_weight(wt, p2);
+      }
+      if (hp) {
+        tetra_weights(w, ep, n, g, wt);
+        d1 = corner_weight(wt, pp);
+      }
+      if (hm) {
+        tetra_weights(w, em, n, g, wt);
+        d1 -= corner_weight(wt, pm);
+      }
+      double2 acc = w_out[(size_t)l * nb2];
+      acc.x = fma(d2, 1.0 / 6.0, acc.x);
+      acc.y = fma(d1, 1.0 / 6.0, acc.y);
+      w_out[(size_t)l * nb2] = acc;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(ISE_THREADS)
+ise_accumulate_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3, int target,
+                      const double* __restrict__ omega, const int32_t* __restrict__ q1_idx, int n_q1,
+                      const double* __restrict__ p, const double2* __restrict__ wts, const double* __restrict__ temps,
+                      int n_t, double cutoff, double* __restrict__ work) {
+  __shared__ double red[ISE_THREADS][ISE_T_TILE];
+  const int l = blockIdx.y, t0 = blockIdx.z * ISE_T_TILE;
+  const int t_here = min(ISE_T_TILE, n_t - t0);
+  const int64_t nb2 = (int64_t)n_band * n_band, n_items = (int64_t)n_q1 * nb2;
+  const int64_t begin = n_items * blockIdx.x / gridDim.x, end = n_items * (blockIdx.x + 1) / gridDim.x;
+  double acc[ISE_T_TILE];
+#pragma unroll
+  for (int t = 0; t < ISE_T_TILE; ++t) acc[t] = 0.0;
+  double tt[ISE_T_TILE];
+#pragma unroll
+  for (int t = 0; t < ISE_T_TILE; ++t) tt[t] = t < t_here ? __ldg(temps + t0 + t) : 0.0;
+  const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
+  if (__ldg(omega + l) >= cutoff) {
+    for (int64_t i = begin + threadIdx.x; i < end; i += ISE_THREADS) {
+      const int q1l = (int)(i / nb2);
+      const size_t at = ((size_t)q1l * n_band + l) * nb2 + (size_t)(i % nb2);
+      const double2 w = __ldg(wts + at);
+      if (w.x == 0.0 && w.y == 0.0) continue;
+      const double pv = __ldg(p + at);
+      if (pv == 0.0) continue;
+      const int l1 = (int)((i / n_band) % n_band), l2 = (int)(i % n_band);
+      const int q1 = __ldg(q1_idx + q1l);
+      const int a = q1 / (n2 * n3), b = (q1 / n3) % n2, c = q1 % n3;
+      int a2 = ta - a, b2 = tb - b, c2 = tc - c;
+      a2 += a2 < 0 ? n1 : 0;
+      b2 += b2 < 0 ? n2 : 0;
+      c2 += c2 < 0 ? n3 : 0;
+      const double nu1 = __ldg(freqs + (int64_t)q1 * n_band + l1);
+      const double nu2 = __ldg(freqs + (int64_t)((a2 * n2 + b2) * n3 + c2) * n_band + l2);
+#pragma unroll
+      for (int t = 0; t < ISE_T_TILE; ++t) {
+        if (t >= t_here) break;
+        const double b1 = bose(nu1, tt[t]), b2v = bose(nu2, tt[t]);
+        acc[t] = fma(pv, fma(1.0 + b1 + b2v, w.x, (b1 - b2v) * w.y), acc[t]);
+      }
+    }
+  }
+#pragma unroll
+  for (int t = 0; t < ISE_T_TILE; ++t) red[threadIdx.x][t] = acc[t];
+  __syncthreads();
+  if (threadIdx.x < t_here) {
+    double s = 0.0;
+    for (int i = 0; i < ISE_THREADS; ++i) s += red[i][threadIdx.x];
+    work[((size_t)blockIdx.x * n_t + t0 + threadIdx.x) * n_band + l] = s * (18.0 * 3.141592653589793 / (ISE_H * ISE_H));
+  }
+}
+
 }  // namespace
 }  // namespace chg
 
@@ -816,5 +1187,80 @@ extern "C" int chg_broadened_spectrum(const double* freqs, const double* weights
   CHG_CUDA(reduce_chunks(work, chunks, (int64_t)n_t * n_groups_here * n_freq,
                          SpectrumStore{out, n_freq, n_groups_here, g_first, n_groups, 1.0 / group_size},
                          as_stream(stream)));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_phonon_interaction(const double* fc3, const int32_t* img_ptr, const double* img_vec,
+                                      const int32_t* s2p, const double* inv_sqrt_m, const double* frac, int32_t n_prim,
+                                      int32_t n_super, int32_t n1, int32_t n2, int32_t n3, const double* freqs,
+                                      const double* eigvecs, int32_t target, const int32_t* q1_idx, int32_t n_q1,
+                                      double cutoff_thz, double* work, int64_t work_doubles, double* out,
+                                      void* stream) {
+  CHG_CHECK_ARG(n_prim >= 0 && n_super >= 0 && n_q1 >= 0 && n1 > 0 && n2 > 0 && n3 > 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(target >= 0 && (int64_t)target < (int64_t)n1 * n2 * n3, "target outside the mesh");
+  if (n_prim == 0 || n_q1 == 0) return CHG_OK;
+  CHG_CHECK_ARG(fc3 && img_ptr && img_vec && s2p && inv_sqrt_m && frac && freqs && eigvecs && q1_idx && work && out,
+                "null pointer");
+  CHG_CHECK_ARG(n_super % n_prim == 0, "n_super must be a multiple of n_prim (atom-major supercell)");
+  CHG_CHECK_ARG(n_q1 <= 65535, "too many q1 in one call (at most 65535)");
+  const int64_t nb = 3 * (int64_t)n_prim, n33 = nb * nb * nb;
+  const int64_t rho_n = (int64_t)n_q1 * 2 * n_prim * n_super;
+  CHG_CHECK_ARG(work_doubles >= 2 * (rho_n + 2 * (int64_t)n_q1 * n33), "work holds less than 4 n_q1 (n_prim n_super + (3 n_prim)^3) doubles");
+  double2* rho = reinterpret_cast<double2*>(work);
+  double2* buf_a = rho + rho_n;
+  double2* buf_b = buf_a + (size_t)n_q1 * n33;
+  const double2* eig = reinterpret_cast<const double2*>(eigvecs);
+  cudaStream_t st = as_stream(stream);
+  rho_kernel<<<(unsigned)((rho_n + PH3_THREADS - 1) / PH3_THREADS), PH3_THREADS, 0, st>>>(
+      img_ptr, img_vec, s2p, inv_sqrt_m, frac, n_prim, n_super, n1, n2, n3, target, q1_idx, n_q1, rho);
+  count_launch();
+  const int64_t n_r = (int64_t)n_prim * n_prim * n_prim * 27;
+  const dim3 rgrid((unsigned)((n_r + PH3_THREADS - 1) / PH3_THREADS), (unsigned)((n_q1 + PH3_Q1_TILE - 1) / PH3_Q1_TILE));
+  fc3_fourier_kernel<<<rgrid, PH3_THREADS, 0, st>>>(fc3, rho, n_prim, n_super, n_q1, buf_a);
+  count_launch();
+  const int64_t t1 = (nb + PH3_TILE - 1) / PH3_TILE, t2 = (nb * nb + PH3_TILE - 1) / PH3_TILE;
+  const double p_scale = SQW_C * SQW_C * SQW_C / (36.0 * (double)n1 * n2 * n3);
+  contract_kernel<0><<<dim3((unsigned)(t1 * t2), 1, n_q1), 256, 0, st>>>(
+      eig, freqs, n_prim, n1, n2, n3, target, q1_idx, cutoff_thz, p_scale, buf_a, buf_b, nullptr);
+  count_launch();
+  contract_kernel<1><<<dim3((unsigned)(nb * t1 * t1), 1, n_q1), 256, 0, st>>>(
+      eig, freqs, n_prim, n1, n2, n3, target, q1_idx, cutoff_thz, p_scale, buf_b, buf_a, nullptr);
+  count_launch();
+  contract_kernel<2><<<dim3((unsigned)(t2 * t1), 1, n_q1), 256, 0, st>>>(
+      eig, freqs, n_prim, n1, n2, n3, target, q1_idx, cutoff_thz, p_scale, buf_a, nullptr, out);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_imag_self_energy(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                                    const int32_t* tetrahedra, int32_t target, const double* omega,
+                                    const int32_t* q1_idx, int32_t n_q1, const double* p, const double* temperatures,
+                                    int32_t n_t, double cutoff_thz, double* work, int64_t work_doubles, double* gamma,
+                                    void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_q1 >= 0 && n_t >= 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 * std::max(n_band, 1) < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(target >= 0 && (int64_t)target < (int64_t)n1 * n2 * n3, "target outside the mesh");
+  if (n_band == 0 || n_q1 == 0 || n_t == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && tetrahedra && omega && q1_idx && p && temperatures && work && gamma, "null pointer");
+  const int64_t nb2 = (int64_t)n_band * n_band, n_items = (int64_t)n_q1 * nb2;
+  const int64_t n_w = 2 * n_items * n_band;
+  CHG_CHECK_ARG(work_doubles >= n_w + (int64_t)CHG_ISE_MAX_CHUNKS * n_t * n_band,
+                "work holds less than 2 n_q1 n_band^3 + CHG_ISE_MAX_CHUNKS n_t n_band doubles");
+  const int64_t t_tiles = ((int64_t)n_t + ISE_T_TILE - 1) / ISE_T_TILE;
+  CHG_CHECK_ARG(n_band <= 65535 && t_tiles <= 65535, "too many bands or temperatures");
+  double2* wts = reinterpret_cast<double2*>(work);
+  double* partial = work + n_w;
+  cudaStream_t st = as_stream(stream);
+  ise_weights_kernel<<<(unsigned)((n_items + ISE_THREADS - 1) / ISE_THREADS), ISE_THREADS, 0, st>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, target, omega, q1_idx, n_q1, cutoff_thz, wts);
+  count_launch();
+  // enough chunks for about 4 096 blocks in all, at most CHG_ISE_MAX_CHUNKS and one pass of the block's threads each
+  const int64_t others = (int64_t)n_band * t_tiles;
+  const int64_t want = (4096 + others - 1) / others;
+  const int chunks = (int)std::max<int64_t>(
+      1, std::min<int64_t>({(int64_t)CHG_ISE_MAX_CHUNKS, (n_items + ISE_THREADS - 1) / ISE_THREADS, want}));
+  ise_accumulate_kernel<<<dim3(chunks, (unsigned)n_band, (unsigned)t_tiles), ISE_THREADS, 0, st>>>(
+      freqs, n_band, n1, n2, n3, target, omega, q1_idx, n_q1, p, wts, temperatures, n_t, cutoff_thz, partial);
+  CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_t * n_band, AccumulateStore{gamma}, st));
   CHG_LAUNCH_END();
 }

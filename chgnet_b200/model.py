@@ -902,7 +902,8 @@ class CHGNet(nn.Module):
             out.update(relaxed_ion=relaxed, hessian=h, unstable_modes=unstable)
         return out
 
-    def phonons(self, structure, supercell_matrix, *, batch_size: int = 16):
+    def phonons(self, structure, supercell_matrix, *, batch_size: int = 16, third_order: bool = False,
+                displacement: float = 0.03):
         """Harmonic phonons of a crystal from exact supercell force constants: a ``chgnet_b200.phonons.Phonons``.
 
         ``structure`` is the primitive cell, in any form ``GraphConverter`` accepts (a structure-like object or a
@@ -916,15 +917,29 @@ class CHGNet(nn.Module):
         ``Phonons.thermal_properties``, with the dynamical matrices built on the device.
 
         The supercell should be large enough that the force constants have decayed at its boundary, and the structure
-        should be relaxed: unstable modes are reported as imaginary (negative) frequencies, not hidden."""
-        from chgnet_b200.phonons import Phonons, compact_force_constants, make_supercell
+        should be relaxed: unstable modes are reported as imaginary (negative) frequencies, not hidden.
 
+        With ``third_order``, also the third-order force constants ``[n_prim, N, N, 3, 3, 3]`` in eV/A^3
+        (``third_order_force_constants``, ``Phonons.force_constants3``) for ``Phonons.linewidths`` and
+        ``Phonons.thermal_conductivity``: central differences of full supercell Hessians with each atom of one
+        primitive cell moved by +-``displacement`` (A) along each axis, 6 n_prim displaced supercells, each with a graph
+        of its own (the neighbour lists follow the displacement) and 3N Hessian-vector columns.  ValueError unless
+        ``displacement`` is finite and > 0."""
+        from chgnet_b200.phonons import Phonons, compact_force_constants, make_supercell, third_order_force_constants
+
+        h = float(displacement)
+        if not (math.isfinite(h) and h > 0):
+            raise ValueError(f"displacement must be finite and positive, got {displacement!r}")
         if self.graph_converter is None:
             raise ValueError("graph_converter cannot be None!")
         sc = make_supercell(*self._structure_arrays(structure), supercell_matrix)
         graph = self.graph_converter((sc.z, sc.frac, sc.lattice))
         fc = compact_force_constants(lambda v: self._hvp_replicas(graph, v, batch_size), sc)
-        return Phonons(fc, sc, device=self.device)
+        fc3 = None
+        if third_order:
+            fc3 = third_order_force_constants(
+                lambda frac, v: self._hvp_replicas(self.graph_converter((sc.z, frac, sc.lattice)), v, batch_size), sc, h)
+        return Phonons(fc, sc, fc3=fc3, device=self.device)
 
     def static_evaluator(self, graph, *, task: PredTask = "efsm"):
         """Evaluator for graph(s) whose TOPOLOGY stays fixed while coordinates / cells change (finite differences,

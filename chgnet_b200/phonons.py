@@ -14,12 +14,16 @@
   joint densities of states and their occupation-weighted forms at mesh q-points, and per mode as the three-phonon
   phase space (``chg_joint_dos``); coherent one-phonon neutron structure factors S(Q, omega) per mode at scattering
   vectors and their broadened spectra, per Q (``dynamic_structure_factor``) and averaged over directions for powders
-  (``powder_spectrum``), with ``chg_structure_factors`` and ``chg_broadened_spectrum``.
+  (``powder_spectrum``), with ``chg_structure_factors`` and ``chg_broadened_spectrum``; with third-order force
+  constants (``third_order_force_constants``), three-phonon interaction strengths (``chg_phonon_interaction``),
+  linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation.
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
 primitive cell for densities of states, A^2 for thermal displacement matrices, 1/THz for joint densities of states,
-b^2 per primitive cell for structure factors (b the caller's scattering lengths) and b^2/THz for their spectra.
+b^2 per primitive cell for structure factors (b the caller's scattering lengths) and b^2/THz for their spectra,
+eV/A^3 for third-order force constants, eV^2 for interaction strengths, THz for linewidths, ps for lifetimes and
+W/(m K) for thermal conductivities.
 """
 from __future__ import annotations
 
@@ -30,7 +34,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from chgnet_b200._lib import JDOS_MAX_CHUNKS, sqw_scratch_doubles
+from chgnet_b200._lib import JDOS_MAX_CHUNKS, ise_scratch_doubles, ph3_scratch_doubles, sqw_scratch_doubles
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -47,6 +51,8 @@ IMAGE_TOL = 1e-5
 THERMAL_CUTOFF_THZ = 1e-3
 # adjacent modes closer than this (THz) form a degenerate set for the group velocities
 DEGENERACY_THZ = 1e-4
+# eV THz / (K A) in W/(m K): the unit of C v v tau / V with C in eV/K, v in THz A, tau in ps and V in A^3
+KAPPA_W_PER_MK = _EV * 1e12 / _ANGSTROM
 
 
 def supercell_matrix(m) -> np.ndarray:
@@ -184,6 +190,35 @@ def compact_force_constants(hvp, sc: Supercell) -> np.ndarray:
     return np.ascontiguousarray(cols.reshape(n_prim, 3, n, 3).transpose(0, 2, 1, 3))
 
 
+def third_order_force_constants(hvp_at, sc: Supercell, displacement: float) -> np.ndarray:
+    """Compact third-order force constants ``[n_prim, N, N, 3, 3, 3]`` in eV/A^3 (phono3py's compact layout) by
+    central differences of Hessians: Phi3[k, j', j'', a, b, c] = (H+ - H-)[j' b, j'' c] / 2h, H+- the supercell
+    Hessian with atom ``p2s[k]`` moved by +-h (``displacement``, A) along the Cartesian axis a.  Returned as computed
+    (not symmetrised).
+
+    ``hvp_at(frac [N, 3], v [K, N, 3]) -> [K, N, 3]`` computes H v (eV/A^2) for the supercell ``sc`` with the
+    fractional coordinates ``frac`` (same lattice); it is called 6 n_prim times, each with the 3N unit directions.
+    ValueError unless ``displacement`` is finite and > 0."""
+    h = float(displacement)
+    if not (np.isfinite(h) and h > 0):
+        raise ValueError(f"displacement must be finite and positive, got {displacement!r}")
+    n_prim, n = len(sc.p2s), len(sc.s2p)
+    inv = np.linalg.inv(np.asarray(sc.lattice, dtype=np.float64))
+    cols = np.eye(3 * n).reshape(3 * n, n, 3)
+    out = np.empty((n_prim, n, n, 3, 3, 3))
+    for k in range(n_prim):
+        for a in range(3):
+            hs = []
+            for sgn in (1.0, -1.0):
+                frac = np.array(sc.frac, dtype=np.float64)
+                frac[sc.p2s[k]] += sgn * h * inv[a]  # Cartesian step h e_a in supercell fractional coordinates
+                hv = np.asarray(hvp_at(frac % 1.0, cols), dtype=np.float64).reshape(3 * n, 3 * n)  # row c: H e_c
+                hs.append(hv.T)  # H[j' b, j'' c]
+            d = (hs[0] - hs[1]) / (2.0 * h)
+            out[k, :, :, a] = d.reshape(n, 3, n, 3).transpose(0, 2, 1, 3)
+    return out
+
+
 def acoustic_sum_rule(fc: np.ndarray, p2s: np.ndarray) -> tuple[np.ndarray, float]:
     """Copy of ``fc`` with the self-term correction Phi(k0, k0) -= sum_j Phi(k0, j), and the largest entry of the
     correction (eV/A^2)."""
@@ -283,6 +318,28 @@ def _zero_gamma_rows(nu: torch.Tensor, q: np.ndarray) -> None:
         nu[r[:, None], torch.argsort(nu[r].abs(), dim=1, stable=True)[:, :3]] = 0.0
 
 
+def _mesh_indices(mesh, q: np.ndarray) -> np.ndarray:
+    """[Q] int64 indices of the reduced ``q`` [Q, 3] on the full Gamma-centred ``mesh``; ValueError unless q * mesh is
+    integral to 1e-8."""
+    m = np.asarray(mesh, dtype=np.int64).reshape(-1)
+    x = q * m
+    if not np.all(np.isfinite(x)) or np.any(np.abs(x - np.round(x)) > 1e-8):
+        raise ValueError(f"qpoints must lie on the {m.tolist()} mesh (q * mesh integral), got {q.tolist()}")
+    idx = np.round(x).astype(np.int64) % m
+    return (idx[:, 0] * m[1] + idx[:, 1]) * m[2] + idx[:, 2]
+
+
+def _degenerate_average(gamma: torch.Tensor, nu: torch.Tensor) -> torch.Tensor:
+    """gamma [T, 3n] averaged over each set of degenerate modes of nu [3n] (adjacent |d nu| < ``DEGENERACY_THZ``), and
+    0 for the modes below ``THERMAL_CUTOFF_THZ``."""
+    gap = (nu[1:] - nu[:-1]).abs() >= DEGENERACY_THZ
+    sid = torch.cat([torch.zeros(1, dtype=torch.long, device=nu.device), gap.long().cumsum(0)])
+    n_sets = int(sid[-1]) + 1
+    sums = torch.zeros(gamma.shape[0], n_sets, dtype=gamma.dtype, device=gamma.device).index_add_(1, sid, gamma)
+    counts = torch.bincount(sid, minlength=n_sets).to(gamma.dtype)
+    return torch.where(nu >= THERMAL_CUTOFF_THZ, (sums / counts)[:, sid], 0.0)
+
+
 def _gaussian_sigma(width) -> float | None:
     """The standard deviation (THz) of a Gaussian of FWHM ``width``, width / (2 sqrt(2 ln 2)); None for None, and
     ValueError unless it is finite and > 0."""
@@ -310,7 +367,8 @@ class Phonons:
     Attributes: ``force_constants`` ``[n_prim, N, 3, 3]`` eV/A^2 as computed (not symmetrised), relative to
     ``supercell`` = ``(z, frac, lattice)``; ``p2s`` / ``s2p`` the atom maps (supercell atom j = k n_cells + l);
     ``asr_correction`` the largest entry of the acoustic-sum-rule correction (eV/A^2); ``masses`` of the primitive
-    atoms (amu, ``chgnet_b200.dynamics.ATOMIC_MASSES``).
+    atoms (amu, ``chgnet_b200.dynamics.ATOMIC_MASSES``); ``force_constants3`` ``[n_prim, N, N, 3, 3, 3]`` eV/A^3 (the
+    ``fc3`` argument, as computed; None without it), which ``linewidths`` and ``thermal_conductivity`` need.
 
     D(q) follows phonopy: the phase of the full interatomic vector r_j - r_k (basis offsets included) over the minimum
     images of the supercell, each weighted by 1 / multiplicity; built from the force constants with the self-term
@@ -327,7 +385,11 @@ class Phonons:
     # many bytes (or at one group of rows, when a group alone needs more)
     sqw_chunk_bytes = 1 << 28
 
-    def __init__(self, force_constants: np.ndarray, sc: Supercell, *, device="cuda", kernels=None) -> None:
+    # linewidths and thermal_conductivity: q1 per chg_phonon_interaction / chg_imag_self_energy call keep P, the
+    # tetrahedron weights and both calls' scratch below this many bytes
+    ph3_chunk_bytes = 1 << 28
+
+    def __init__(self, force_constants: np.ndarray, sc: Supercell, *, fc3=None, device="cuda", kernels=None) -> None:
         if kernels is None:
             from chgnet_b200._lib import CudaKernels
 
@@ -349,6 +411,13 @@ class Phonons:
         self._s2p = torch.as_tensor(sc.s2p).to(dev)
         self._inv_sqrt_m = torch.as_tensor(1.0 / np.sqrt(self.masses)).to(dev)
         self._lattice = torch.as_tensor(np.ascontiguousarray(sc.prim_lattice, dtype=np.float64)).to(dev)
+        self.force_constants3 = None
+        if fc3 is not None:
+            self.force_constants3 = np.asarray(fc3, dtype=np.float64)
+            if self.force_constants3.shape != (n_prim, n, n, 3, 3, 3):
+                raise ValueError(f"third-order force constants must have shape {[n_prim, n, n, 3, 3, 3]}, got "
+                                 f"{list(self.force_constants3.shape)}")
+            self._fc3 = torch.as_tensor(np.ascontiguousarray(self.force_constants3)).to(dev)
 
     def dynamical_matrices(self, qpoints) -> torch.Tensor:
         """D(q) ``[Q, 3 n_prim, 3 n_prim]`` complex128 on the device, in eV/(A^2 amu), for reduced ``qpoints [Q,3]``."""
@@ -570,13 +639,9 @@ class Phonons:
         q = np.asarray(qpoints, dtype=np.float64)
         single = q.ndim == 1
         q = q.reshape(-1, 3)
-        m = np.asarray(mesh, dtype=np.int64).reshape(-1)
-        x = q * m
-        if not np.all(np.isfinite(x)) or np.any(np.abs(x - np.round(x)) > 1e-8):
-            raise ValueError(f"qpoints must lie on the {m.tolist()} mesh (q * mesh integral), got {q.tolist()}")
+        idx = _mesh_indices(mesh, q)
         mesh, nu, n_imaginary, tets, temps, t = self._jdos_mesh(mesh, temperatures)
-        idx = np.round(x).astype(np.int64) % m
-        targets = torch.as_tensor(((idx[:, 0] * m[1] + idx[:, 1]) * m[2] + idx[:, 2]).astype(np.int32)).to(self.device)
+        targets = torch.as_tensor(idx.astype(np.int32)).to(self.device)
         if frequency_points is None:
             top = 2 * nu.max()
             omega = torch.lerp(torch.zeros_like(top).expand(201), top.expand(201),
@@ -788,3 +853,137 @@ class Phonons:
         if dw_imag is not None:
             res["debye_waller_n_imaginary"] = dw_imag
         return res
+
+    def _three_phonon_mesh(self, mesh, temperatures):
+        """The mesh, its frequencies [N, 3n] on the device with the three modes of smallest |nu| at Gamma set to 0,
+        the mode-major eigenvectors [N, mode, 3n], ``n_imaginary`` (counted before that), the tetrahedra and the
+        temperatures (fp64 array; None allowed) for the three-phonon methods.  ValueError without fc3."""
+        if self.force_constants3 is None:
+            raise ValueError("this needs third-order force constants: build the phonons with "
+                             "CHGNet.phonons(..., third_order=True), or pass fc3 to Phonons")
+        temps = None if temperatures is None else _temperatures(temperatures)
+        mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
+        q = gamma_mesh(mesh)
+        n3, dev = 3 * len(self.p2s), self.device
+        nu = torch.empty(len(q), n3, dtype=torch.float64, device=dev)
+        e = torch.empty(len(q), n3, n3, dtype=torch.complex128, device=dev)
+        for s, nu_s, e_s in self._eigh_chunks(q, eigenvectors=True, eigh_batch=self.eigh_batch):
+            nu[s] = nu_s
+            e[s] = e_s.mT  # eigh's columns are the modes: the kernels read them mode-major
+        n_imaginary = int((nu < -THERMAL_CUTOFF_THZ).sum())
+        _zero_gamma_acoustic(nu)
+        tets = torch.as_tensor(tetrahedra(mesh, self.cell.prim_lattice)).to(dev)
+        return mesh, nu, e, n_imaginary, tets, temps
+
+    def _q1_chunk(self, n_t) -> int:
+        """q1 per ``chg_phonon_interaction`` / ``chg_imag_self_energy`` call: P, both calls' scratch within
+        ``ph3_chunk_bytes`` (at least one)."""
+        n_prim = len(self.p2s)
+        nb = 3 * n_prim
+        per_q1 = 8 * (nb**3 + ph3_scratch_doubles(1, n_prim, len(self.s2p)) + ise_scratch_doubles(1, nb, 0))
+        fixed = 8 * ise_scratch_doubles(0, nb, n_t)
+        return int(max(1, min(65535, (self.ph3_chunk_bytes - fixed) // per_q1)))
+
+    def _interactions(self, mesh, nu, e, target: int, q1: torch.Tensor) -> torch.Tensor:
+        """P [len(q1), 3n, 3n, 3n] (eV^2) of the mesh index ``target`` with the mesh indices ``q1`` (int32, device)."""
+        nb = 3 * len(self.p2s)
+        frac = torch.as_tensor(np.ascontiguousarray(self.cell.prim_frac, dtype=np.float64)).to(self.device)
+        p = torch.empty(len(q1), nb, nb, nb, dtype=torch.float64, device=self.device)
+        self.kernels.phonon_interaction(self._fc3, self._img_ptr, self._img_vec, self._s2p, self._inv_sqrt_m, frac,
+                                        mesh, nu, e, int(target), q1, THERMAL_CUTOFF_THZ, p)
+        return p
+
+    def _target_linewidths(self, mesh, nu, e, tets, t, target: int) -> torch.Tensor:
+        """Gamma [T, 3n] (THz) of the modes of the mesh index ``target``: P and its contribution to Gamma per chunk of
+        q1 (``_q1_chunk``, chunks in mesh order), then averaged over degenerate sets."""
+        n_mesh, nb = nu.shape
+        gamma = torch.zeros(len(t), nb, dtype=torch.float64, device=self.device)
+        omega = nu[target].contiguous()
+        chunk = self._q1_chunk(len(t))
+        for s in range(0, n_mesh, chunk):
+            q1 = torch.arange(s, min(s + chunk, n_mesh), dtype=torch.int32, device=self.device)
+            p = self._interactions(mesh, nu, e, target, q1)
+            self.kernels.imag_self_energy(nu, mesh, tets, int(target), omega, q1, p, t, THERMAL_CUTOFF_THZ, gamma)
+        return _degenerate_average(gamma, omega)
+
+    def _interaction_strength(self, mesh, q, q1=None) -> np.ndarray:
+        """The interaction strengths P [Q1, 3n, 3n, 3n] (eV^2, ``chg_phonon_interaction``) of the mesh point ``q`` [3]
+        with the mesh points ``q1`` [Q1, 3] (default: the whole mesh, in mesh order), q2 = q - q1 on the mesh."""
+        mesh_t, nu, e, _, _, _ = self._three_phonon_mesh(mesh, None)
+        target = int(_mesh_indices(mesh_t, np.asarray(q, dtype=np.float64).reshape(1, 3))[0])
+        if q1 is None:
+            idx = np.arange(nu.shape[0])
+        else:
+            idx = _mesh_indices(mesh_t, np.asarray(q1, dtype=np.float64).reshape(-1, 3))
+        q1_t = torch.as_tensor(idx.astype(np.int32)).to(self.device)
+        return self._interactions(mesh_t, nu, e, target, q1_t).cpu().numpy()
+
+    def linewidths(self, mesh, qpoints, temperatures) -> dict:
+        """Three-phonon linewidths (phono3py's imaginary self-energy at omega = nu, half width) of the modes at
+        ``qpoints`` ([Q, 3] or [3], reduced, on the full Gamma-centred ``mesh``: q * mesh integral to 1e-8, else
+        ValueError) at ``temperatures`` (K, finite and >= 0, else ValueError), in THz (DESIGN.md section 12.7):
+
+            Gamma_l(q; T) = 18 pi / h^2 sum_{q1 l1 l2} P_l,l1,l2(q; q1) {(1 + n1 + n2) g2 + (n1 - n2) [g1+ - g1-]}
+
+        over the N mesh points q1, q2 = q - q1 on the mesh, P the interaction strengths (eV^2, 1/N included) of the
+        third-order force constants, n = 1 / expm1(h nu / k T) and g2, g1+, g1- the linear-tetrahedron weights of
+        vertex q1 for d(w - nu1 - nu2), d(w + nu1 - nu2) and d(w - nu1 + nu2) with the tetrahedra of ``joint_dos``.
+        Modes below ``THERMAL_CUTOFF_THZ``, and the three modes of smallest |nu| at Gamma, take no part (P = 0) and get
+        0; Gamma is averaged over each set of degenerate modes at q (adjacent |d nu| < ``DEGENERACY_THZ``).  The
+        lifetime is tau = 1 / (4 pi Gamma) ps.
+
+        Returns ``frequencies`` [Q, 3n] (THz, with that Gamma rule), ``temperatures``, ``linewidths`` [T, Q, 3n] and
+        ``n_imaginary`` (the modes below -``THERMAL_CUTOFF_THZ`` over the mesh).  Needs ``force_constants3``
+        (``CHGNet.phonons(..., third_order=True)``), else ValueError.  Frequencies and eigenvectors of the mesh come
+        from one eigendecomposition per call; P (``chg_phonon_interaction``) is made and consumed
+        (``chg_imag_self_energy``) per chunk of q1 within ``ph3_chunk_bytes``, on the device."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = q.reshape(-1, 3)
+        idx = _mesh_indices(mesh, q)
+        if temperatures is None:
+            raise ValueError("linewidths needs temperatures")
+        mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        t = torch.as_tensor(temps).to(self.device)
+        gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, int(i)) for i in idx], 1)
+        res = {"frequencies": nu[torch.as_tensor(idx).to(self.device)].cpu().numpy(), "temperatures": temps,
+               "linewidths": gamma.cpu().numpy(), "n_imaginary": n_imaginary}
+        if single:
+            res["frequencies"], res["linewidths"] = res["frequencies"][0], res["linewidths"][:, 0]
+        return res
+
+    def thermal_conductivity(self, mesh, temperatures) -> dict:
+        """Lattice thermal conductivity in the relaxation-time approximation on the full Gamma-centred ``mesh``, every
+        mesh point a target (no symmetry reduction), in W/(m K):
+
+            kappa(T) = 1 / (N V0) sum_{q l} C_l v_l (x) v_l tau_l,   C = k_B x^2 e^x / (e^x - 1)^2,  x = h nu / k T
+
+        with tau = 1 / (4 pi Gamma) from ``linewidths``, v from ``group_velocities`` and V0 the primitive-cell volume.
+        Modes below ``THERMAL_CUTOFF_THZ`` (and the three modes of smallest |nu| at Gamma) are left out, and so are
+        modes with Gamma <= 0, whose lifetime is undefined; ``n_zero_linewidth`` [T] counts those.
+
+        Returns ``temperatures``, ``kappa`` [T, 3, 3], per mode ``frequencies`` [N, 3n] (THz), ``linewidths``
+        [T, N, 3n] (THz), ``group_velocities`` [N, 3n, 3] (THz A) and ``heat_capacity`` [T, N, 3n] (eV/K), and
+        ``n_imaginary`` and ``n_zero_linewidth``.  Needs ``force_constants3``, else ValueError; bad temperatures raise
+        ValueError."""
+        if temperatures is None:
+            raise ValueError("thermal_conductivity needs temperatures")
+        mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        dev = self.device
+        t = torch.as_tensor(temps).to(dev)
+        gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, i) for i in range(nu.shape[0])], 1)
+        v = torch.as_tensor(self.group_velocities(gamma_mesh(mesh))).to(dev)  # [N, 3n, 3]
+        kept = nu >= THERMAL_CUTOFF_THZ
+        tt = t[:, None, None]
+        x = H_OVER_KB_K_PER_THZ * torch.where(kept, nu, 1.0)[None] / torch.where(tt > 0, tt, 1.0)
+        em = torch.exp(-x)
+        cv = torch.where(kept[None] & (tt > 0), KB * x * x * em / torch.expm1(-x) ** 2, 0.0)  # [T, N, 3n]
+        use = kept[None] & (gamma > 0)
+        tau = torch.where(use, 1.0 / (4 * math.pi * torch.where(use, gamma, 1.0)), 0.0)
+        vv = v[:, :, :, None] * v[:, :, None, :]  # [N, 3n, 3, 3]
+        vol = abs(float(np.linalg.det(self.cell.prim_lattice)))
+        kappa = torch.einsum("tqm,qmab->tab", cv * tau, vv) * (KAPPA_W_PER_MK / (nu.shape[0] * vol))
+        return {"temperatures": temps, "kappa": kappa.cpu().numpy(), "frequencies": nu.cpu().numpy(),
+                "linewidths": gamma.cpu().numpy(), "group_velocities": v.cpu().numpy(),
+                "heat_capacity": cv.cpu().numpy(), "n_imaginary": n_imaginary,
+                "n_zero_linewidth": (kept[None] & ~(gamma > 0)).sum(dim=(1, 2)).cpu().numpy()}

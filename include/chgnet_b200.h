@@ -626,6 +626,34 @@ int chg_structure_factors(const double* freqs, const double* eigvecs, const doub
 int chg_broadened_spectrum(const double* freqs, const double* weights, int32_t n_q, int32_t n_modes, int32_t n_t,
                            int64_t row0, int32_t group_size, int64_t n_groups, const double* omega, int32_t n_freq,
                            double sigma, double* work, int64_t work_doubles, double* out, void* stream);
+/* Three-phonon interaction strengths for one target q (mesh index) of the full Gamma-centred mesh n1 x n2 x n3 and the
+ * q1 (mesh indices q1_idx [n_q1]); q2 = q - q1 on the mesh, G = q - q1 - q2:
+ *   R[k a][k' b][k'' c] = e^{-2 pi i G.x_k} sum_{j' in k', j'' in k''} fc3[k][j'][j''][a][b][c] rho_kj'(q1) rho_kj''(q2),
+ *   out [n_q1][3n][3n][3n] = P[l][l1][l2] = C^3 / (36 N nu nu1 nu2) |sum e*_l(q) e_l1(q1) e_l2(q2) R / sqrt(m m' m'')|^2
+ * in eV^2, N = n1 n2 n3, C = h / (8 pi^2 amu THz) in A^2, P = 0 when nu, nu1 or nu2 is below cutoff_thz.  fc3
+ * [n_prim][n_super][n_super][3][3][3] eV/A^3 (fp64); img_ptr, img_vec, s2p and inv_sqrt_m as chg_dynamical_matrices,
+ * rho_kj the image average (1/m_kj) sum e^{2 pi i q.v}; the supercell must be atom-major (s2p[j] = j / (n_super /
+ * n_prim)); frac [n_prim][3] fractional positions x_k; freqs [n1 n2 n3][3n] THz; eigvecs [n1 n2 n3][mode][3n]
+ * complex128, mode-major.  work: at least 4 n_q1 (n_prim n_super + (3 n_prim)^3) doubles of scratch (work_doubles).
+ * All fp64, no atomics: deterministic.                                                                            */
+int chg_phonon_interaction(const double* fc3, const int32_t* img_ptr, const double* img_vec, const int32_t* s2p,
+                           const double* inv_sqrt_m, const double* frac, int32_t n_prim, int32_t n_super, int32_t n1,
+                           int32_t n2, int32_t n3, const double* freqs, const double* eigvecs, int32_t target,
+                           const int32_t* q1_idx, int32_t n_q1, double cutoff_thz, double* work,
+                           int64_t work_doubles, double* out, void* stream);
+/* Imaginary self-energy (half width, THz) of the modes of one target q: gamma [n_t][n_band] +=
+ *   18 pi / h^2 sum over the q1 of the call and (l1, l2) of P [(1 + n1 + n2) g2 + (n1 - n2) (g1+ - g1-)]
+ * at w = omega[l] (the target's band frequencies; 0 where omega[l] < cutoff_thz), h in eV/THz, P = p [n_q1][l][l1][l2]
+ * as chg_phonon_interaction writes it, n = 1 / expm1(h nu / k_B T) (0 at T = 0) and g2, g1+, g1- the linear-tetrahedron
+ * weights (tetrahedra as chg_joint_dos) with which vertex q1 enters the averages of d(w - nu1 - nu2), d(w + nu1 - nu2)
+ * and d(w - nu1 + nu2), items with nu1 or nu2 below cutoff_thz left out.  freqs [n1 n2 n3][n_band] THz; temperatures
+ * [n_t] K.  work: at least 2 n_q1 n_band^3 + CHG_ISE_MAX_CHUNKS n_t n_band doubles (work_doubles).  Deterministic:
+ * per-block partial sums added in a fixed order, no atomics.                                                        */
+#define CHG_ISE_MAX_CHUNKS 64
+int chg_imag_self_energy(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                         const int32_t* tetrahedra, int32_t target, const double* omega, const int32_t* q1_idx,
+                         int32_t n_q1, const double* p, const double* temperatures, int32_t n_t, double cutoff_thz,
+                         double* work, int64_t work_doubles, double* gamma, void* stream);
 
 #ifdef __cplusplus
 }
