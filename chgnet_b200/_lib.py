@@ -76,6 +76,7 @@ SIGNATURES: dict[str, list] = {
     "chg_broadened_spectrum": [P, P, I, I, I, I64, I, I64, P, I, D, P, I64, P, P],
     "chg_phonon_interaction": [P, P, P, P, P, P, I, I, I, I, I, P, P, I, P, I, D, P, I64, P, P],
     "chg_imag_self_energy": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
+    "chg_collision_rows": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -114,6 +115,12 @@ def ise_scratch_doubles(n_q1, n_band, n_t):
     """The scratch of one ``chg_imag_self_energy`` call: the tetrahedron weights [n_q1, n_band^3, 2] and
     ``ISE_MAX_CHUNKS`` chunks of [n_t, n_band] partial sums."""
     return 2 * n_q1 * n_band**3 + ISE_MAX_CHUNKS * n_t * n_band
+
+
+def collision_scratch_doubles(n_q1, n_band):
+    """The scratch of one ``chg_collision_rows`` call: the tetrahedron weights g2, g1+ and g1-, three [n_q1, n_band^3]
+    planes."""
+    return 3 * n_q1 * n_band**3
 
 _lib = None
 
@@ -600,6 +607,22 @@ class CudaKernels:
         work = torch.empty(max(1, ise_scratch_doubles(n_q1, nb, n_t)), dtype=torch.float64, device=freqs.device)
         self._call("chg_imag_self_energy", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), _p(q1),
                    n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(gamma))
+
+    def collision_rows(self, freqs, mesh, tetrahedra, target, omega, q1, p, temperatures, cutoff_thz, out):
+        """out [4, T, n_band, n1 n2 n3, n_band] fp64: the collision-matrix role sums (1/ps) of the target's modes with
+        the vertices q1 (mesh indices ``q1`` [n_q1] int32), written at out[:, :, :, q1] and nowhere else
+        (``chg_collision_rows``, DESIGN.md section 12.8); the other arguments as ``imag_self_energy``."""
+        self._chk(freqs, tetrahedra, omega, q1, p, temperatures, out)
+        n1, n2, n3 = _mesh_args("collision_rows", mesh, freqs, tetrahedra, "freqs, omega, p, temperatures and out",
+                                (freqs, omega, p, temperatures, out))
+        nb, n_q1, n_t = freqs.shape[1], q1.shape[0], temperatures.shape[0]
+        if (q1.dtype != torch.int32 or q1.dim() != 1 or tuple(omega.shape) != (nb,) or temperatures.dim() != 1
+                or tuple(p.shape) != (n_q1, nb, nb, nb) or tuple(out.shape) != (4, n_t, nb, n1 * n2 * n3, nb)):
+            raise ChgnetB200Error(f"collision_rows: q1 must be int32 [Q1], omega [{nb}], p [Q1, {nb}, {nb}, {nb}], "
+                                  f"temperatures [T] and out [4, T, {nb}, {n1 * n2 * n3}, {nb}]")
+        work = torch.empty(max(1, collision_scratch_doubles(n_q1, nb)), dtype=torch.float64, device=freqs.device)
+        self._call("chg_collision_rows", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), _p(q1),
+                   n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(out))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

@@ -900,6 +900,9 @@ __device__ __forceinline__ double corner_weight(const double (&wt)[4], int p) {
   return p == 0 ? wt[0] : (p == 1 ? wt[1] : (p == 2 ? wt[2] : wt[3]));
 }
 
+// SPLIT false: wts [q1][l][l1][l2] of (g2, g1+ - g1-) (chg_imag_self_energy).  SPLIT true: wts holds three planes
+// of doubles [3][n_q1][l][l1][l2], g2, g1+ and g1- (chg_collision_rows).
+template <bool SPLIT>
 __global__ void __launch_bounds__(ISE_THREADS)
 ise_weights_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
                    const int32_t* __restrict__ tet, int target, const double* __restrict__ omega,
@@ -909,7 +912,17 @@ ise_weights_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2,
   if (i >= (int64_t)n_q1 * nb2) return;
   const int q1l = (int)(i / nb2), l1 = (int)((i / n_band) % n_band), l2 = (int)(i % n_band);
   double2* w_out = wts + (size_t)q1l * n_band * nb2 + (size_t)(i % nb2);
-  for (int l = 0; l < n_band; ++l) w_out[(size_t)l * nb2] = make_double2(0.0, 0.0);
+  double* w_plane = reinterpret_cast<double*>(wts) + (size_t)q1l * n_band * nb2 + (size_t)(i % nb2);
+  const size_t plane = (size_t)n_q1 * n_band * nb2;
+  if constexpr (SPLIT) {
+    for (int l = 0; l < n_band; ++l) {
+      w_plane[(size_t)l * nb2] = 0.0;
+      w_plane[plane + (size_t)l * nb2] = 0.0;
+      w_plane[2 * plane + (size_t)l * nb2] = 0.0;
+    }
+  } else {
+    for (int l = 0; l < n_band; ++l) w_out[(size_t)l * nb2] = make_double2(0.0, 0.0);
+  }
   const int q1 = __ldg(q1_idx + q1l);
   const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
   const auto nu_pair = [&](int a, int b, int c, double& nu1, double& nu2) {
@@ -955,7 +968,7 @@ ise_weights_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2,
       if (!(w >= cutoff)) continue;
       const bool h2 = w >= e2[0] && w < e2[3], hp = w >= ep[0] && w < ep[3], hm = w >= em[0] && w < em[3];
       if (!(h2 || hp || hm)) continue;
-      double n, g, wt[4], d2 = 0.0, d1 = 0.0;
+      double n, g, wt[4], d2 = 0.0, d1 = 0.0, dm = 0.0;
       if (h2) {
         tetra_weights(w, e2, n, g, wt);
         d2 = corner_weight(wt, p2);
@@ -966,12 +979,23 @@ ise_weights_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2,
       }
       if (hm) {
         tetra_weights(w, em, n, g, wt);
-        d1 -= corner_weight(wt, pm);
+        if constexpr (SPLIT) {
+          dm = corner_weight(wt, pm);
+        } else {
+          d1 -= corner_weight(wt, pm);
+        }
       }
-      double2 acc = w_out[(size_t)l * nb2];
-      acc.x = fma(d2, 1.0 / 6.0, acc.x);
-      acc.y = fma(d1, 1.0 / 6.0, acc.y);
-      w_out[(size_t)l * nb2] = acc;
+      if constexpr (SPLIT) {
+        double* o = w_plane + (size_t)l * nb2;
+        o[0] = fma(d2, 1.0 / 6.0, o[0]);
+        o[plane] = fma(d1, 1.0 / 6.0, o[plane]);
+        o[2 * plane] = fma(dm, 1.0 / 6.0, o[2 * plane]);
+      } else {
+        double2 acc = w_out[(size_t)l * nb2];
+        acc.x = fma(d2, 1.0 / 6.0, acc.x);
+        acc.y = fma(d1, 1.0 / 6.0, acc.y);
+        w_out[(size_t)l * nb2] = acc;
+      }
     }
   }
 }
@@ -1025,6 +1049,83 @@ ise_accumulate_kernel(const double* __restrict__ freqs, int n_band, int n1, int 
     double s = 0.0;
     for (int i = 0; i < ISE_THREADS; ++i) s += red[i][threadIdx.x];
     work[((size_t)blockIdx.x * n_t + t0 + threadIdx.x) * n_band + l] = s * (18.0 * 3.141592653589793 / (ISE_H * ISE_H));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Collision-matrix rows.  For the target q, a vertex q1 of the call, q2 = q - q1 and s(nu) = sinh(h nu / 2 k T), the
+// four role sums of (l, b), each times 2 pi 18 pi / h^2:
+//   A = -sum_k P[l][b][k] (g2 + g1-)[l][b][k] / s(nu2_k)    B = +sum_k P[l][b][k] g1+[l][b][k] / s(nu2_k)
+//   C = -sum_k P[l][k][b] (g2 + g1+)[l][k][b] / s(nu1_k)    D = +sum_k P[l][k][b] g1-[l][k][b] / s(nu1_k)
+// (nu1 at q1, nu2 at q2) go to out[role][t][l][q1][b], q1 the mesh index.  collision_rows_kernel: block (q1 of the
+// call, tile of COLL_T_TILE temperatures); it stages 1 / s(nu1) and 1 / s(nu2) of the tile in shared memory (0 below
+// the cutoff and at T = 0), then each thread owns whole (l, b) pairs and sums k in ascending order for all four roles
+// and the tile's temperatures.  Every output element is written by one thread, no atomics.
+constexpr int COLL_THREADS = 256;
+constexpr int COLL_T_TILE = 4;
+constexpr int COLL_MAX_BAND = 768;  // the staged 1 / s: 2 x COLL_T_TILE x n_band doubles within 48 KiB
+
+__global__ void __launch_bounds__(COLL_THREADS)
+collision_rows_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3, int target,
+                      const int32_t* __restrict__ q1_idx, int n_q1, const double* __restrict__ p,
+                      const double* __restrict__ wts, const double* __restrict__ temps, int n_t, double cutoff,
+                      double* __restrict__ out) {
+  extern __shared__ double inv_s[];  // [2][COLL_T_TILE][n_band]: side 0 at q1, side 1 at q2
+  const int q1l = blockIdx.x, t0 = blockIdx.y * COLL_T_TILE;
+  const int t_here = min(COLL_T_TILE, n_t - t0);
+  const int n_mesh = n1 * n2 * n3;
+  const int q1 = __ldg(q1_idx + q1l);
+  const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
+  int a2 = ta - q1 / (n2 * n3), b2 = tb - (q1 / n3) % n2, c2 = tc - q1 % n3;
+  a2 += a2 < 0 ? n1 : 0;
+  b2 += b2 < 0 ? n2 : 0;
+  c2 += c2 < 0 ? n3 : 0;
+  const int q2 = (a2 * n2 + b2) * n3 + c2;
+  for (int i = threadIdx.x; i < 2 * COLL_T_TILE * n_band; i += COLL_THREADS) {
+    const int side = i / (COLL_T_TILE * n_band), t = (i / n_band) % COLL_T_TILE, k = i % n_band;
+    const double nu = __ldg(freqs + (int64_t)(side == 0 ? q1 : q2) * n_band + k);
+    const double temp = t < t_here ? __ldg(temps + t0 + t) : 0.0;
+    inv_s[i] = nu >= cutoff && temp > 0.0 ? 1.0 / sinh(0.5 * TD_H_OVER_K * nu / temp) : 0.0;
+  }
+  __syncthreads();
+  const int64_t nb2 = (int64_t)n_band * n_band, n_w = (int64_t)n_q1 * n_band * nb2;
+  const double* pq = p + (size_t)q1l * n_band * nb2;
+  const double* g2 = wts + (size_t)q1l * n_band * nb2;
+  const double* gp = g2 + n_w;
+  const double* gm = g2 + 2 * n_w;
+  const double scale = 2.0 * 3.141592653589793 * (18.0 * 3.141592653589793 / (ISE_H * ISE_H));
+  for (int64_t i = threadIdx.x; i < nb2; i += COLL_THREADS) {
+    const int l = (int)(i / n_band), b = (int)(i % n_band);
+    double ra[COLL_T_TILE], rb[COLL_T_TILE], rc[COLL_T_TILE], rd[COLL_T_TILE];
+#pragma unroll
+    for (int t = 0; t < COLL_T_TILE; ++t) ra[t] = rb[t] = rc[t] = rd[t] = 0.0;
+    const size_t row = (size_t)l * nb2 + (size_t)b * n_band;  // [l][b][k]
+    const size_t col = (size_t)l * nb2 + b;                    // [l][k][b] at k = 0
+    for (int k = 0; k < n_band; ++k) {
+      const double pr = __ldg(pq + row + k), pc = __ldg(pq + col + (size_t)k * n_band);
+      // P is 0 wherever a mode is below the cutoff; the weights are 0 off the delta functions' support
+      const double x2 = pr * (__ldg(g2 + row + k) + __ldg(gm + row + k)), xp = pr * __ldg(gp + row + k);
+      const double y2 = pc * (__ldg(g2 + col + (size_t)k * n_band) + __ldg(gp + col + (size_t)k * n_band));
+      const double ym = pc * __ldg(gm + col + (size_t)k * n_band);
+#pragma unroll
+      for (int t = 0; t < COLL_T_TILE; ++t) {
+        const double s2 = inv_s[(COLL_T_TILE + t) * n_band + k], s1 = inv_s[t * n_band + k];
+        ra[t] = fma(x2, s2, ra[t]);
+        rb[t] = fma(xp, s2, rb[t]);
+        rc[t] = fma(y2, s1, rc[t]);
+        rd[t] = fma(ym, s1, rd[t]);
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < COLL_T_TILE; ++t) {
+      if (t >= t_here) break;
+      const size_t o = (((size_t)(t0 + t) * n_band + l) * n_mesh + q1) * n_band + b;
+      const size_t role = (size_t)n_t * n_band * n_mesh * n_band;
+      out[o] = -scale * ra[t];
+      out[role + o] = scale * rb[t];
+      out[2 * role + o] = -scale * rc[t];
+      out[3 * role + o] = scale * rd[t];
+    }
   }
 }
 
@@ -1251,7 +1352,7 @@ extern "C" int chg_imag_self_energy(const double* freqs, int32_t n_band, int32_t
   double2* wts = reinterpret_cast<double2*>(work);
   double* partial = work + n_w;
   cudaStream_t st = as_stream(stream);
-  ise_weights_kernel<<<(unsigned)((n_items + ISE_THREADS - 1) / ISE_THREADS), ISE_THREADS, 0, st>>>(
+  ise_weights_kernel<false><<<(unsigned)((n_items + ISE_THREADS - 1) / ISE_THREADS), ISE_THREADS, 0, st>>>(
       freqs, n_band, n1, n2, n3, tetrahedra, target, omega, q1_idx, n_q1, cutoff_thz, wts);
   count_launch();
   // enough chunks for about 4 096 blocks in all, at most CHG_ISE_MAX_CHUNKS and one pass of the block's threads each
@@ -1262,5 +1363,29 @@ extern "C" int chg_imag_self_energy(const double* freqs, int32_t n_band, int32_t
   ise_accumulate_kernel<<<dim3(chunks, (unsigned)n_band, (unsigned)t_tiles), ISE_THREADS, 0, st>>>(
       freqs, n_band, n1, n2, n3, target, omega, q1_idx, n_q1, p, wts, temperatures, n_t, cutoff_thz, partial);
   CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_t * n_band, AccumulateStore{gamma}, st));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_collision_rows(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                                  const int32_t* tetrahedra, int32_t target, const double* omega, const int32_t* q1_idx,
+                                  int32_t n_q1, const double* p, const double* temperatures, int32_t n_t,
+                                  double cutoff_thz, double* work, int64_t work_doubles, double* out, void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_q1 >= 0 && n_t >= 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 * std::max(n_band, 1) < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(target >= 0 && (int64_t)target < (int64_t)n1 * n2 * n3, "target outside the mesh");
+  CHG_CHECK_ARG(n_band <= COLL_MAX_BAND, "too many bands (at most 768)");
+  if (n_band == 0 || n_q1 == 0 || n_t == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && tetrahedra && omega && q1_idx && p && temperatures && work && out, "null pointer");
+  const int64_t n_items = (int64_t)n_q1 * n_band * n_band;
+  CHG_CHECK_ARG(work_doubles >= 3 * n_items * n_band, "work holds less than 3 n_q1 n_band^3 doubles");
+  const int64_t t_tiles = ((int64_t)n_t + COLL_T_TILE - 1) / COLL_T_TILE;
+  CHG_CHECK_ARG(t_tiles <= 65535, "too many temperatures");
+  cudaStream_t st = as_stream(stream);
+  ise_weights_kernel<true><<<(unsigned)((n_items + ISE_THREADS - 1) / ISE_THREADS), ISE_THREADS, 0, st>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, target, omega, q1_idx, n_q1, cutoff_thz, reinterpret_cast<double2*>(work));
+  count_launch();
+  const size_t smem = sizeof(double) * 2 * COLL_T_TILE * n_band;
+  collision_rows_kernel<<<dim3((unsigned)n_q1, (unsigned)t_tiles), COLL_THREADS, smem, st>>>(
+      freqs, n_band, n1, n2, n3, target, q1_idx, n_q1, p, work, temperatures, n_t, cutoff_thz, out);
   CHG_LAUNCH_END();
 }

@@ -340,6 +340,15 @@ def _degenerate_average(gamma: torch.Tensor, nu: torch.Tensor) -> torch.Tensor:
     return torch.where(nu >= THERMAL_CUTOFF_THZ, (sums / counts)[:, sid], 0.0)
 
 
+def _degenerate_operators(nu: torch.Tensor) -> torch.Tensor:
+    """[N, 3n, 3n]: per row of nu [N, 3n] the matrix that averages over its degenerate sets (the grouping of
+    ``_degenerate_average``), A[q, i, j] = 1 / |set| when modes i and j of q share a set, else 0 (symmetric)."""
+    gap = (nu[:, 1:] - nu[:, :-1]).abs() >= DEGENERACY_THZ
+    sid = torch.cat([torch.zeros(nu.shape[0], 1, dtype=torch.long, device=nu.device), gap.long().cumsum(1)], 1)
+    same = (sid[:, :, None] == sid[:, None, :]).to(nu.dtype)
+    return same / same.sum(-1, keepdim=True)
+
+
 def _gaussian_sigma(width) -> float | None:
     """The standard deviation (THz) of a Gaussian of FWHM ``width``, width / (2 sqrt(2 ln 2)); None for None, and
     ValueError unless it is finite and > 0."""
@@ -388,6 +397,9 @@ class Phonons:
     # linewidths and thermal_conductivity: q1 per chg_phonon_interaction / chg_imag_self_energy call keep P, the
     # tetrahedron weights and both calls' scratch below this many bytes
     ph3_chunk_bytes = 1 << 28
+    # thermal_conductivity_lbte: the collision matrices of all temperatures are built in one pass over the targets when
+    # they fit in this many bytes (fp64, M^2 per temperature), else in groups of temperatures
+    lbte_matrix_bytes = 8 << 30
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, fc3=None, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -882,7 +894,18 @@ class Phonons:
         nb = 3 * n_prim
         per_q1 = 8 * (nb**3 + ph3_scratch_doubles(1, n_prim, len(self.s2p)) + ise_scratch_doubles(1, nb, 0))
         fixed = 8 * ise_scratch_doubles(0, nb, n_t)
+        # chg_collision_rows' scratch, collision_scratch_doubles(1, nb) = 3 nb^3 per q1, is less than the
+        # chg_phonon_interaction scratch counted here and is allocated after that has been released, so this chunk
+        # also bounds thermal_conductivity_lbte (and stays the chunk of thermal_conductivity, whose Gamma it shares)
         return int(max(1, min(65535, (self.ph3_chunk_bytes - fixed) // per_q1)))
+
+    def _interaction_chunks(self, mesh, nu, e, target: int, chunk: int):
+        """Yields ``(q1, P)`` per chunk of ``chunk`` q1 of the mesh, in mesh order: the mesh indices (int32, device) and
+        their interaction strengths with the mesh index ``target``."""
+        n_mesh = nu.shape[0]
+        for s in range(0, n_mesh, chunk):
+            q1 = torch.arange(s, min(s + chunk, n_mesh), dtype=torch.int32, device=self.device)
+            yield q1, self._interactions(mesh, nu, e, target, q1)
 
     def _interactions(self, mesh, nu, e, target: int, q1: torch.Tensor) -> torch.Tensor:
         """P [len(q1), 3n, 3n, 3n] (eV^2) of the mesh index ``target`` with the mesh indices ``q1`` (int32, device)."""
@@ -896,13 +919,9 @@ class Phonons:
     def _target_linewidths(self, mesh, nu, e, tets, t, target: int) -> torch.Tensor:
         """Gamma [T, 3n] (THz) of the modes of the mesh index ``target``: P and its contribution to Gamma per chunk of
         q1 (``_q1_chunk``, chunks in mesh order), then averaged over degenerate sets."""
-        n_mesh, nb = nu.shape
-        gamma = torch.zeros(len(t), nb, dtype=torch.float64, device=self.device)
+        gamma = torch.zeros(len(t), nu.shape[1], dtype=torch.float64, device=self.device)
         omega = nu[target].contiguous()
-        chunk = self._q1_chunk(len(t))
-        for s in range(0, n_mesh, chunk):
-            q1 = torch.arange(s, min(s + chunk, n_mesh), dtype=torch.int32, device=self.device)
-            p = self._interactions(mesh, nu, e, target, q1)
+        for q1, p in self._interaction_chunks(mesh, nu, e, target, self._q1_chunk(len(t))):
             self.kernels.imag_self_energy(nu, mesh, tets, int(target), omega, q1, p, t, THERMAL_CUTOFF_THZ, gamma)
         return _degenerate_average(gamma, omega)
 
@@ -972,7 +991,12 @@ class Phonons:
         dev = self.device
         t = torch.as_tensor(temps).to(dev)
         gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, i) for i in range(nu.shape[0])], 1)
-        v = torch.as_tensor(self.group_velocities(gamma_mesh(mesh))).to(dev)  # [N, 3n, 3]
+        return self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+
+    def _rta_conductivity(self, mesh, nu, gamma, t, temps, n_imaginary) -> dict:
+        """``thermal_conductivity``'s result from the mesh frequencies nu [N, 3n] and the linewidths gamma [T, N, 3n]
+        at the temperatures t (device) and temps (array)."""
+        v = torch.as_tensor(self.group_velocities(gamma_mesh(mesh))).to(self.device)  # [N, 3n, 3]
         kept = nu >= THERMAL_CUTOFF_THZ
         tt = t[:, None, None]
         x = H_OVER_KB_K_PER_THZ * torch.where(kept, nu, 1.0)[None] / torch.where(tt > 0, tt, 1.0)
@@ -987,3 +1011,139 @@ class Phonons:
                 "linewidths": gamma.cpu().numpy(), "group_velocities": v.cpu().numpy(),
                 "heat_capacity": cv.cpu().numpy(), "n_imaginary": n_imaginary,
                 "n_zero_linewidth": (kept[None] & ~(gamma > 0)).sum(dim=(1, 2)).cpu().numpy()}
+
+    def _collision_passes(self, mesh, nu, e, tets, t, groups):
+        """One pass over the targets per group of temperature indices in ``groups`` (P remade per pass).  Yields
+        ``(group, target, gamma, rows)``: gamma [T, 3n] the degenerate-averaged linewidths of the target at all the
+        temperatures t, from the first pass only (None after; made exactly as ``thermal_conductivity`` makes them), and
+        rows [len(group), 3n, N, 3n] the target's rows of S, row l against column (c, l'), before any averaging:
+
+            S[q l][c l'] = R_A[c] + R_B[-c] + R_C[q - c] + R_D[q + c]   (R by vertex q1, ``chg_collision_rows``)"""
+        n_mesh, nb = nu.shape
+        dev = self.device
+        size = np.array(mesh)
+        coords = np.stack(np.unravel_index(np.arange(n_mesh), mesh), 1)
+        flat = lambda c: torch.as_tensor(np.ravel_multi_index(tuple((c % size).T), mesh)).to(dev)  # noqa: E731
+        neg = flat(-coords)
+        chunk = self._q1_chunk(len(t))
+        for gi, group in enumerate(groups):
+            tg = t[torch.as_tensor(group, dtype=torch.long).to(dev)].contiguous()
+            r = torch.zeros(4, len(group), nb, n_mesh, nb, dtype=torch.float64, device=dev)
+            for target in range(n_mesh):
+                gamma = torch.zeros(len(t), nb, dtype=torch.float64, device=dev) if gi == 0 else None
+                omega = nu[target].contiguous()
+                for q1, p in self._interaction_chunks(mesh, nu, e, target, chunk):
+                    if gamma is not None:
+                        self.kernels.imag_self_energy(nu, mesh, tets, target, omega, q1, p, t, THERMAL_CUTOFF_THZ, gamma)
+                    if len(group):
+                        self.kernels.collision_rows(nu, mesh, tets, target, omega, q1, p, tg, THERMAL_CUTOFF_THZ, r)
+                rows = r[0] + r[1][:, :, neg] + r[2][:, :, flat(coords[target] - coords)]
+                rows = rows + r[3][:, :, flat(coords[target] + coords)]
+                yield group, target, (None if gamma is None else _degenerate_average(gamma, omega)), rows
+
+    def _collision_matrix(self, mesh, temperatures):
+        """For the tests: S [T, N 3n, N 3n] (1/ps) before degenerate averaging and symmetrisation, rows and columns in
+        mesh-major (q, l) order, the degenerate-averaged linewidths [T, N, 3n] (THz) and the kept mask [T, N 3n] of
+        ``thermal_conductivity_lbte`` (nu >= the cutoff, the Gamma rule and Gamma > 0)."""
+        mesh, nu, e, _, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        n_mesh, nb = nu.shape
+        t = torch.as_tensor(temps).to(self.device)
+        s = torch.zeros(len(temps), n_mesh * nb, n_mesh * nb, dtype=torch.float64, device=self.device)
+        gamma = torch.zeros(len(temps), n_mesh, nb, dtype=torch.float64, device=self.device)
+        for _, target, g, rows in self._collision_passes(mesh, nu, e, tets, t, [list(range(len(temps)))]):
+            s[:, target * nb : (target + 1) * nb] = rows.reshape(len(temps), nb, -1)
+            gamma[:, target] = g
+        kept = (nu >= THERMAL_CUTOFF_THZ)[None] & (gamma > 0)
+        return s, gamma, kept.reshape(len(temps), -1)
+
+    def thermal_conductivity_lbte(self, mesh, temperatures, *, pinv_cutoff=1e-8) -> dict:
+        """Lattice thermal conductivity (W/(m K)) from the direct solution of the linearised phonon Boltzmann equation
+        (Chaput, PRL 110, 265506 (2013)) on the full Gamma-centred ``mesh``, every mesh point a target (DESIGN.md
+        section 12.8).  The collision matrix, symmetrised and in 1/ps,
+
+            Omega = diag(4 pi Gamma) + S,   S[q l][c] = sum over the processes of mode q l with mode c of
+                    u_q u_c 2 pi 18 pi / h^2 P g / sinh(h nu_o / 2 k T)
+
+        (g the tetrahedron weight of the process, o its third mode, u = +1 for the mode alone on its side of the
+        process, -1 for the other two), averaged over degenerate sets (rows, then columns) and made symmetric, keeps
+        the modes ``thermal_conductivity`` keeps (nu >= ``THERMAL_CUTOFF_THZ``, not the three acoustic modes at Gamma,
+        Gamma > 0).  With Omega = U diag(eta) U^T and X = sqrt(C) v per mode,
+
+            kappa = 1 / (N V0) sum over eta_k > pinv_cutoff of (U^T X)_k (x) (U^T X)_k / eta_k
+
+        which is ``thermal_conductivity``'s kappa when S = 0.  Eigenvalues <= ``pinv_cutoff`` (1/ps; the energy mode
+        near 0 and small negative ones) are left out and counted.  At T = 0 kappa is 0 and no matrix is built.
+
+        Returns ``temperatures``, ``kappa`` and ``kappa_rta`` [T, 3, 3] (the latter bitwise ``thermal_conductivity``'s
+        kappa), per mode ``frequencies``, ``linewidths``, ``group_velocities`` and ``heat_capacity`` as
+        ``thermal_conductivity``, ``n_imaginary``, ``n_zero_linewidth``, ``n_dropped`` [T] (eigenvalues <=
+        pinv_cutoff) and ``min_eigenvalue`` [T] (1/ps, NaN where no matrix was built).  The matrices of all
+        temperatures above 0 are built in one pass over the targets when n_t M^2 8 bytes fit in ``lbte_matrix_bytes``
+        (M: the modes at or above the cutoff), else in groups of temperatures with P remade per group; ValueError
+        with the bytes needed when one temperature alone does not fit.  Needs ``force_constants3``, else ValueError;
+        bad temperatures and a ``pinv_cutoff`` that is not finite and >= 0 raise ValueError."""
+        if temperatures is None:
+            raise ValueError("thermal_conductivity_lbte needs temperatures")
+        cutoff = float(pinv_cutoff)
+        if not (math.isfinite(cutoff) and cutoff >= 0):
+            raise ValueError(f"pinv_cutoff must be finite and non-negative, got {pinv_cutoff!r}")
+        mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        n_mesh, nb = nu.shape
+        dev, f64 = self.device, torch.float64
+        t = torch.as_tensor(temps).to(dev)
+        cols = torch.nonzero((nu >= THERMAL_CUTOFF_THZ).reshape(-1))[:, 0]
+        m0 = len(cols)
+        hot = [int(i) for i in np.nonzero(temps > 0)[0]]
+        per_t = 8 * m0 * m0
+        if hot and per_t > self.lbte_matrix_bytes:
+            raise ValueError(f"thermal_conductivity_lbte needs {per_t} bytes for the collision matrix of one "
+                             f"temperature ({m0} modes), more than lbte_matrix_bytes = {self.lbte_matrix_bytes}")
+        per_group = max(1, self.lbte_matrix_bytes // max(per_t, 1))
+        groups = [hot[i : i + per_group] for i in range(0, len(hot), per_group)] or [[]]
+        avg = _degenerate_operators(nu)  # [N, 3n, 3n]
+        pos = torch.full((n_mesh * nb,), -1, dtype=torch.long, device=dev)
+        pos[cols] = torch.arange(m0, device=dev)
+        gamma = torch.zeros(len(temps), n_mesh, nb, dtype=f64, device=dev)
+        kappa = torch.zeros(len(temps), 3, 3, dtype=f64, device=dev)
+        n_dropped = np.zeros(len(temps), dtype=np.int64)
+        min_eig = np.full(len(temps), np.nan)
+        res = x = s = None
+        for group, target, g, rows in self._collision_passes(mesh, nu, e, tets, t, groups):
+            if target == 0:
+                s = torch.zeros(len(group), m0, m0, dtype=f64, device=dev)
+            if g is not None:
+                gamma[:, target] = g
+            here = cols[(cols >= target * nb) & (cols < (target + 1) * nb)]
+            for j in range(len(group)):  # per temperature, so that the grouping cannot change a bit
+                rj = torch.einsum("ij,jcl->icl", avg[target], rows[j])
+                rj = torch.einsum("icl,clk->ick", rj, avg).reshape(nb, -1)
+                s[j, pos[here]] = rj[here - target * nb][:, cols]
+            if target < n_mesh - 1:
+                continue
+            if res is None:  # the end of the first pass: every Gamma is known
+                res = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+                x = (torch.as_tensor(res["heat_capacity"]).to(dev).sqrt()[..., None]
+                     * torch.as_tensor(res["group_velocities"]).to(dev)[None]).reshape(len(temps), -1, 3)[:, cols]
+            for j, ti in enumerate(group):
+                kappa[ti], n_dropped[ti], min_eig[ti] = self._lbte_solve(s[j], gamma[ti].reshape(-1)[cols], x[ti],
+                                                                         cutoff)
+            s = None
+        vol = abs(float(np.linalg.det(self.cell.prim_lattice)))
+        res["kappa_rta"] = res["kappa"]
+        res["kappa"] = (kappa * (KAPPA_W_PER_MK / (n_mesh * vol))).cpu().numpy()
+        res["n_dropped"], res["min_eigenvalue"] = n_dropped, min_eig
+        return res
+
+    @staticmethod
+    def _lbte_solve(s, gamma, x, cutoff):
+        """(sum over eta > cutoff of (U^T x)_k (x) (U^T x)_k / eta_k [3, 3], the count of eta <= cutoff, min eta) for
+        Omega = diag(4 pi gamma) + (s + s^T) / 2 restricted to gamma > 0; s [M, M] averaged, gamma [M], x [M, 3]."""
+        omega = (s + s.mT) * 0.5
+        omega.diagonal().add_(4 * math.pi * gamma)
+        keep = gamma > 0
+        omega = omega[keep][:, keep]
+        eta, u = torch.linalg.eigh(omega)
+        y = u.mT @ x[keep]
+        use = eta > cutoff
+        k = (y[use] / eta[use, None]).mT @ y[use]
+        return k, int((~use).sum()), float(eta.min()) if len(eta) else math.nan

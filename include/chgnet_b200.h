@@ -654,6 +654,20 @@ int chg_imag_self_energy(const double* freqs, int32_t n_band, int32_t n1, int32_
                          const int32_t* tetrahedra, int32_t target, const double* omega, const int32_t* q1_idx,
                          int32_t n_q1, const double* p, const double* temperatures, int32_t n_t, double cutoff_thz,
                          double* work, int64_t work_doubles, double* gamma, void* stream);
+/* Collision-matrix role sums of one target q (linearised phonon Boltzmann equation, DESIGN.md section 12.8).  For each
+ * q1 of the call (q2 = q - q1 on the mesh), band l of q and band b, with s(nu) = sinh(h nu / 2 k_B T) and K = 18 pi / h^2:
+ *   out[0][t][l][q1][b] = -2 pi K sum_k P[l][b][k] (g2 + g1-) / s(nu(q2, k))   (to column (q1, b))
+ *   out[1][t][l][q1][b] = +2 pi K sum_k P[l][b][k] g1+ / s(nu(q2, k))          (to column (-q1, b))
+ *   out[2][t][l][q1][b] = -2 pi K sum_k P[l][k][b] (g2 + g1+) / s(nu(q1, k))   (to column (q2, b))
+ *   out[3][t][l][q1][b] = +2 pi K sum_k P[l][k][b] g1- / s(nu(q1, k))          (to column (-q2, b))
+ * in 1/ps, out [4][n_t][n_band][n1 n2 n3][n_band] indexed by the mesh index of q1 (only the q1 of the call are
+ * written), P, the weights g2, g1+, g1- and the other arguments as chg_imag_self_energy; 1 / s = 0 below cutoff_thz
+ * and at T = 0.  n_band <= 768.  work: at least 3 n_q1 n_band^3 doubles (work_doubles).  Every element is written by
+ * one thread, k summed in ascending order, no atomics: deterministic.                                             */
+int chg_collision_rows(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                       const int32_t* tetrahedra, int32_t target, const double* omega, const int32_t* q1_idx,
+                       int32_t n_q1, const double* p, const double* temperatures, int32_t n_t, double cutoff_thz,
+                       double* work, int64_t work_doubles, double* out, void* stream);
 
 #ifdef __cplusplus
 }
