@@ -77,6 +77,7 @@ SIGNATURES: dict[str, list] = {
     "chg_phonon_interaction": [P, P, P, P, P, P, I, I, I, I, I, P, P, I, P, I, D, P, I64, P, P],
     "chg_imag_self_energy": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
     "chg_collision_rows": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
+    "chg_self_energy_spectrum": [P, I, I, I, I, P, I, P, I, P, I, P, P, I, D, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -121,6 +122,17 @@ def collision_scratch_doubles(n_q1, n_band):
     """The scratch of one ``chg_collision_rows`` call: the tetrahedron weights g2, g1+ and g1-, three [n_q1, n_band^3]
     planes."""
     return 3 * n_q1 * n_band**3
+
+
+# CHG_SE_MAX_CHUNKS: the most chunks chg_self_energy_spectrum's partial sums use (tests/test_spectral_function_spec.py
+# ties it to the header)
+SE_MAX_CHUNKS = 128
+
+
+def se_scratch_doubles(n_band, n_freq, n_t):
+    """The scratch of one ``chg_self_energy_spectrum`` call: ``SE_MAX_CHUNKS`` chunks of [n_t, n_band, n_freq] partial
+    sums (no per-q1 part)."""
+    return SE_MAX_CHUNKS * n_t * n_band * n_freq
 
 _lib = None
 
@@ -623,6 +635,22 @@ class CudaKernels:
         work = torch.empty(max(1, collision_scratch_doubles(n_q1, nb)), dtype=torch.float64, device=freqs.device)
         self._call("chg_collision_rows", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), _p(q1),
                    n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(out))
+
+    def self_energy_spectrum(self, freqs, mesh, tetrahedra, target, omega, q1, p, temperatures, cutoff_thz, gamma):
+        """gamma [T, n_band, F] fp64 += the contribution of the q1 (mesh indices ``q1`` [n_q1] int32) to the imaginary
+        self-energy (half width, THz) of the target's modes at the points omega [F] (ascending, shared by every band;
+        0 below cutoff_thz) (``chg_self_energy_spectrum``); the other arguments as ``imag_self_energy``."""
+        self._chk(freqs, tetrahedra, omega, q1, p, temperatures, gamma)
+        n1, n2, n3 = _mesh_args("self_energy_spectrum", mesh, freqs, tetrahedra,
+                                "freqs, omega, p, temperatures and gamma", (freqs, omega, p, temperatures, gamma))
+        nb, n_q1, n_t, n_f = freqs.shape[1], q1.shape[0], temperatures.shape[0], omega.shape[0]
+        if (q1.dtype != torch.int32 or q1.dim() != 1 or omega.dim() != 1 or temperatures.dim() != 1
+                or tuple(p.shape) != (n_q1, nb, nb, nb) or tuple(gamma.shape) != (n_t, nb, n_f)):
+            raise ChgnetB200Error(f"self_energy_spectrum: q1 must be int32 [Q1], omega [F], p [Q1, {nb}, {nb}, {nb}], "
+                                  f"temperatures [T] and gamma [T, {nb}, F]")
+        work = torch.empty(max(1, se_scratch_doubles(nb, n_f, n_t)), dtype=torch.float64, device=freqs.device)
+        self._call("chg_self_energy_spectrum", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), n_f,
+                   _p(q1), n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(gamma))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

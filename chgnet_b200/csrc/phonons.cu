@@ -1129,6 +1129,206 @@ collision_rows_kernel(const double* __restrict__ freqs, int n_band, int n1, int 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Self-energy spectrum.  gamma[t][l][f] += 18 pi / h^2 sum over the items (q1, l1, l2) of the call of
+//   P[q1][l][l1][l2] [(1 + n1 + n2) g2(w_f) + (n1 - n2) (g1+ - g1-)(w_f)]
+// with the vertex weights of ise_weights_kernel, evaluated at the points w_f shared by every band instead of at the
+// band frequencies; a point below the cutoff gets 0.  Block (chunk of item tiles, tile of SE_F_TILE points x tile of
+// SE_L_TILE bands, tile of SE_T_TILE temperatures), SE_THREADS threads, per tile of SE_ITEMS items:
+//   1. thread (item, tv) sorts the three corner sets (nu1 + nu2, nu2 - nu1, nu1 - nu2) of the tetrahedron-corner tv
+//      around q1 into shared memory, with the position of q1 in each; the other threads stage P[q1][l][l1][l2] of the
+//      band tile and the occupation factors 1 + n1 + n2 and n1 - n2 of each item at the tile's temperatures;
+//   2. thread (item = warp, point = lane) walks its item's 24 x 3 sets in the order of ise_weights_kernel and
+//      writes (g2, g1+ - g1-) at its point; the warp marks an item with no weight at any point of the tile;
+//   3. thread (band = warp + 8 j, point = lane) adds P times the occupation-weighted weights over the tile's items in
+//      order, skipping the marked items and P = 0 (both uniform across the warp).
+// The block writes work[chunk][t][l][f], each element by one thread; chunk_reduce_kernel adds the chunks in chunk order
+// to gamma.  No atomics, and no per-(item, point) value leaves the SM.
+constexpr int SE_THREADS = 256;
+constexpr int SE_ITEMS = 8;                            // items per staged tile: one warp each in step 2
+constexpr int SE_F_TILE = 32;                          // points per block: one lane each
+constexpr int SE_L_PER = 4;                            // bands per thread in step 3
+constexpr int SE_L_TILE = SE_L_PER * SE_THREADS / 32;  // bands per block
+constexpr int SE_T_TILE = 4;                           // temperatures per block
+constexpr int SE_SORTERS = SE_ITEMS * 24;              // step-1 threads that sort; the rest stage P and occupations
+
+__global__ void __launch_bounds__(SE_THREADS)
+self_energy_spectrum_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
+                            const int32_t* __restrict__ tet, int target, const double* __restrict__ omega, int n_freq,
+                            const int32_t* __restrict__ q1_idx, int n_q1, const double* __restrict__ p,
+                            const double* __restrict__ temps, int n_t, double cutoff, double* __restrict__ work) {
+  __shared__ double s_e[SE_ITEMS][24][3][4];        // sorted corner values per (item, tv, class)
+  __shared__ int8_t s_pos[SE_ITEMS][24][3];         // the position of q1 among them
+  __shared__ double s_p[SE_ITEMS][SE_L_TILE];       // P[q1][l0 + j][l1][l2]
+  __shared__ double s_occ[SE_ITEMS][SE_T_TILE][2];  // 1 + n1 + n2, n1 - n2
+  __shared__ double2 s_w[SE_ITEMS][SE_F_TILE];      // (g2, g1+ - g1-) at the tile's points
+  __shared__ int s_any[SE_ITEMS];
+  const int f_tiles = (n_freq + SE_F_TILE - 1) / SE_F_TILE;
+  const int f0 = (blockIdx.y % f_tiles) * SE_F_TILE, l0 = (blockIdx.y / f_tiles) * SE_L_TILE;
+  const int t0 = blockIdx.z * SE_T_TILE;
+  const int t_here = min(SE_T_TILE, n_t - t0);
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int f = f0 + lane;
+  const double w = f < n_freq ? __ldg(omega + f) : 0.0;
+  const bool live_point = f < n_freq && w >= cutoff;
+  const int64_t nb2 = (int64_t)n_band * n_band, n_items = (int64_t)n_q1 * nb2;
+  const int ta = target / (n2 * n3), tb = (target / n3) % n2, tc = target % n3;
+  double acc[SE_L_PER][SE_T_TILE];
+#pragma unroll
+  for (int j = 0; j < SE_L_PER; ++j)
+#pragma unroll
+    for (int t = 0; t < SE_T_TILE; ++t) acc[j][t] = 0.0;
+  const int64_t n_tiles = (n_items + SE_ITEMS - 1) / SE_ITEMS;
+  const int64_t t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  for (int64_t tile = n_tiles * blockIdx.x / gridDim.x; tile < t_end; ++tile) {
+    __syncthreads();  // the previous tile has been read
+    if (threadIdx.x < SE_SORTERS) {
+      const int it = threadIdx.x / 24, tv = threadIdx.x % 24;
+      const int64_t i = tile * SE_ITEMS + it;
+      double e2[4], ep[4], em[4];
+      int x2[4], xp[4], xm[4];
+      bool live = false;
+      if (i < n_items) {
+        const int q1 = __ldg(q1_idx + (int)(i / nb2)), l1 = (int)((i / n_band) % n_band), l2 = (int)(i % n_band);
+        const auto nu_pair = [&](int a, int b, int c, double& nu1, double& nu2) {
+          int a2 = ta - a, b2 = tb - b, c2 = tc - c;
+          a2 += a2 < 0 ? n1 : 0;
+          b2 += b2 < 0 ? n2 : 0;
+          c2 += c2 < 0 ? n3 : 0;
+          nu1 = __ldg(freqs + (int64_t)((a * n2 + b) * n3 + c) * n_band + l1);
+          nu2 = __ldg(freqs + (int64_t)((a2 * n2 + b2) * n3 + c2) * n_band + l2);
+        };
+        const int qa = q1 / (n2 * n3), qb = (q1 / n3) % n2, qc = q1 % n3;
+        double nu1, nu2;
+        nu_pair(qa, qb, qc, nu1, nu2);
+        live = nu1 >= cutoff && nu2 >= cutoff;
+        if (live) {
+          const int iv = tv / 4, v = tv % 4;
+          const int32_t* o = tet + (iv * 4 + v) * 3;
+          // the cell whose corner v of tetrahedron iv is q1
+          int ca = qa - __ldg(o), cb = qb - __ldg(o + 1), cc = qc - __ldg(o + 2);
+          ca += ca < 0 ? n1 : 0;
+          cb += cb < 0 ? n2 : 0;
+          cc += cc < 0 ? n3 : 0;
+          tetrahedron_corners(tet, ((int64_t)(ca * n2 + cb) * n3 + cc) * 6 + iv, n1, n2, n3,
+                              [&](int u, int a, int b, int c) {
+                                double v1, v2;
+                                nu_pair(a, b, c, v1, v2);
+                                e2[u] = v1 + v2, ep[u] = v2 - v1, em[u] = v1 - v2;
+                                x2[u] = xp[u] = xm[u] = u;
+                              });
+          sort4(e2, x2);
+          sort4(ep, xp);
+          sort4(em, xm);
+          int p2 = 0, pp = 0, pm = 0;
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            p2 = x2[u] == v ? u : p2;
+            pp = xp[u] == v ? u : pp;
+            pm = xm[u] == v ? u : pm;
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            s_e[it][tv][0][u] = e2[u];
+            s_e[it][tv][1][u] = ep[u];
+            s_e[it][tv][2][u] = em[u];
+          }
+          s_pos[it][tv][0] = (int8_t)p2, s_pos[it][tv][1] = (int8_t)pp, s_pos[it][tv][2] = (int8_t)pm;
+        }
+      }
+      if (!live) {  // an empty range: no point is evaluated
+#pragma unroll
+        for (int k = 0; k < 3; ++k) s_e[it][tv][k][0] = CUDART_INF;
+      }
+    } else {
+      for (int k = threadIdx.x - SE_SORTERS; k < SE_ITEMS * SE_L_TILE; k += SE_THREADS - SE_SORTERS) {
+        const int it = k / SE_L_TILE, l = l0 + k % SE_L_TILE;
+        const int64_t i = tile * SE_ITEMS + it;
+        s_p[it][k % SE_L_TILE] =
+            i < n_items && l < n_band ? __ldg(p + ((i / nb2) * n_band + l) * nb2 + (i % nb2)) : 0.0;
+      }
+      for (int k = threadIdx.x - SE_SORTERS; k < SE_ITEMS * SE_T_TILE; k += SE_THREADS - SE_SORTERS) {
+        const int it = k / SE_T_TILE, t = k % SE_T_TILE;
+        const int64_t i = tile * SE_ITEMS + it;
+        double b1 = 0.0, b2v = 0.0;
+        if (i < n_items && t < t_here) {
+          const int q1 = __ldg(q1_idx + (int)(i / nb2)), l1 = (int)((i / n_band) % n_band), l2 = (int)(i % n_band);
+          int a2 = ta - q1 / (n2 * n3), b2 = tb - (q1 / n3) % n2, c2 = tc - q1 % n3;
+          a2 += a2 < 0 ? n1 : 0;
+          b2 += b2 < 0 ? n2 : 0;
+          c2 += c2 < 0 ? n3 : 0;
+          const double temp = __ldg(temps + t0 + t);
+          b1 = bose(__ldg(freqs + (int64_t)q1 * n_band + l1), temp);
+          b2v = bose(__ldg(freqs + (int64_t)((a2 * n2 + b2) * n3 + c2) * n_band + l2), temp);
+        }
+        s_occ[it][t][0] = 1.0 + b1 + b2v;
+        s_occ[it][t][1] = b1 - b2v;
+      }
+    }
+    __syncthreads();
+    {
+      double gx = 0.0, gy = 0.0;
+      if (live_point) {
+        for (int tv = 0; tv < 24; ++tv) {
+          const double* s2 = s_e[warp][tv][0];
+          const double* sp = s_e[warp][tv][1];
+          const double* sm = s_e[warp][tv][2];
+          const bool h2 = w >= s2[0] && w < s2[3], hp = w >= sp[0] && w < sp[3], hm = w >= sm[0] && w < sm[3];
+          if (!(h2 || hp || hm)) continue;
+          double n, g, wt[4], d2 = 0.0, d1 = 0.0;
+          if (h2) {
+            const double e[4] = {s2[0], s2[1], s2[2], s2[3]};
+            tetra_weights(w, e, n, g, wt);
+            d2 = corner_weight(wt, s_pos[warp][tv][0]);
+          }
+          if (hp) {
+            const double e[4] = {sp[0], sp[1], sp[2], sp[3]};
+            tetra_weights(w, e, n, g, wt);
+            d1 = corner_weight(wt, s_pos[warp][tv][1]);
+          }
+          if (hm) {
+            const double e[4] = {sm[0], sm[1], sm[2], sm[3]};
+            tetra_weights(w, e, n, g, wt);
+            d1 -= corner_weight(wt, s_pos[warp][tv][2]);
+          }
+          gx = fma(d2, 1.0 / 6.0, gx);
+          gy = fma(d1, 1.0 / 6.0, gy);
+        }
+      }
+      s_w[warp][lane] = make_double2(gx, gy);
+      const bool any = __any_sync(0xffffffffu, gx != 0.0 || gy != 0.0);
+      if (lane == 0) s_any[warp] = any;
+    }
+    __syncthreads();
+    for (int it = 0; it < SE_ITEMS; ++it) {
+      if (!s_any[it]) continue;
+      const double2 g = s_w[it][lane];
+      double c2[SE_T_TILE], c1[SE_T_TILE];
+#pragma unroll
+      for (int t = 0; t < SE_T_TILE; ++t) c2[t] = s_occ[it][t][0], c1[t] = s_occ[it][t][1];
+#pragma unroll
+      for (int j = 0; j < SE_L_PER; ++j) {
+        const double pv = s_p[it][warp + 8 * j];
+        if (pv == 0.0) continue;
+#pragma unroll
+        for (int t = 0; t < SE_T_TILE; ++t) acc[j][t] = fma(pv, fma(c2[t], g.x, c1[t] * g.y), acc[j][t]);
+      }
+    }
+  }
+  if (f >= n_freq) return;
+  const double scale = 18.0 * 3.141592653589793 / (ISE_H * ISE_H);
+#pragma unroll
+  for (int j = 0; j < SE_L_PER; ++j) {
+    const int l = l0 + warp + 8 * j;
+    if (l >= n_band) continue;
+#pragma unroll
+    for (int t = 0; t < SE_T_TILE; ++t) {
+      if (t >= t_here) break;
+      work[(((size_t)blockIdx.x * n_t + t0 + t) * n_band + l) * n_freq + f] = scale * acc[j][t];
+    }
+  }
+}
+
 }  // namespace
 }  // namespace chg
 
@@ -1387,5 +1587,36 @@ extern "C" int chg_collision_rows(const double* freqs, int32_t n_band, int32_t n
   const size_t smem = sizeof(double) * 2 * COLL_T_TILE * n_band;
   collision_rows_kernel<<<dim3((unsigned)n_q1, (unsigned)t_tiles), COLL_THREADS, smem, st>>>(
       freqs, n_band, n1, n2, n3, target, q1_idx, n_q1, p, work, temperatures, n_t, cutoff_thz, out);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_self_energy_spectrum(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                                        const int32_t* tetrahedra, int32_t target, const double* omega, int32_t n_freq,
+                                        const int32_t* q1_idx, int32_t n_q1, const double* p,
+                                        const double* temperatures, int32_t n_t, double cutoff_thz, double* work,
+                                        int64_t work_doubles, double* gamma, void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_freq >= 0 && n_q1 >= 0 && n_t >= 0, "bad size");
+  CHG_CHECK_ARG((int64_t)n1 * n2 * n3 * std::max(n_band, 1) < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(target >= 0 && (int64_t)target < (int64_t)n1 * n2 * n3, "target outside the mesh");
+  if (n_band == 0 || n_freq == 0 || n_q1 == 0 || n_t == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && tetrahedra && omega && q1_idx && p && temperatures && work && gamma, "null pointer");
+  const int64_t n_out = (int64_t)n_t * n_band * n_freq;
+  CHG_CHECK_ARG(work_doubles >= (int64_t)CHG_SE_MAX_CHUNKS * n_out,
+                "work holds less than CHG_SE_MAX_CHUNKS n_t n_band n_freq doubles");
+  const int64_t f_tiles = ((int64_t)n_freq + SE_F_TILE - 1) / SE_F_TILE;
+  const int64_t l_tiles = ((int64_t)n_band + SE_L_TILE - 1) / SE_L_TILE;
+  const int64_t t_tiles = ((int64_t)n_t + SE_T_TILE - 1) / SE_T_TILE;
+  CHG_CHECK_ARG(f_tiles * l_tiles <= 65535 && t_tiles <= 65535, "too many frequency points, bands or temperatures");
+  // enough chunks for about 4 096 blocks in all, at most CHG_SE_MAX_CHUNKS and one item tile each
+  const int64_t n_tiles = ((int64_t)n_q1 * n_band * n_band + SE_ITEMS - 1) / SE_ITEMS;
+  const int64_t others = f_tiles * l_tiles * t_tiles;
+  const int64_t want = (4096 + others - 1) / others;
+  const int chunks =
+      (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)CHG_SE_MAX_CHUNKS, n_tiles, want}));
+  cudaStream_t st = as_stream(stream);
+  self_energy_spectrum_kernel<<<dim3(chunks, (unsigned)(f_tiles * l_tiles), (unsigned)t_tiles), SE_THREADS, 0, st>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, target, omega, n_freq, q1_idx, n_q1, p, temperatures, n_t, cutoff_thz,
+      work);
+  CHG_CUDA(reduce_chunks(work, chunks, n_out, AccumulateStore{gamma}, st));
   CHG_LAUNCH_END();
 }

@@ -16,14 +16,15 @@
   vectors and their broadened spectra, per Q (``dynamic_structure_factor``) and averaged over directions for powders
   (``powder_spectrum``), with ``chg_structure_factors`` and ``chg_broadened_spectrum``; with third-order force
   constants (``third_order_force_constants``), three-phonon interaction strengths (``chg_phonon_interaction``),
-  linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation.
+  linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation;
+  frequency-resolved self-energies (``chg_self_energy_spectrum``) and anharmonic phonon spectral functions.
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
 primitive cell for densities of states, A^2 for thermal displacement matrices, 1/THz for joint densities of states,
 b^2 per primitive cell for structure factors (b the caller's scattering lengths) and b^2/THz for their spectra,
 eV/A^3 for third-order force constants, eV^2 for interaction strengths, THz for linewidths, ps for lifetimes and
-W/(m K) for thermal conductivities.
+W/(m K) for thermal conductivities, 1/THz for spectral functions.
 """
 from __future__ import annotations
 
@@ -34,7 +35,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from chgnet_b200._lib import JDOS_MAX_CHUNKS, ise_scratch_doubles, ph3_scratch_doubles, sqw_scratch_doubles
+from chgnet_b200._lib import (JDOS_MAX_CHUNKS, ise_scratch_doubles, ph3_scratch_doubles, se_scratch_doubles,
+                              sqw_scratch_doubles)
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -349,6 +351,31 @@ def _degenerate_operators(nu: torch.Tensor) -> torch.Tensor:
     return same / same.sum(-1, keepdim=True)
 
 
+def _hat_matrix(x: torch.Tensor, grid: torch.Tensor, h: float) -> torch.Tensor:
+    """[X, M]: the hat functions max(0, 1 - |x - w_k| / h) of the uniform ``grid`` w_k = k h [M] at the points ``x``
+    [X]; Gamma_hat(x) = this @ Gamma_k, the piecewise-linear interpolant, 0 beyond the last hat."""
+    return (1.0 - (x[:, None] - grid[None, :]).abs() / h).clamp_min(0.0)
+
+
+def _hilbert_matrix(x: torch.Tensor, grid: torch.Tensor, h: float) -> torch.Tensor:
+    """[X, M]: Delta(x) = this @ Gamma_k, the Hilbert transform of the odd extension of ``_hat_matrix``'s interpolant
+    (DESIGN.md section 12.9), in closed form:
+
+        Delta(x) = (1/pi) sum_{k >= 1} Gamma_k [H_k(x) + H_k(-x)],
+        H_k(x) = [g(x - w_k + h) - 2 g(x - w_k) + g(x - w_k - h)] / h,   g(x) = x ln|x|,  g(0) = 0
+
+    Column 0 (w_0 = 0, where the odd extension is 0) is 0."""
+    def g(u):
+        return torch.where(u == 0, 0.0, u * torch.log(torch.where(u == 0, 1.0, u.abs())))
+
+    def hk(u):
+        return (g(u + h) - 2.0 * g(u) + g(u - h)) / h
+
+    k = (hk(x[:, None] - grid[None, :]) + hk(-x[:, None] - grid[None, :])) / math.pi
+    k[:, 0] = 0.0
+    return k
+
+
 def _gaussian_sigma(width) -> float | None:
     """The standard deviation (THz) of a Gaussian of FWHM ``width``, width / (2 sqrt(2 ln 2)); None for None, and
     ValueError unless it is finite and > 0."""
@@ -400,6 +427,8 @@ class Phonons:
     # thermal_conductivity_lbte: the collision matrices of all temperatures are built in one pass over the targets when
     # they fit in this many bytes (fp64, M^2 per temperature), else in groups of temperatures
     lbte_matrix_bytes = 8 << 30
+    # spectral_function: report frequencies evaluated per pass (the interpolation and Hilbert matrices are [F, M])
+    spectrum_points_per_pass = 4096
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, fc3=None, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -969,6 +998,103 @@ class Phonons:
                "linewidths": gamma.cpu().numpy(), "n_imaginary": n_imaginary}
         if single:
             res["frequencies"], res["linewidths"] = res["frequencies"][0], res["linewidths"][:, 0]
+        return res
+
+    def _spectrum_q1_chunk(self, n_t, n_freq) -> int:
+        """q1 per ``chg_phonon_interaction`` / ``chg_self_energy_spectrum`` call in ``spectral_function``: P, the
+        interaction's scratch and the spectrum's partial sums within ``ph3_chunk_bytes`` (at least one)."""
+        n_prim = len(self.p2s)
+        nb = 3 * n_prim
+        per_q1 = 8 * (nb**3 + ph3_scratch_doubles(1, n_prim, len(self.s2p)))
+        fixed = 8 * (se_scratch_doubles(nb, n_freq, n_t) + n_t * nb * n_freq)
+        return int(max(1, min(65535, (self.ph3_chunk_bytes - fixed) // per_q1)))
+
+    def _target_self_energy(self, mesh, nu, e, tets, t, target: int, grid: torch.Tensor) -> torch.Tensor:
+        """Gamma [T, 3n, M] (THz) of the modes of the mesh index ``target`` at the points ``grid`` [M]: P and its
+        contribution per chunk of q1 (``_spectrum_q1_chunk``, chunks in mesh order), then averaged over the degenerate
+        sets of each point (``_degenerate_average``)."""
+        nb, m = nu.shape[1], grid.shape[0]
+        gamma = torch.zeros(len(t), nb, m, dtype=torch.float64, device=self.device)
+        for q1, p in self._interaction_chunks(mesh, nu, e, target, self._spectrum_q1_chunk(len(t), m)):
+            self.kernels.self_energy_spectrum(nu, mesh, tets, int(target), grid, q1, p, t, THERMAL_CUTOFF_THZ, gamma)
+        avg = _degenerate_average(gamma.transpose(1, 2).reshape(-1, nb), nu[target])
+        return avg.reshape(len(t), m, nb).transpose(1, 2)
+
+    def spectral_function(self, mesh, qpoints, temperatures, frequency_points=None, *, self_energy_points=201) -> dict:
+        """Frequency-resolved three-phonon self-energies and anharmonic phonon spectral functions of the modes at
+        ``qpoints`` ([Q, 3] or [3], reduced, on the full Gamma-centred ``mesh``) at ``temperatures`` (K), DESIGN.md
+        section 12.9.  Gamma_l(q; w) is ``linewidths``' sum with the tetrahedron weights at w instead of at nu_l, on
+        the grid w_k = k h, k = 0 ... M - 1, h = 2 nu_max / (M - 1) (M = ``self_energy_points``, nu_max the highest
+        mesh frequency); between the points it is the piecewise-linear interpolant, 0 beyond.  The real part is the
+        exact Hilbert transform of the odd extension of that interpolant, in closed form,
+
+            Delta_l(w) = (1/pi) PV int_0^inf Gamma_l(w') [1 / (w - w') - 1 / (w + w')] dw'
+
+        so Sigma = Delta - i Gamma is causal, and the spectral function (1/THz) with the harmonic nu_l is
+
+            A_l(q; w) = (1/pi) 4 nu_l^2 Gamma_l(w) / [(w^2 - nu_l^2 - 2 nu_l Delta_l(w))^2 + 4 nu_l^2 Gamma_l(w)^2]
+
+        (0 where Gamma_l(w) = 0), which keeps int_0^inf w A dw = nu_l when it has no undamped pole.  Gamma is
+        averaged over each set of degenerate modes at q at every grid point (so are Delta, A and the shifts); modes
+        below ``THERMAL_CUTOFF_THZ``, and the three modes of smallest |nu| at Gamma, get 0 throughout.
+
+        Returns ``frequencies`` [Q, 3n] (THz, with that Gamma rule), ``temperatures``, ``self_energy_points`` [M]
+        (THz), ``gamma`` and ``delta`` [T, Q, 3n, M] (THz) on them, ``frequency_points`` [F] (THz; default 2 001
+        points from 0 to 2 nu_max), ``spectral_function`` [T, Q, 3n, F], ``frequency_shifts`` [T, Q, 3n] = Delta_l
+        (nu_l) (THz) and ``n_imaginary`` (the modes below -``THERMAL_CUTOFF_THZ`` over the mesh).  A single q drops
+        the Q axis.  ValueError without ``force_constants3``, for bad temperatures, q off the mesh,
+        ``self_energy_points`` not an integer >= 3, and ``frequency_points`` that are not a non-empty list of finite
+        numbers >= 0.  The mesh is diagonalised once per call; P (``chg_phonon_interaction``) is made and consumed
+        (``chg_self_energy_spectrum``) per chunk of q1 within ``ph3_chunk_bytes``, on the device."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = q.reshape(-1, 3)
+        idx = _mesh_indices(mesh, q)
+        if temperatures is None:
+            raise ValueError("spectral_function needs temperatures")
+        if isinstance(self_energy_points, (bool, np.bool_)) or not isinstance(self_energy_points, (int, np.integer)) \
+                or self_energy_points < 3:
+            raise ValueError(f"self_energy_points must be an integer >= 3, got {self_energy_points!r}")
+        m = int(self_energy_points)
+        report = None
+        if frequency_points is not None:
+            report = np.asarray(frequency_points, dtype=np.float64).reshape(-1)
+            if report.size == 0 or not np.all(np.isfinite(report)) or np.any(report < 0):
+                raise ValueError("frequency_points must be a non-empty list of finite frequencies >= 0 (THz), got "
+                                 f"{np.asarray(frequency_points).tolist()}")
+        mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        dev, f64 = self.device, torch.float64
+        t = torch.as_tensor(temps).to(dev)
+        top = float(2 * nu.max())
+        h = top / (m - 1)
+        grid = torch.arange(m, dtype=f64, device=dev) * h
+        if report is None:
+            omega = torch.lerp(torch.zeros((), dtype=f64, device=dev).expand(2001),
+                               torch.full((), top, dtype=f64, device=dev).expand(2001),
+                               torch.arange(2001, dtype=f64, device=dev) / 2000)
+        else:
+            omega = torch.as_tensor(report).to(dev)
+        gamma = torch.stack([self._target_self_energy(mesh, nu, e, tets, t, int(i), grid) for i in idx], 1)
+        nq = nu[torch.as_tensor(idx).to(dev)]  # [Q, 3n]
+        delta = gamma @ _hilbert_matrix(grid, grid, h).T  # [T, Q, 3n, M]
+        shifts = (gamma * _hilbert_matrix(nq.reshape(-1), grid, h).view(*nq.shape, m)[None]).sum(-1)
+        v = nq[None, :, :, None]
+        a = torch.empty(*gamma.shape[:3], len(omega), dtype=f64, device=dev)
+        for s in range(0, len(omega), self.spectrum_points_per_pass):  # keeps the [F, M] matrices small
+            w = omega[s : s + self.spectrum_points_per_pass]
+            g_rep = gamma @ _hat_matrix(w, grid, h).T  # [T, Q, 3n, F]
+            d_rep = gamma @ _hilbert_matrix(w, grid, h).T
+            den = (w * w - v * v - 2 * v * d_rep) ** 2 + 4 * v * v * g_rep * g_rep
+            a[..., s : s + len(w)] = torch.where(
+                g_rep != 0, 4 * v * v * g_rep / (math.pi * torch.where(g_rep != 0, den, 1.0)), 0.0)
+        res = {"frequencies": nq.cpu().numpy(), "temperatures": temps, "self_energy_points": grid.cpu().numpy(),
+               "gamma": gamma.cpu().numpy(), "delta": delta.cpu().numpy(), "frequency_points": omega.cpu().numpy(),
+               "spectral_function": a.cpu().numpy(), "frequency_shifts": shifts.cpu().numpy(),
+               "n_imaginary": n_imaginary}
+        if single:
+            res["frequencies"] = res["frequencies"][0]
+            for k in ("gamma", "delta", "spectral_function", "frequency_shifts"):
+                res[k] = res[k][:, 0]
         return res
 
     def thermal_conductivity(self, mesh, temperatures) -> dict:

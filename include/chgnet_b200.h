@@ -668,6 +668,18 @@ int chg_collision_rows(const double* freqs, int32_t n_band, int32_t n1, int32_t 
                        const int32_t* tetrahedra, int32_t target, const double* omega, const int32_t* q1_idx,
                        int32_t n_q1, const double* p, const double* temperatures, int32_t n_t, double cutoff_thz,
                        double* work, int64_t work_doubles, double* out, void* stream);
+/* Imaginary self-energy spectrum (half width, THz) of the modes of one target q on a list of frequency points:
+ * gamma [n_t][n_band][n_freq] += the sum of chg_imag_self_energy with its w = omega[l] replaced by w = omega[f], the
+ * same points for every band (DESIGN.md section 12.9).  omega [n_freq] THz, ascending; a point below cutoff_thz gets
+ * 0.  The other arguments as chg_imag_self_energy.  work: at least CHG_SE_MAX_CHUNKS n_t n_band n_freq doubles
+ * (work_doubles); no per-(item, point) weight leaves the SM.  Deterministic: per-block partial sums added in a fixed
+ * order, no atomics.                                                                                               */
+#define CHG_SE_MAX_CHUNKS 128
+int chg_self_energy_spectrum(const double* freqs, int32_t n_band, int32_t n1, int32_t n2, int32_t n3,
+                             const int32_t* tetrahedra, int32_t target, const double* omega, int32_t n_freq,
+                             const int32_t* q1_idx, int32_t n_q1, const double* p, const double* temperatures,
+                             int32_t n_t, double cutoff_thz, double* work, int64_t work_doubles, double* gamma,
+                             void* stream);
 
 #ifdef __cplusplus
 }
