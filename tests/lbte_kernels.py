@@ -4,7 +4,7 @@
 ``Phonons(..., fc3=..., device="cpu", kernels=LbteSpecKernels())`` runs ``thermal_conductivity_lbte`` on the host.
 Two switches plant the bugs the tests must catch: ``time_reversal=False`` sends the (b) and (c) terms of DESIGN.md
 section 12.8 to the columns q1 and q2 instead of -q1 and -q2, and ``class1_sign=-1`` flips u_q u_c of the class-1
-terms.
+terms.  ``axes_reversed`` is ``ThreePhononSpecKernels``'.
 """
 from __future__ import annotations
 
@@ -30,7 +30,8 @@ def inverse_sinh(nu, temperatures, cutoff_thz):
 class LbteSpecKernels(ThreePhononSpecKernels):
     """``ThreePhononSpecKernels`` with the specification of ``chg_collision_rows``."""
 
-    def __init__(self, *, time_reversal: bool = True, class1_sign: float = 1.0):
+    def __init__(self, *, time_reversal: bool = True, class1_sign: float = 1.0, axes_reversed: bool = False):
+        super().__init__(axes_reversed=axes_reversed)
         self.time_reversal, self.class1_sign = time_reversal, class1_sign
 
     def collision_rows(self, freqs, mesh, tetrahedra, target, omega, q1, p, temperatures, cutoff_thz, out):
@@ -42,9 +43,10 @@ class LbteSpecKernels(ThreePhononSpecKernels):
         mesh_t = tuple(int(n) for n in mesh)
         size = torch.tensor(mesh_t, device=dev)
         nu = freqs.to(f64)
-        w = vertex_weights(nu, mesh_t, tetrahedra, target, omega, q1, cutoff_thz, self.ise_chunk_items)
-        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t)
-        c1 = _mesh_coords(q1.long(), mesh_t)
+        w = vertex_weights(nu, mesh_t, tetrahedra, target, omega, q1, cutoff_thz, self.ise_chunk_items,
+                           self.axes_reversed)
+        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t, self.axes_reversed)
+        c1 = _mesh_coords(q1.long(), mesh_t, self.axes_reversed)
         i2 = _mesh_index((tc - c1) % size, mesh_t)
         is1 = inverse_sinh(nu[q1.long()], temperatures, cutoff_thz)  # [Q1, nb, T]
         is2 = inverse_sinh(nu[i2], temperatures, cutoff_thz)

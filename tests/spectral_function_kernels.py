@@ -4,7 +4,7 @@
 ``Phonons(..., fc3=..., device="cpu", kernels=SpectralFunctionSpecKernels())`` runs ``spectral_function`` on the host.
 The weights come from ``vertex_weights``, which evaluates n_band points at a time: the points are passed in slices of
 n_band, the last one padded with 0, which lies below the cutoff and so gets no weight.  ``class1_sign=-1`` plants the
-bug the tests must catch: it flips g1+ - g1-.
+bug the tests must catch: it flips g1+ - g1-.  ``axes_reversed`` is ``ThreePhononSpecKernels``'.
 """
 from __future__ import annotations
 
@@ -20,7 +20,8 @@ from three_phonon_kernels import ThreePhononSpecKernels, _mesh_coords, _mesh_ind
 class SpectralFunctionSpecKernels(ThreePhononSpecKernels):
     """``ThreePhononSpecKernels`` with the specification of ``chg_self_energy_spectrum``."""
 
-    def __init__(self, *, class1_sign: float = 1.0):
+    def __init__(self, *, class1_sign: float = 1.0, axes_reversed: bool = False):
+        super().__init__(axes_reversed=axes_reversed)
         self.class1_sign = class1_sign
 
     def self_energy_spectrum(self, freqs, mesh, tetrahedra, target, omega, q1, p, temperatures, cutoff_thz, gamma):
@@ -33,8 +34,8 @@ class SpectralFunctionSpecKernels(ThreePhononSpecKernels):
         size = torch.tensor(mesh_t, device=dev)
         nu = freqs.to(f64)
         nb, n_f = nu.shape[1], omega.shape[0]
-        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t)
-        i2 = _mesh_index((tc - _mesh_coords(q1.long(), mesh_t)) % size, mesh_t)
+        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t, self.axes_reversed)
+        i2 = _mesh_index((tc - _mesh_coords(q1.long(), mesh_t, self.axes_reversed)) % size, mesh_t)
         nu1, nu2 = nu[q1.long()], nu[i2]  # [Q1, nb]
         n1 = occupations(torch.where(nu1 >= cutoff_thz, nu1, 1.0), temperatures)  # [Q1, nb, T]
         n2 = occupations(torch.where(nu2 >= cutoff_thz, nu2, 1.0), temperatures)
@@ -46,7 +47,8 @@ class SpectralFunctionSpecKernels(ThreePhononSpecKernels):
             pts = torch.zeros(nb, dtype=f64, device=dev)
             here = min(nb, n_f - s)
             pts[:here] = omega[s : s + here].to(f64)
-            w = vertex_weights(nu, mesh_t, tetrahedra, target, pts, q1, cutoff_thz, self.ise_chunk_items)
+            w = vertex_weights(nu, mesh_t, tetrahedra, target, pts, q1, cutoff_thz, self.ise_chunk_items,
+                               self.axes_reversed)
             w = w[:, :here]  # [Q1, point, l1, l2, 3]
             g2 = torch.einsum("qlab,qjab,qabt->tlj", p, w[..., 0], c2)
             g1 = torch.einsum("qlab,qjab,qabt->tlj", p, w[..., 1] - w[..., 2], c1)

@@ -5,7 +5,8 @@
 ``Phonons(..., fc3=..., device="cpu", kernels=ThreePhononSpecKernels())`` runs ``linewidths`` and
 ``thermal_conductivity`` on the host.  ``interaction_strengths`` evaluates P for explicit (q, q1, q2), q2 not
 necessarily reduced, and ``vertex_weights`` the tetrahedron weights of each vertex q1; both are module functions so
-that the tests can use them on their own.
+that the tests can use them on their own.  ``axes_reversed=True`` plants the bug the non-cubic meshes must catch: every
+mesh index is split into coordinates as if the mesh were (n3, n2, n1), which changes nothing on a cubic mesh.
 """
 from __future__ import annotations
 
@@ -67,16 +68,19 @@ def interaction_strengths(fc3, img_ptr, img_vec, s2p, inv_sqrt_m, frac, n_mesh, 
     return torch.where(keep, scale * (t.real**2 + t.imag**2) / torch.where(keep, den, 1.0), 0.0)
 
 
-def _mesh_coords(i, mesh):
-    n1, n2, n3 = mesh
-    return torch.stack([i // (n2 * n3), (i // n3) % n2, i % n3], -1)
+def _mesh_coords(i, mesh, axes_reversed=False):
+    """The coordinates [..., 3] of the mesh indices ``i``; ``axes_reversed`` splits with (n3, n2, n1) instead and wraps
+    the result onto the mesh (the planted bug)."""
+    n1, n2, n3 = mesh[::-1] if axes_reversed else mesh
+    c = torch.stack([i // (n2 * n3), (i // n3) % n2, i % n3], -1)
+    return c % torch.tensor(mesh, device=c.device) if axes_reversed else c
 
 
 def _mesh_index(c, mesh):
     return (c[..., 0] * mesh[1] + c[..., 1]) * mesh[2] + c[..., 2]
 
 
-def vertex_weights(freqs, mesh, tetrahedra, target, omega, q1, cutoff_thz, chunk_items=1 << 14):
+def vertex_weights(freqs, mesh, tetrahedra, target, omega, q1, cutoff_thz, chunk_items=1 << 14, axes_reversed=False):
     """[Q1, l, l1, l2, 3]: the weights (g2, g1+, g1-) with which vertex q1 (mesh indices ``q1`` [Q1]) enters the
     tetrahedron averages of d(w - nu1 - nu2), d(w + nu1 - nu2) and d(w - nu1 + nu2) at w = omega[l]: 1/6 of the sum
     over the 24 (tetrahedron, corner) whose corner is q1 of ``tetrahedron_weights``' weight of that corner, the corner
@@ -89,8 +93,8 @@ def vertex_weights(freqs, mesh, tetrahedra, target, omega, q1, cutoff_thz, chunk
     nu = freqs.to(f64)
     n_q1, nb = q1.shape[0], nu.shape[1]
     om = omega.to(f64)
-    tgt = _mesh_coords(torch.tensor(int(target), device=dev), mesh)
-    c1 = _mesh_coords(q1.long(), mesh)  # [Q1, 3]
+    tgt = _mesh_coords(torch.tensor(int(target), device=dev), mesh, axes_reversed)
+    c1 = _mesh_coords(q1.long(), mesh, axes_reversed)  # [Q1, 3]
     off = tetrahedra.long()  # [6, 4, 3]
     # corners of the 24 (tetrahedron t, corner v) around each q1: cell = q1 - off[t, v], corners cell + off[t, u]
     corners = (c1[:, None, None, None, :] - off[:, :, None, :][None] + off[:, None, :, :][None]) % size  # [Q1,6,4,4,3]
@@ -121,12 +125,16 @@ def vertex_weights(freqs, mesh, tetrahedra, target, omega, q1, cutoff_thz, chunk
 
 
 class ThreePhononSpecKernels(PhononSpecKernels):
-    """``PhononSpecKernels`` with the specifications of the two three-phonon kernels."""
+    """``PhononSpecKernels`` with the specifications of the two three-phonon kernels; ``axes_reversed=True`` plants
+    the axis-reversed split of ``_mesh_coords`` in every kernel of this class and its subclasses."""
 
     # fc3-by-q1 work per chunk of the interaction specification (complex128 elements of its largest intermediate)
     ph3_chunk_elems = 1 << 22
     # (q1, l1, l2) items per chunk of the vertex weights
     ise_chunk_items = 1 << 14
+
+    def __init__(self, *, axes_reversed: bool = False):
+        self.axes_reversed = axes_reversed
 
     def phonon_interaction(self, fc3, img_ptr, img_vec, s2p, inv_sqrt_m, frac, mesh, freqs, eigvecs, target, q1,
                            cutoff_thz, out):
@@ -137,8 +145,8 @@ class ThreePhononSpecKernels(PhononSpecKernels):
         size = torch.tensor(mesh, device=dev)
         n_mesh = mesh[0] * mesh[1] * mesh[2]
         n_prim, n_super = fc3.shape[0], fc3.shape[1]
-        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh)
-        c1 = _mesh_coords(q1.long(), mesh)
+        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh, self.axes_reversed)
+        c1 = _mesh_coords(q1.long(), mesh, self.axes_reversed)
         c2 = (tc - c1) % size
         i2 = _mesh_index(c2, mesh)
         chunk = max(1, self.ph3_chunk_elems // (n_prim * n_super * n_prim * 27))
@@ -159,9 +167,10 @@ class ThreePhononSpecKernels(PhononSpecKernels):
         mesh_t = tuple(int(n) for n in mesh)
         size = torch.tensor(mesh_t, device=dev)
         nu = freqs.to(f64)
-        w = vertex_weights(nu, mesh_t, tetrahedra, target, omega, q1, cutoff_thz, self.ise_chunk_items)
-        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t)
-        i2 = _mesh_index((tc - _mesh_coords(q1.long(), mesh_t)) % size, mesh_t)
+        w = vertex_weights(nu, mesh_t, tetrahedra, target, omega, q1, cutoff_thz, self.ise_chunk_items,
+                           self.axes_reversed)
+        tc = _mesh_coords(torch.tensor(int(target), device=dev), mesh_t, self.axes_reversed)
+        i2 = _mesh_index((tc - _mesh_coords(q1.long(), mesh_t, self.axes_reversed)) % size, mesh_t)
         nu1, nu2 = nu[q1.long()], nu[i2]  # [Q1, nb]
         n1 = occupations(torch.where(nu1 >= cutoff_thz, nu1, 1.0), temperatures)  # [Q1, nb, T]
         n2 = occupations(torch.where(nu2 >= cutoff_thz, nu2, 1.0), temperatures)
