@@ -78,6 +78,7 @@ SIGNATURES: dict[str, list] = {
     "chg_imag_self_energy": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
     "chg_collision_rows": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
     "chg_self_energy_spectrum": [P, I, I, I, I, P, I, P, I, P, I, P, P, I, D, P, I64, P, P],
+    "chg_coherence_conductivity": [P, P, P, P, P, P, I, I, I, D, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -133,6 +134,17 @@ def se_scratch_doubles(n_band, n_freq, n_t):
     """The scratch of one ``chg_self_energy_spectrum`` call: ``SE_MAX_CHUNKS`` chunks of [n_t, n_band, n_freq] partial
     sums (no per-q1 part)."""
     return SE_MAX_CHUNKS * n_t * n_band * n_freq
+
+
+# CHG_WIGNER_MAX_CHUNKS: the most chunks chg_coherence_conductivity's partial sums use (tests/test_wigner_spec.py ties
+# it to the header)
+WIGNER_MAX_CHUNKS = 256
+
+
+def coherence_scratch_doubles(n_q, n_band, n_t):
+    """The scratch of one ``chg_coherence_conductivity`` call: W = dD/dQ E and the velocity operator V, two
+    [n_q, 3, n_band, n_band] complex buffers, and ``WIGNER_MAX_CHUNKS`` chunks of [n_t, 6] partial sums."""
+    return 12 * n_q * n_band**2 + WIGNER_MAX_CHUNKS * n_t * 6
 
 _lib = None
 
@@ -651,6 +663,30 @@ class CudaKernels:
         work = torch.empty(max(1, se_scratch_doubles(nb, n_f, n_t)), dtype=torch.float64, device=freqs.device)
         self._call("chg_self_energy_spectrum", _p(freqs), nb, n1, n2, n3, _p(tetrahedra), int(target), _p(omega), n_f,
                    _p(q1), n_q1, _p(p), _p(temperatures), n_t, float(cutoff_thz), _p(work), work.numel(), _p(gamma))
+
+    def coherence_conductivity(self, freqs, eigvecs, ddyn, set_id, heat_capacity, gamma, cutoff_thz, kappa):
+        """kappa [T, 3, 3] fp64 += the unscaled Wigner coherence pair sum of the q of the call
+        (``chg_coherence_conductivity``, DESIGN.md section 12.10): freqs [Q, n_band] THz (the Gamma acoustic modes
+        already 0), eigvecs [Q, mode, n_band] complex128 (mode-major), ddyn [Q, 3, n_band, n_band] complex128 as
+        ``dynamical_matrix_derivatives`` writes it, set_id [Q, n_band] int32 degenerate-set ids, heat_capacity (eV/K)
+        and gamma (THz) [T, Q, n_band]; pairs of modes below cutoff_thz, with Gamma <= 0 or in one set are left out."""
+        self._chk(freqs, eigvecs, ddyn, set_id, heat_capacity, gamma, kappa)
+        f64, c128 = torch.float64, torch.complex128
+        if (any(t.dtype != f64 for t in (freqs, heat_capacity, gamma, kappa)) or eigvecs.dtype != c128
+                or ddyn.dtype != c128 or set_id.dtype != torch.int32):
+            raise ChgnetB200Error("coherence_conductivity: eigvecs and ddyn must be complex128, set_id int32 and every "
+                                  "other tensor float64")
+        n_q, nb = freqs.shape
+        n_t = gamma.shape[0]
+        if (tuple(eigvecs.shape) != (n_q, nb, nb) or tuple(ddyn.shape) != (n_q, 3, nb, nb)
+                or tuple(set_id.shape) != (n_q, nb) or tuple(heat_capacity.shape) != (n_t, n_q, nb)
+                or tuple(gamma.shape) != (n_t, n_q, nb) or tuple(kappa.shape) != (n_t, 3, 3)):
+            raise ChgnetB200Error(f"coherence_conductivity: freqs must be [Q, n_band], eigvecs [{n_q}, {nb}, {nb}], "
+                                  f"ddyn [{n_q}, 3, {nb}, {nb}], set_id [{n_q}, {nb}], heat_capacity and gamma "
+                                  f"[T, {n_q}, {nb}] and kappa [T, 3, 3]")
+        work = torch.empty(max(1, coherence_scratch_doubles(n_q, nb, n_t)), dtype=f64, device=freqs.device)
+        self._call("chg_coherence_conductivity", _p(freqs), _p(eigvecs), _p(ddyn), _p(set_id), _p(heat_capacity),
+                   _p(gamma), n_q, nb, n_t, float(cutoff_thz), _p(work), work.numel(), _p(kappa))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

@@ -1329,6 +1329,176 @@ self_energy_spectrum_kernel(const double* __restrict__ freqs, int n_band, int n1
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Wigner coherence conductivity (DESIGN.md section 12.10).  Per q of the call and Cartesian axis a, with E[k][s] =
+// eigvecs[q][s][k] (mode-major) and c^2 = THZ_PER_SQRT_EV_A2_AMU^2, the velocity operator (THz A)
+//   W_a = dD/dQ_a E,   V_a[s][s'] = c^2 (E^H W_a)[s][s'] / (|nu_s| + |nu_s'|)   (0 where both are 0)
+// by two batched complex GEMMs (coh_gemm_kernel, STAGE 0 then 1; W and V live in scratch only).  coh_pair_kernel:
+// block (range of q, tile of COH_T_TILE temperatures); each thread owns (s, s') pairs of one q at a time and adds, for
+// every ordered pair of modes kept (nu >= cutoff, Gamma > 0) in different degenerate sets (set_id),
+//   (nu_s + nu_s') / 4 (C_s / nu_s + C_s' / nu_s') Re(V_a[s][s'] conj(V_b[s][s'])) L,
+//   L = (Gamma_s + Gamma_s') / (2 pi [(nu_s - nu_s')^2 + (Gamma_s + Gamma_s')^2]),
+// for the 6 components (a, b) and the tile's temperatures in registers.  V is Hermitian, so conj(V_b[s][s']) stands for
+// V_b[s'][s] and every term is symmetric in (a, b).  The block reduces in a fixed order (warp shuffles, then the warps
+// in order) and writes work[chunk][t][6]; chunk_reduce_kernel adds the chunks in chunk order into kappa [t][3][3].
+// No atomics.
+constexpr int COH_TILE = 32;   // GEMM output tile (both dimensions)
+constexpr int COH_KTILE = 16;  // GEMM reduction tile
+constexpr int COH_THREADS = 256;
+constexpr int COH_T_TILE = 4;  // temperatures per pair block
+
+// STAGE 0: out[q][a] = W_a [k][s'] = sum_k' ddyn[q][a][k][k'] E[k'][s'] (in = ddyn).  STAGE 1: out[q][a] = V_a [s][s']
+// = c2 sum_k conj(E[k][s]) W_a[k][s'] / (|nu_s| + |nu_s'|) (in = W).  Grid (tiles of the [nb][nb] output, q, a).
+template <int STAGE>
+__global__ void __launch_bounds__(256)
+coh_gemm_kernel(const double2* __restrict__ eig, const double2* __restrict__ in, const double* __restrict__ freqs, int nb,
+                double c2, double2* __restrict__ out) {
+  __shared__ double2 sa[COH_KTILE][COH_TILE];
+  __shared__ double2 sb[COH_KTILE][COH_TILE + 1];
+  const size_t nb2 = (size_t)nb * nb;
+  const int q = blockIdx.y;
+  const int tn = (nb + COH_TILE - 1) / COH_TILE;
+  const int m0 = blockIdx.x / tn * COH_TILE, c0 = blockIdx.x % tn * COH_TILE;
+  const double2* e = eig + (size_t)q * nb2;
+  const double2* x = in + ((size_t)q * 3 + blockIdx.z) * nb2;
+  const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
+  double cr[2][2] = {{0.0, 0.0}, {0.0, 0.0}}, ci[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
+  for (int k0 = 0; k0 < nb; k0 += COH_KTILE) {
+    __syncthreads();  // the previous tiles have been read
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int i = threadIdx.x + 256 * r;
+      const int am = i / COH_KTILE, ak = i % COH_KTILE;  // A(m0 + am, k0 + ak), row-major, k fastest
+      double2 va = make_double2(0.0, 0.0);
+      if (m0 + am < nb && k0 + ak < nb) {
+        if constexpr (STAGE == 0) {
+          va = __ldg(x + (size_t)(m0 + am) * nb + k0 + ak);
+        } else {  // A(s, k) = conj(E[k][s]) = conj(eig[s][k])
+          va = __ldg(e + (size_t)(m0 + am) * nb + k0 + ak);
+          va.y = -va.y;
+        }
+      }
+      sa[ak][am] = va;
+      double2 vb = make_double2(0.0, 0.0);
+      if constexpr (STAGE == 0) {  // B(k, n) = E[k][n] = eig[n][k]: k fastest
+        const int bn = i / COH_KTILE, bk = i % COH_KTILE;
+        if (c0 + bn < nb && k0 + bk < nb) vb = __ldg(e + (size_t)(c0 + bn) * nb + k0 + bk);
+        sb[bk][bn] = vb;
+      } else {  // B(k, n) = W[k][n], row-major
+        const int bk = i / COH_TILE, bn = i % COH_TILE;
+        if (c0 + bn < nb && k0 + bk < nb) vb = __ldg(x + (size_t)(k0 + bk) * nb + c0 + bn);
+        sb[bk][bn] = vb;
+      }
+    }
+    __syncthreads();
+    const int kn = min(COH_KTILE, nb - k0);
+    for (int kk = 0; kk < kn; ++kk) {
+      const double2 a0 = sa[kk][ty], a1 = sa[kk][ty + 16];
+      const double2 b0 = sb[kk][tx], b1 = sb[kk][tx + 16];
+      cr[0][0] = fma(a0.x, b0.x, fma(-a0.y, b0.y, cr[0][0]));
+      ci[0][0] = fma(a0.x, b0.y, fma(a0.y, b0.x, ci[0][0]));
+      cr[0][1] = fma(a0.x, b1.x, fma(-a0.y, b1.y, cr[0][1]));
+      ci[0][1] = fma(a0.x, b1.y, fma(a0.y, b1.x, ci[0][1]));
+      cr[1][0] = fma(a1.x, b0.x, fma(-a1.y, b0.y, cr[1][0]));
+      ci[1][0] = fma(a1.x, b0.y, fma(a1.y, b0.x, ci[1][0]));
+      cr[1][1] = fma(a1.x, b1.x, fma(-a1.y, b1.y, cr[1][1]));
+      ci[1][1] = fma(a1.x, b1.y, fma(a1.y, b1.x, ci[1][1]));
+    }
+  }
+  double2* o = out + ((size_t)q * 3 + blockIdx.z) * nb2;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int m = m0 + ty + 16 * i, c = c0 + tx + 16 * j;
+      if (m >= nb || c >= nb) continue;
+      if constexpr (STAGE == 0) {
+        o[(size_t)m * nb + c] = make_double2(cr[i][j], ci[i][j]);
+      } else {
+        const double den = fabs(__ldg(freqs + (size_t)q * nb + m)) + fabs(__ldg(freqs + (size_t)q * nb + c));
+        o[(size_t)m * nb + c] = den > 0.0 ? make_double2(c2 * cr[i][j] / den, c2 * ci[i][j] / den)
+                                          : make_double2(0.0, 0.0);
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(COH_THREADS)
+coh_pair_kernel(const double* __restrict__ freqs, const int32_t* __restrict__ set_id, const double2* __restrict__ vel,
+                const double* __restrict__ cv, const double* __restrict__ gamma, int n_q, int nb, int n_t,
+                double cutoff, double* __restrict__ work) {
+  __shared__ double red[COH_THREADS / 32][6 * COH_T_TILE];
+  const int t0 = blockIdx.y * COH_T_TILE;
+  const int t_here = min(COH_T_TILE, n_t - t0);
+  const int q_begin = (int)((int64_t)n_q * blockIdx.x / gridDim.x);
+  const int q_end = (int)((int64_t)n_q * (blockIdx.x + 1) / gridDim.x);
+  const int64_t nb2 = (int64_t)nb * nb;
+  double acc[6][COH_T_TILE];
+#pragma unroll
+  for (int c = 0; c < 6; ++c)
+#pragma unroll
+    for (int t = 0; t < COH_T_TILE; ++t) acc[c][t] = 0.0;
+  for (int q = q_begin; q < q_end; ++q) {
+    const double* nu = freqs + (size_t)q * nb;
+    const int32_t* sid = set_id + (size_t)q * nb;
+    const double2* v = vel + (size_t)q * 3 * nb2;
+    for (int64_t i = threadIdx.x; i < nb2; i += COH_THREADS) {
+      const int s = (int)(i / nb), sp = (int)(i % nb);
+      const double n1 = __ldg(nu + s), n2 = __ldg(nu + sp);
+      if (!(n1 >= cutoff && n2 >= cutoff) || __ldg(sid + s) == __ldg(sid + sp)) continue;
+      const double2 vx = __ldg(v + i), vy = __ldg(v + nb2 + i), vz = __ldg(v + 2 * nb2 + i);
+      double prod[6];  // Re(V_a conj(V_b)) in Voigt order xx, yy, zz, yz, xz, xy
+      prod[0] = fma(vx.x, vx.x, vx.y * vx.y);
+      prod[1] = fma(vy.x, vy.x, vy.y * vy.y);
+      prod[2] = fma(vz.x, vz.x, vz.y * vz.y);
+      prod[3] = fma(vy.x, vz.x, vy.y * vz.y);
+      prod[4] = fma(vx.x, vz.x, vx.y * vz.y);
+      prod[5] = fma(vx.x, vy.x, vx.y * vy.y);
+      const double quarter = 0.25 * (n1 + n2), dnu = n1 - n2;
+#pragma unroll
+      for (int t = 0; t < COH_T_TILE; ++t) {
+        if (t >= t_here) break;
+        const size_t o = ((size_t)(t0 + t) * n_q + q) * nb;
+        const double g1 = __ldg(gamma + o + s), g2 = __ldg(gamma + o + sp);
+        if (!(g1 > 0.0 && g2 > 0.0)) continue;
+        const double gs = g1 + g2;
+        const double w = quarter * (__ldg(cv + o + s) / n1 + __ldg(cv + o + sp) / n2) * gs /
+                         (2.0 * 3.141592653589793 * fma(dnu, dnu, gs * gs));
+#pragma unroll
+        for (int c = 0; c < 6; ++c) acc[c][t] = fma(w, prod[c], acc[c][t]);
+      }
+    }
+  }
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+#pragma unroll
+  for (int c = 0; c < 6; ++c) {
+#pragma unroll
+    for (int t = 0; t < COH_T_TILE; ++t) {
+      double x = acc[c][t];
+#pragma unroll
+      for (int off = 16; off > 0; off /= 2) x += __shfl_down_sync(0xffffffffu, x, off);
+      if (lane == 0) red[warp][t * 6 + c] = x;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 6 * t_here) {
+    double s = 0.0;
+    for (int w = 0; w < COH_THREADS / 32; ++w) s += red[w][threadIdx.x];
+    work[((size_t)blockIdx.x * n_t + t0) * 6 + threadIdx.x] = s;
+  }
+}
+
+struct SymmetricStore {  // work[chunk][t][6] (xx, yy, zz, yz, xz, xy): kappa[t][a][b] and kappa[t][b][a] += the sum
+  double* kappa;
+  __device__ void operator()(int64_t o, double s) const {
+    const int c = (int)(o % 6);
+    const int a = c < 3 ? c : (c == 3 ? 1 : 0), b = c < 3 ? c : (c == 5 ? 1 : 2);
+    double* k = kappa + (o / 6) * 9;
+    k[a * 3 + b] += s;
+    if (a != b) k[b * 3 + a] += s;
+  }
+};
+
 }  // namespace
 }  // namespace chg
 
@@ -1618,5 +1788,40 @@ extern "C" int chg_self_energy_spectrum(const double* freqs, int32_t n_band, int
       freqs, n_band, n1, n2, n3, tetrahedra, target, omega, n_freq, q1_idx, n_q1, p, temperatures, n_t, cutoff_thz,
       work);
   CHG_CUDA(reduce_chunks(work, chunks, n_out, AccumulateStore{gamma}, st));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_coherence_conductivity(const double* freqs, const double* eigvecs, const double* ddyn,
+                                          const int32_t* set_id, const double* heat_capacity, const double* gamma,
+                                          int32_t n_q, int32_t n_band, int32_t n_t, double cutoff_thz, double* work,
+                                          int64_t work_doubles, double* kappa, void* stream) {
+  CHG_CHECK_ARG(n_q >= 0 && n_band >= 0 && n_t >= 0, "negative size");
+  if (n_q == 0 || n_band == 0 || n_t == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && eigvecs && ddyn && set_id && heat_capacity && gamma && work && kappa, "null pointer");
+  CHG_CHECK_ARG(n_q <= 65535, "too many q in one call (at most 65535)");
+  CHG_CHECK_ARG(n_band <= 46340, "too many bands");
+  const int64_t t_tiles = ((int64_t)n_t + COH_T_TILE - 1) / COH_T_TILE;
+  CHG_CHECK_ARG(t_tiles <= 65535, "too many temperatures");
+  const int64_t nb2 = (int64_t)n_band * n_band, n_v = 3 * (int64_t)n_q * nb2;  // complex elements of W and of V
+  CHG_CHECK_ARG(work_doubles >= 4 * n_v + (int64_t)CHG_WIGNER_MAX_CHUNKS * n_t * 6,
+                "work holds less than 12 n_q n_band^2 + CHG_WIGNER_MAX_CHUNKS n_t 6 doubles");
+  double2* w_buf = reinterpret_cast<double2*>(work);
+  double2* v_buf = w_buf + n_v;
+  double* partial = work + 4 * n_v;
+  const double2* eig = reinterpret_cast<const double2*>(eigvecs);
+  // c = THZ_PER_SQRT_EV_A2_AMU of chgnet_b200.phonons: the same expression in the same order
+  const double ang = 1e-10;
+  const double c = sqrt(1.602176634e-19 / (ang * ang * 1.66053906660e-27)) / (2 * 3.141592653589793) / 1e12;
+  const int64_t tiles = ((int64_t)n_band + COH_TILE - 1) / COH_TILE;
+  const dim3 ggrid((unsigned)(tiles * tiles), (unsigned)n_q, 3);
+  cudaStream_t st = as_stream(stream);
+  coh_gemm_kernel<0><<<ggrid, 256, 0, st>>>(eig, reinterpret_cast<const double2*>(ddyn), freqs, n_band, c * c, w_buf);
+  count_launch();
+  coh_gemm_kernel<1><<<ggrid, 256, 0, st>>>(eig, w_buf, freqs, n_band, c * c, v_buf);
+  count_launch();
+  const int chunks = std::min(CHG_WIGNER_MAX_CHUNKS, n_q);
+  coh_pair_kernel<<<dim3(chunks, (unsigned)t_tiles), COH_THREADS, 0, st>>>(freqs, set_id, v_buf, heat_capacity, gamma,
+                                                                          n_q, n_band, n_t, cutoff_thz, partial);
+  CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_t * 6, SymmetricStore{kappa}, st));
   CHG_LAUNCH_END();
 }

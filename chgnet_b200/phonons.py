@@ -17,7 +17,8 @@
   (``powder_spectrum``), with ``chg_structure_factors`` and ``chg_broadened_spectrum``; with third-order force
   constants (``third_order_force_constants``), three-phonon interaction strengths (``chg_phonon_interaction``),
   linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation;
-  frequency-resolved self-energies (``chg_self_energy_spectrum``) and anharmonic phonon spectral functions.
+  frequency-resolved self-energies (``chg_self_energy_spectrum``) and anharmonic phonon spectral functions; the Wigner
+  coherence term of the thermal conductivity (``chg_coherence_conductivity``).
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
@@ -35,8 +36,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from chgnet_b200._lib import (JDOS_MAX_CHUNKS, ise_scratch_doubles, ph3_scratch_doubles, se_scratch_doubles,
-                              sqw_scratch_doubles)
+from chgnet_b200._lib import (JDOS_MAX_CHUNKS, coherence_scratch_doubles, ise_scratch_doubles, ph3_scratch_doubles,
+                              se_scratch_doubles, sqw_scratch_doubles)
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -331,11 +332,17 @@ def _mesh_indices(mesh, q: np.ndarray) -> np.ndarray:
     return (idx[:, 0] * m[1] + idx[:, 1]) * m[2] + idx[:, 2]
 
 
+def _degenerate_set_ids(nu: torch.Tensor) -> torch.Tensor:
+    """int64 [..., 3n]: the degenerate set of each mode of nu [..., 3n] (ascending along the last axis), numbered from 0
+    along that axis: adjacent modes closer than ``DEGENERACY_THZ`` share a set."""
+    gap = (nu[..., 1:] - nu[..., :-1]).abs() >= DEGENERACY_THZ
+    return torch.cat([torch.zeros_like(gap[..., :1], dtype=torch.long), gap.long().cumsum(-1)], -1)
+
+
 def _degenerate_average(gamma: torch.Tensor, nu: torch.Tensor) -> torch.Tensor:
-    """gamma [T, 3n] averaged over each set of degenerate modes of nu [3n] (adjacent |d nu| < ``DEGENERACY_THZ``), and
-    0 for the modes below ``THERMAL_CUTOFF_THZ``."""
-    gap = (nu[1:] - nu[:-1]).abs() >= DEGENERACY_THZ
-    sid = torch.cat([torch.zeros(1, dtype=torch.long, device=nu.device), gap.long().cumsum(0)])
+    """gamma [T, 3n] averaged over each set of degenerate modes of nu [3n] (``_degenerate_set_ids``), and 0 for the
+    modes below ``THERMAL_CUTOFF_THZ``."""
+    sid = _degenerate_set_ids(nu)
     n_sets = int(sid[-1]) + 1
     sums = torch.zeros(gamma.shape[0], n_sets, dtype=gamma.dtype, device=gamma.device).index_add_(1, sid, gamma)
     counts = torch.bincount(sid, minlength=n_sets).to(gamma.dtype)
@@ -345,8 +352,7 @@ def _degenerate_average(gamma: torch.Tensor, nu: torch.Tensor) -> torch.Tensor:
 def _degenerate_operators(nu: torch.Tensor) -> torch.Tensor:
     """[N, 3n, 3n]: per row of nu [N, 3n] the matrix that averages over its degenerate sets (the grouping of
     ``_degenerate_average``), A[q, i, j] = 1 / |set| when modes i and j of q share a set, else 0 (symmetric)."""
-    gap = (nu[:, 1:] - nu[:, :-1]).abs() >= DEGENERACY_THZ
-    sid = torch.cat([torch.zeros(nu.shape[0], 1, dtype=torch.long, device=nu.device), gap.long().cumsum(1)], 1)
+    sid = _degenerate_set_ids(nu)
     same = (sid[:, :, None] == sid[:, None, :]).to(nu.dtype)
     return same / same.sum(-1, keepdim=True)
 
@@ -429,6 +435,9 @@ class Phonons:
     lbte_matrix_bytes = 8 << 30
     # spectral_function: report frequencies evaluated per pass (the interpolation and Hilbert matrices are [F, M])
     spectrum_points_per_pass = 4096
+    # thermal_conductivity_wigner: q per chg_coherence_conductivity call keep dD/dQ and the call's scratch below this
+    # many bytes (at least one q)
+    wigner_chunk_bytes = 1 << 28
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, fc3=None, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -534,9 +543,8 @@ class Phonons:
             m = e.conj().transpose(1, 2)[:, None] @ dd @ e[:, None]  # [nq, 3, n3, n3]
             dlam = torch.diagonal(m, dim1=-2, dim2=-1).real.clone()  # [nq, 3, n3]
             # degenerate sets: set ids ascending along the (ascending) modes
-            gap = (nu[:, 1:] - nu[:, :-1]).abs() >= DEGENERACY_THZ
-            sid = torch.cat([torch.zeros(nq, 1, dtype=torch.long, device=dev), gap.long().cumsum(1)], dim=1)
-            idx = torch.nonzero((~gap).any(dim=1)).flatten()
+            sid = _degenerate_set_ids(nu)
+            idx = torch.nonzero((sid[:, 1:] == sid[:, :-1]).any(dim=1)).flatten()
             if idx.numel():
                 ids = sid[idx]
                 mb = m[idx] * (ids[:, :, None] == ids[:, None, :])[:, None]  # block diagonal, one block per set
@@ -1137,6 +1145,55 @@ class Phonons:
                 "linewidths": gamma.cpu().numpy(), "group_velocities": v.cpu().numpy(),
                 "heat_capacity": cv.cpu().numpy(), "n_imaginary": n_imaginary,
                 "n_zero_linewidth": (kept[None] & ~(gamma > 0)).sum(dim=(1, 2)).cpu().numpy()}
+
+    def thermal_conductivity_wigner(self, mesh, temperatures) -> dict:
+        """Lattice thermal conductivity with the Wigner coherence term (Simoncelli, Marzari and Mauri, Nat. Phys. 15,
+        809 (2019)) on the full Gamma-centred ``mesh``, every mesh point a target, in W/(m K) (DESIGN.md section
+        12.10): kappa = kappa_P + kappa_C, kappa_P ``thermal_conductivity``'s kappa (bitwise: the same linewidths and
+        the same sum) and
+
+            kappa_C(T) = 1 / (N V0) sum_q sum_{s != s'} (nu_s + nu_s') / 4 (C_s / nu_s + C_s' / nu_s')
+                         Re(V_s,s' (x) V_s',s) (Gamma_s + Gamma_s') / (2 pi [(nu_s - nu_s')^2 + (Gamma_s + Gamma_s')^2])
+
+        with V_s,s' = c^2 <e_s| dD/dQ |e_s'> / (|nu_s| + |nu_s'|) the velocity operator (THz A, c =
+        ``THZ_PER_SQRT_EV_A2_AMU``; its diagonal is the group velocity of a non-degenerate mode), C and Gamma the heat
+        capacities and degenerate-averaged linewidths of ``thermal_conductivity``.  The pairs are the ordered pairs of
+        modes that ``thermal_conductivity`` keeps (nu >= ``THERMAL_CUTOFF_THZ``, not the three acoustic modes at Gamma,
+        Gamma > 0) and that lie in different degenerate sets (adjacent |d nu| < ``DEGENERACY_THZ``): a pair inside a
+        set depends on the basis eigh picks in it, and the set's basis-invariant part is already in kappa_P.
+
+        Returns everything ``thermal_conductivity`` returns, with ``kappa`` = kappa_P + kappa_C, plus ``kappa_p`` and
+        ``kappa_c`` [T, 3, 3].  Needs ``force_constants3``, else ValueError; bad temperatures raise ValueError.  dD/dQ
+        (``chg_dynamical_matrix_derivatives``) and the pair sum (``chg_coherence_conductivity``) run on the device per
+        chunk of q within ``wigner_chunk_bytes``."""
+        if temperatures is None:
+            raise ValueError("thermal_conductivity_wigner needs temperatures")
+        mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        dev = self.device
+        t = torch.as_tensor(temps).to(dev)
+        gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, i) for i in range(nu.shape[0])], 1)
+        res = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+        cv = torch.as_tensor(res["heat_capacity"]).to(dev)
+        sid = _degenerate_set_ids(nu).to(torch.int32)
+        q = gamma_mesh(mesh)
+        n_mesh, nb = nu.shape
+        per_q = 16 * 3 * nb * nb + 8 * coherence_scratch_doubles(1, nb, 0)
+        chunk = int(max(1, min(65535, (self.wigner_chunk_bytes - 8 * coherence_scratch_doubles(0, nb, len(temps)))
+                               // per_q)))
+        kappa_c = torch.zeros(len(temps), 3, 3, dtype=torch.float64, device=dev)
+        for s in range(0, n_mesh, chunk):
+            sl = slice(s, s + chunk)
+            qd = torch.as_tensor(q[sl]).to(dev)
+            dd = torch.empty(qd.shape[0], 3, nb, nb, dtype=torch.complex128, device=dev)
+            self.kernels.dynamical_matrix_derivatives(self._fc, self._img_ptr, self._img_vec, self._s2p,
+                                                      self._inv_sqrt_m, qd, self._lattice, dd)
+            self.kernels.coherence_conductivity(nu[sl], e[sl], dd, sid[sl], cv[:, sl].contiguous(),
+                                                gamma[:, sl].contiguous(), THERMAL_CUTOFF_THZ, kappa_c)
+        vol = abs(float(np.linalg.det(self.cell.prim_lattice)))
+        res["kappa_p"] = res["kappa"]
+        res["kappa_c"] = (kappa_c * (KAPPA_W_PER_MK / (n_mesh * vol))).cpu().numpy()
+        res["kappa"] = res["kappa_p"] + res["kappa_c"]
+        return res
 
     def _collision_passes(self, mesh, nu, e, tets, t, groups):
         """One pass over the targets per group of temperature indices in ``groups`` (P remade per pass).  Yields

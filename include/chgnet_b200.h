@@ -680,6 +680,21 @@ int chg_self_energy_spectrum(const double* freqs, int32_t n_band, int32_t n1, in
                              const int32_t* q1_idx, int32_t n_q1, const double* p, const double* temperatures,
                              int32_t n_t, double cutoff_thz, double* work, int64_t work_doubles, double* gamma,
                              void* stream);
+/* Wigner coherence conductivity pair sum (DESIGN.md section 12.10), unscaled: kappa [n_t][3][3] +=
+ *   sum over q and the ordered pairs (s, s') of (nu_s + nu_s') / 4 (C_s / nu_s + C_s' / nu_s') Re(V_a[s][s'] V_b[s'][s])
+ *   (Gamma_s + Gamma_s') / (2 pi [(nu_s - nu_s')^2 + (Gamma_s + Gamma_s')^2]),
+ *   V_a[s][s'] = c^2 <e_s| dD/dQ_a |e_s'> / (|nu_s| + |nu_s'|),  c = 15.633304 THz / sqrt(eV / (A^2 amu)),
+ * over the pairs whose two modes have nu >= cutoff_thz and Gamma > 0 (per temperature) and lie in different degenerate
+ * sets (set_id differs).  freqs [n_q][n_band] THz (fp64; the Gamma acoustic modes already 0); eigvecs [n_q][mode]
+ * [n_band] interleaved complex128, mode-major; ddyn [n_q][3][n_band][n_band] complex128 as
+ * chg_dynamical_matrix_derivatives writes it; set_id [n_q][n_band] int32; heat_capacity (eV/K) and gamma (THz)
+ * [n_t][n_q][n_band] fp64.  n_q <= 65535.  work: at least 12 n_q n_band^2 + CHG_WIGNER_MAX_CHUNKS n_t 6 doubles
+ * (work_doubles).  Deterministic: per-block partial sums added in a fixed order, no atomics.                      */
+#define CHG_WIGNER_MAX_CHUNKS 256
+int chg_coherence_conductivity(const double* freqs, const double* eigvecs, const double* ddyn, const int32_t* set_id,
+                               const double* heat_capacity, const double* gamma, int32_t n_q, int32_t n_band,
+                               int32_t n_t, double cutoff_thz, double* work, int64_t work_doubles, double* kappa,
+                               void* stream);
 
 #ifdef __cplusplus
 }
