@@ -79,6 +79,7 @@ SIGNATURES: dict[str, list] = {
     "chg_collision_rows": [P, I, I, I, I, P, I, P, P, I, P, P, I, D, P, I64, P, P],
     "chg_self_energy_spectrum": [P, I, I, I, I, P, I, P, I, P, I, P, P, I, D, P, I64, P, P],
     "chg_coherence_conductivity": [P, P, P, P, P, P, I, I, I, D, P, I64, P, P],
+    "chg_isotope_scattering": [P, P, I, I, I, I, P, P, I, P, I, P, D, P, P, I64, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -145,6 +146,17 @@ def coherence_scratch_doubles(n_q, n_band, n_t):
     """The scratch of one ``chg_coherence_conductivity`` call: W = dD/dQ E and the velocity operator V, two
     [n_q, 3, n_band, n_band] complex buffers, and ``WIGNER_MAX_CHUNKS`` chunks of [n_t, 6] partial sums."""
     return 12 * n_q * n_band**2 + WIGNER_MAX_CHUNKS * n_t * 6
+
+
+# CHG_ISO_MAX_CHUNKS: the most chunks chg_isotope_scattering's partial sums use (tests/test_isotope_spec.py ties it to
+# the header)
+ISO_MAX_CHUNKS = 128
+
+
+def isotope_scratch_doubles(n_target, n_q, n_band):
+    """The scratch of one ``chg_isotope_scattering`` call: the overlaps [n_target, n_q, n_band, n_band] and
+    ``ISO_MAX_CHUNKS`` chunks of [n_target, n_band] partial sums."""
+    return n_target * n_q * n_band**2 + ISO_MAX_CHUNKS * n_target * n_band
 
 _lib = None
 
@@ -687,6 +699,27 @@ class CudaKernels:
         work = torch.empty(max(1, coherence_scratch_doubles(n_q, nb, n_t)), dtype=f64, device=freqs.device)
         self._call("chg_coherence_conductivity", _p(freqs), _p(eigvecs), _p(ddyn), _p(set_id), _p(heat_capacity),
                    _p(gamma), n_q, nb, n_t, float(cutoff_thz), _p(work), work.numel(), _p(kappa))
+
+    def isotope_scattering(self, freqs, mesh, tetrahedra, eigvecs, mass_variances, targets, omega, cutoff_thz, gamma):
+        """gamma [Q, n_band] fp64 (overwritten) = the isotope scattering rates (half width, THz) of the targets' modes at
+        w = omega [Q, n_band], before degenerate averaging (``chg_isotope_scattering``, DESIGN.md section 12.11):
+        freqs [n1 n2 n3, n_band] THz and eigvecs [n1 n2 n3, mode, n_band] complex128 (mode-major) of the full
+        Gamma-centred ``mesh``, tetrahedra [6, 4, 3] int32, mass_variances [n_band / 3] fp64, targets [Q] int32 mesh
+        indices; vertex modes below cutoff_thz take no part, and w below cutoff_thz gives 0."""
+        self._chk(freqs, tetrahedra, eigvecs, mass_variances, targets, omega, gamma)
+        n1, n2, n3 = _mesh_args("isotope_scattering", mesh, freqs, tetrahedra,
+                                "freqs, mass_variances, omega and gamma", (freqs, mass_variances, omega, gamma))
+        n_q, nb = freqs.shape
+        n_target = targets.shape[0]
+        if (eigvecs.dtype != torch.complex128 or tuple(eigvecs.shape) != (n_q, nb, nb) or nb % 3
+                or tuple(mass_variances.shape) != (nb // 3,) or targets.dtype != torch.int32 or targets.dim() != 1
+                or tuple(omega.shape) != (n_target, nb) or tuple(gamma.shape) != (n_target, nb)):
+            raise ChgnetB200Error(f"isotope_scattering: eigvecs must be complex128 [{n_q}, {nb}, {nb}], mass_variances "
+                                  f"[{nb // 3}], targets int32 [Q], omega and gamma [Q, {nb}]")
+        work = torch.empty(max(1, isotope_scratch_doubles(n_target, n_q, nb)), dtype=torch.float64, device=freqs.device)
+        self._call("chg_isotope_scattering", _p(freqs), _p(eigvecs), nb, n1, n2, n3, _p(tetrahedra),
+                   _p(mass_variances), nb // 3, _p(targets), n_target, _p(omega), float(cutoff_thz), _p(gamma),
+                   _p(work), work.numel())
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

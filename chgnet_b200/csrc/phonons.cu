@@ -1499,6 +1499,118 @@ struct SymmetricStore {  // work[chunk][t][6] (xx, yy, zz, yz, xz, xy): kappa[t]
   }
 };
 
+// ---------------------------------------------------------------------------------------------------------------
+// Isotope scattering (DESIGN.md section 12.11).  For target t of the call (mesh index targets[t]) and band l at the
+// frequency w = omega[t][l]:
+//   gamma[t][l] = (pi / 4) w^2 (1 / 6N) sum over the tetrahedra T of the mesh and the bands l' of
+//                 sum_v wt_v(w; T, l') O[t][q_v][l'][l],
+//   O[t][q'][l'][l] = sum_k g_k |sum_a conj(e_ka(t, l)) e_ka(q', l')|^2   (0 where freqs[q'][l'] < cutoff),
+// wt_v tetra_weights' corner weight of corner q_v for the corner values freqs[q_v][l'].  Summed per tetrahedron this is
+// (1/N) sum_q' W_l'(q'; w) O with W the vertex weight 1/6 sum over the 24 (tetrahedron, corner) at q'.  Gamma = 0 where
+// w < cutoff.  iso_overlap_kernel: one thread per element of O [t][q'][l'][l], l fastest.  iso_accumulate_kernel:
+// block (chunk of (tetrahedron, l') items, band tile, target); each tile of items is sorted into shared memory as in
+// tetrahedron_dos_kernel, then thread (slice s, band l) adds the items s, s + S, ... of the tile at its own w, reading
+// O coalesced along l; the slices are added in order in shared memory and the block writes work[chunk][t][l].
+// chunk_reduce_kernel adds the chunks in chunk order and applies (pi / 4) w^2 / 6N.  The chunks depend on the mesh and
+// the band count only, so a target's result does not depend on the other targets of the call.  No atomics.
+constexpr int ISO_THREADS = 256;  // threads per block, and items staged per tile
+
+__global__ void __launch_bounds__(ISO_THREADS)
+iso_overlap_kernel(const double2* __restrict__ eig, const double* __restrict__ freqs, int n_band, int n_q,
+                   const double* __restrict__ g, int n_prim, const int32_t* __restrict__ targets, int n_target,
+                   double cutoff, double* __restrict__ overlap) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nb2 = (int64_t)n_band * n_band, per_t = (int64_t)n_q * nb2;
+  if (i >= (int64_t)n_target * per_t) return;
+  const int t = (int)(i / per_t), q = (int)((i / nb2) % n_q), lp = (int)((i / n_band) % n_band);
+  const int l = (int)(i % n_band);
+  double o = 0.0;
+  if (__ldg(freqs + (size_t)q * n_band + lp) >= cutoff) {
+    const double2* a = eig + ((size_t)__ldg(targets + t) * n_band + l) * n_band;
+    const double2* b = eig + ((size_t)q * n_band + lp) * n_band;
+    for (int k = 0; k < n_prim; ++k) {
+      double re = 0.0, im = 0.0;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const double2 x = __ldg(a + 3 * k + c), y = __ldg(b + 3 * k + c);
+        re = fma(x.x, y.x, fma(x.y, y.y, re));
+        im = fma(x.x, y.y, fma(-x.y, y.x, im));
+      }
+      o = fma(__ldg(g + k), fma(re, re, im * im), o);
+    }
+  }
+  overlap[i] = o;
+}
+
+__global__ void __launch_bounds__(ISO_THREADS)
+iso_accumulate_kernel(const double* __restrict__ freqs, int n_band, int n1, int n2, int n3,
+                      const int32_t* __restrict__ tet, const double* __restrict__ omega,
+                      const double* __restrict__ overlap, int n_target, int l_tile, double cutoff,
+                      double* __restrict__ work) {
+  __shared__ double se[ISO_THREADS][4];
+  __shared__ int32_t sq[ISO_THREADS][4];
+  __shared__ int32_t sb[ISO_THREADS];
+  __shared__ double red[ISO_THREADS];
+  const int t = blockIdx.z;
+  const int n_slices = ISO_THREADS / l_tile;
+  const int s = threadIdx.x / l_tile, l = blockIdx.y * l_tile + threadIdx.x % l_tile;
+  const bool active = s < n_slices && l < n_band;
+  const double w = active ? __ldg(omega + (size_t)t * n_band + l) : 0.0;
+  const bool live = active && w >= cutoff;
+  const int64_t n_q = (int64_t)n1 * n2 * n3, nb2 = (int64_t)n_band * n_band;
+  const double* o_t = overlap + (size_t)t * n_q * nb2 + l;
+  const int64_t n_items = n_q * 6 * n_band;
+  const int64_t n_tiles = (n_items + ISO_THREADS - 1) / ISO_THREADS;
+  const int64_t t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  double acc = 0.0;
+  for (int64_t tile = n_tiles * blockIdx.x / gridDim.x; tile < t_end; ++tile) {
+    const int64_t p = tile * ISO_THREADS + threadIdx.x;
+    __syncthreads();  // the previous tile has been read
+    if (p < n_items) {
+      const int band = (int)(p % n_band);
+      double e[4];
+      int32_t q[4];
+      tetrahedron_corners(tet, p / n_band, n1, n2, n3, [&](int v, int a, int b, int c) {
+        q[v] = (a * n2 + b) * n3 + c;
+        e[v] = __ldg(freqs + (int64_t)q[v] * n_band + band);
+      });
+      sort4(e, q);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) se[threadIdx.x][v] = e[v], sq[threadIdx.x][v] = q[v];
+      sb[threadIdx.x] = band;
+    }
+    __syncthreads();
+    if (!live) continue;
+    const int n_here = (int)min((int64_t)ISO_THREADS, n_items - tile * ISO_THREADS);
+    for (int i = s; i < n_here; i += n_slices) {
+      const double e[4] = {se[i][0], se[i][1], se[i][2], se[i][3]};
+      if (!(w >= e[0] && w < e[3])) continue;
+      double n, gw, wt[4];
+      tetra_weights(w, e, n, gw, wt);
+      const int64_t lp = sb[i];
+#pragma unroll
+      for (int v = 0; v < 4; ++v) acc = fma(wt[v], __ldg(o_t + (sq[i][v] * n_band + lp) * n_band), acc);
+    }
+  }
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  if (active && s == 0) {
+    double sum = 0.0;
+    for (int k = 0; k < n_slices; ++k) sum += red[k * l_tile + threadIdx.x];
+    work[((size_t)blockIdx.x * n_target + t) * n_band + l] = sum;
+  }
+}
+
+struct IsotopeStore {  // work[chunk][t][l]: gamma[t][l] = scale * omega[t][l]^2 * the sum
+  double* gamma;
+  const double* omega;
+  double scale;
+  __device__ void operator()(int64_t o, double s) const {
+    const double w = omega[o];
+    gamma[o] = s * (scale * w * w);
+  }
+};
+
 }  // namespace
 }  // namespace chg
 
@@ -1823,5 +1935,38 @@ extern "C" int chg_coherence_conductivity(const double* freqs, const double* eig
   coh_pair_kernel<<<dim3(chunks, (unsigned)t_tiles), COH_THREADS, 0, st>>>(freqs, set_id, v_buf, heat_capacity, gamma,
                                                                           n_q, n_band, n_t, cutoff_thz, partial);
   CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_t * 6, SymmetricStore{kappa}, st));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_isotope_scattering(const double* freqs, const double* eigvecs, int32_t n_band, int32_t n1,
+                                      int32_t n2, int32_t n3, const int32_t* tetrahedra, const double* mass_variances,
+                                      int32_t n_prim, const int32_t* targets, int32_t n_target, const double* omega,
+                                      double cutoff_thz, double* gamma, double* work, int64_t work_doubles,
+                                      void* stream) {
+  CHG_CHECK_ARG(n_band >= 0 && n1 > 0 && n2 > 0 && n3 > 0 && n_prim >= 0 && n_target >= 0, "bad size");
+  CHG_CHECK_ARG(n_band == 3 * n_prim, "n_band must be 3 n_prim");
+  const int64_t n_q = (int64_t)n1 * n2 * n3;
+  CHG_CHECK_ARG(n_q * 6 * std::max(n_band, 1) < (1ll << 31), "mesh too large");
+  CHG_CHECK_ARG(n_target <= 65535, "too many targets in one call (at most 65535)");
+  if (n_band == 0 || n_target == 0) return CHG_OK;
+  CHG_CHECK_ARG(freqs && eigvecs && tetrahedra && mass_variances && targets && omega && gamma && work, "null pointer");
+  const int64_t n_o = (int64_t)n_target * n_q * n_band * n_band;
+  CHG_CHECK_ARG(work_doubles >= n_o + (int64_t)CHG_ISO_MAX_CHUNKS * n_target * n_band,
+                "work holds less than n_target N n_band^2 + CHG_ISO_MAX_CHUNKS n_target n_band doubles");
+  double* partial = work + n_o;
+  cudaStream_t st = as_stream(stream);
+  iso_overlap_kernel<<<(unsigned)((n_o + ISO_THREADS - 1) / ISO_THREADS), ISO_THREADS, 0, st>>>(
+      reinterpret_cast<const double2*>(eigvecs), freqs, n_band, (int)n_q, mass_variances, n_prim, targets, n_target,
+      cutoff_thz, work);
+  count_launch();
+  const int l_tile = std::min(n_band, ISO_THREADS);
+  const int l_tiles = (n_band + l_tile - 1) / l_tile;
+  // at most CHG_ISO_MAX_CHUNKS chunks of item tiles, at least one tile each: a function of the mesh and n_band only
+  const int64_t n_tiles = (n_q * 6 * n_band + ISO_THREADS - 1) / ISO_THREADS;
+  const int chunks = (int)std::min<int64_t>(CHG_ISO_MAX_CHUNKS, n_tiles);
+  iso_accumulate_kernel<<<dim3(chunks, (unsigned)l_tiles, (unsigned)n_target), ISO_THREADS, 0, st>>>(
+      freqs, n_band, n1, n2, n3, tetrahedra, omega, work, n_target, l_tile, cutoff_thz, partial);
+  const double scale = 3.141592653589793 / (4.0 * 6.0 * (double)n_q);
+  CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_target * n_band, IsotopeStore{gamma, omega, scale}, st));
   CHG_LAUNCH_END();
 }

@@ -18,7 +18,8 @@
   constants (``third_order_force_constants``), three-phonon interaction strengths (``chg_phonon_interaction``),
   linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation;
   frequency-resolved self-energies (``chg_self_energy_spectrum``) and anharmonic phonon spectral functions; the Wigner
-  coherence term of the thermal conductivity (``chg_coherence_conductivity``).
+  coherence term of the thermal conductivity (``chg_coherence_conductivity``); isotope scattering rates
+  (``chg_isotope_scattering``, no fc3 needed) and isotope and boundary scattering in every thermal conductivity.
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
@@ -36,8 +37,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from chgnet_b200._lib import (JDOS_MAX_CHUNKS, coherence_scratch_doubles, ise_scratch_doubles, ph3_scratch_doubles,
-                              se_scratch_doubles, sqw_scratch_doubles)
+from chgnet_b200._lib import (JDOS_MAX_CHUNKS, coherence_scratch_doubles, ise_scratch_doubles, isotope_scratch_doubles,
+                              ph3_scratch_doubles, se_scratch_doubles, sqw_scratch_doubles)
 from chgnet_b200.dynamics import ATOMIC_MASSES, KB
 
 # sqrt(eV / (A^2 amu)) / 2 pi in THz, CODATA 2018 (phonopy's older constant is 15.633302)
@@ -357,6 +358,13 @@ def _degenerate_operators(nu: torch.Tensor) -> torch.Tensor:
     return same / same.sum(-1, keepdim=True)
 
 
+def _set_average(x: torch.Tensor, nu: torch.Tensor) -> torch.Tensor:
+    """x [N, 3n] averaged over the degenerate sets of each row of nu [N, 3n] (``_degenerate_operators``), and 0 for the
+    modes below ``THERMAL_CUTOFF_THZ``."""
+    avg = (_degenerate_operators(nu) @ x[..., None])[..., 0]
+    return torch.where(nu >= THERMAL_CUTOFF_THZ, avg, 0.0)
+
+
 def _hat_matrix(x: torch.Tensor, grid: torch.Tensor, h: float) -> torch.Tensor:
     """[X, M]: the hat functions max(0, 1 - |x - w_k| / h) of the uniform ``grid`` w_k = k h [M] at the points ``x``
     [X]; Gamma_hat(x) = this @ Gamma_k, the piecewise-linear interpolant, 0 beyond the last hat."""
@@ -438,6 +446,9 @@ class Phonons:
     # thermal_conductivity_wigner: q per chg_coherence_conductivity call keep dD/dQ and the call's scratch below this
     # many bytes (at least one q)
     wigner_chunk_bytes = 1 << 28
+    # isotope_linewidths and the mass_variances of the conductivities: targets per chg_isotope_scattering call keep
+    # its overlaps, scratch and output below this many bytes (at least one target)
+    isotope_chunk_bytes = 1 << 28
 
     def __init__(self, force_constants: np.ndarray, sc: Supercell, *, fc3=None, device="cuda", kernels=None) -> None:
         if kernels is None:
@@ -911,6 +922,12 @@ class Phonons:
             raise ValueError("this needs third-order force constants: build the phonons with "
                              "CHGNet.phonons(..., third_order=True), or pass fc3 to Phonons")
         temps = None if temperatures is None else _temperatures(temperatures)
+        return (*self._mesh_modes(mesh), temps)
+
+    def _mesh_modes(self, mesh):
+        """The mesh, its frequencies [N, 3n] on the device with the three modes of smallest |nu| at Gamma set to 0, the
+        mode-major eigenvectors [N, mode, 3n], ``n_imaginary`` (counted before that) and the tetrahedra: one
+        eigendecomposition of the mesh in chunks of at most ``eigh_batch`` q."""
         mesh = tuple(int(n) for n in np.asarray(mesh).reshape(-1))
         q = gamma_mesh(mesh)
         n3, dev = 3 * len(self.p2s), self.device
@@ -922,7 +939,7 @@ class Phonons:
         n_imaginary = int((nu < -THERMAL_CUTOFF_THZ).sum())
         _zero_gamma_acoustic(nu)
         tets = torch.as_tensor(tetrahedra(mesh, self.cell.prim_lattice)).to(dev)
-        return mesh, nu, e, n_imaginary, tets, temps
+        return mesh, nu, e, n_imaginary, tets
 
     def _q1_chunk(self, n_t) -> int:
         """q1 per ``chg_phonon_interaction`` / ``chg_imag_self_energy`` call: P, both calls' scratch within
@@ -1007,6 +1024,70 @@ class Phonons:
         if single:
             res["frequencies"], res["linewidths"] = res["frequencies"][0], res["linewidths"][:, 0]
         return res
+
+    def _mass_variances(self, mass_variances) -> torch.Tensor:
+        """``mass_variances`` as [n_prim] fp64 on the device; ValueError unless they are n_prim finite values >= 0."""
+        n_prim = len(self.p2s)
+        g = np.asarray(mass_variances, dtype=np.float64).reshape(-1)
+        if g.shape != (n_prim,) or not np.all(np.isfinite(g)) or np.any(g < 0):
+            raise ValueError(f"mass_variances must be {n_prim} finite values >= 0 (one per primitive atom), got "
+                             f"{np.asarray(mass_variances).tolist()}")
+        return torch.as_tensor(g).to(self.device)
+
+    def _isotope_targets(self, mesh, nu, e, tets, g, idx) -> torch.Tensor:
+        """Gamma^iso [Q, 3n] (THz) of the mesh indices ``idx`` [Q] at their own frequencies, averaged over the
+        degenerate sets of each: ``chg_isotope_scattering`` per chunk of targets within ``isotope_chunk_bytes``."""
+        n_mesh, nb = nu.shape
+        per_target = 8 * (isotope_scratch_doubles(1, n_mesh, nb) + nb)
+        chunk = int(max(1, min(65535, self.isotope_chunk_bytes // per_target)))
+        targets = torch.as_tensor(np.asarray(idx, dtype=np.int32)).to(self.device)
+        omega = nu[targets.long()].contiguous()
+        gamma = torch.empty_like(omega)
+        for s in range(0, len(targets), chunk):
+            self.kernels.isotope_scattering(nu, mesh, tets, e, g, targets[s : s + chunk], omega[s : s + chunk],
+                                            THERMAL_CUTOFF_THZ, gamma[s : s + chunk])
+        return _set_average(gamma, omega)
+
+    def isotope_linewidths(self, mesh, qpoints, mass_variances) -> dict:
+        """Isotope (mass-disorder) scattering rates of Tamura (PRB 27, 858 (1983)), half width in THz, of the modes at
+        ``qpoints`` ([Q, 3] or [3], reduced, on the full Gamma-centred ``mesh``: q * mesh integral to 1e-8, else
+        ValueError), DESIGN.md section 12.11:
+
+            Gamma^iso_l(q) = (pi / 4) nu_l^2 (1/N) sum_{q' l'} W_l'(q'; nu_l) sum_k g_k |sum_a conj(e_ka(q l)) e_ka(q' l')|^2
+
+        with W the linear-tetrahedron vertex weight of d(nu - nu_l'(q')) (the tetrahedra of ``dos``) and g_k =
+        sum_i f_i (1 - m_i / m_k)^2 the ``mass_variances`` of the primitive atoms (phono3py's ``--mass_variances``;
+        n_prim finite values >= 0, else ValueError).  Vertex modes below ``THERMAL_CUTOFF_THZ`` take no part; modes
+        below it, and the three modes of smallest |nu| at Gamma, get 0; Gamma^iso is averaged over each set of
+        degenerate modes at q (adjacent |d nu| < ``DEGENERACY_THZ``) and does not depend on temperature.  Harmonic:
+        no third-order force constants are needed.
+
+        Returns ``frequencies`` [Q, 3n] (THz, with that Gamma rule), ``isotope_linewidths`` [Q, 3n] and
+        ``n_imaginary`` (the modes below -``THERMAL_CUTOFF_THZ`` over the mesh); a single q drops the Q axis.  The
+        mesh is diagonalised once per call, and the sums (``chg_isotope_scattering``) run on the device per chunk of
+        targets within ``isotope_chunk_bytes``."""
+        q = np.asarray(qpoints, dtype=np.float64)
+        single = q.ndim == 1
+        q = q.reshape(-1, 3)
+        idx = _mesh_indices(mesh, q)
+        g = self._mass_variances(mass_variances)
+        mesh, nu, e, n_imaginary, tets = self._mesh_modes(mesh)
+        gamma = self._isotope_targets(mesh, nu, e, tets, g, idx)
+        res = {"frequencies": nu[torch.as_tensor(idx).to(self.device)].cpu().numpy(),
+               "isotope_linewidths": gamma.cpu().numpy(), "n_imaginary": n_imaginary}
+        if single:
+            res["frequencies"], res["isotope_linewidths"] = res["frequencies"][0], res["isotope_linewidths"][0]
+        return res
+
+    def _extra_scattering(self, mesh, nu, e, tets, mass_variances, boundary_mfp):
+        """The checked options of the conductivities: (Gamma^iso [N, 3n] of every mesh point or None, L or None)."""
+        g = None if mass_variances is None else self._mass_variances(mass_variances)
+        if boundary_mfp is not None:
+            boundary_mfp = float(boundary_mfp)
+            if not (math.isfinite(boundary_mfp) and boundary_mfp > 0):
+                raise ValueError(f"boundary_mfp must be finite and positive (micrometres), got {boundary_mfp!r}")
+        iso = None if g is None else self._isotope_targets(mesh, nu, e, tets, g, np.arange(nu.shape[0]))
+        return iso, boundary_mfp
 
     def _spectrum_q1_chunk(self, n_t, n_freq) -> int:
         """q1 per ``chg_phonon_interaction`` / ``chg_self_energy_spectrum`` call in ``spectral_function``: P, the
@@ -1105,7 +1186,7 @@ class Phonons:
                 res[k] = res[k][:, 0]
         return res
 
-    def thermal_conductivity(self, mesh, temperatures) -> dict:
+    def thermal_conductivity(self, mesh, temperatures, *, mass_variances=None, boundary_mfp=None) -> dict:
         """Lattice thermal conductivity in the relaxation-time approximation on the full Gamma-centred ``mesh``, every
         mesh point a target (no symmetry reduction), in W/(m K):
 
@@ -1115,38 +1196,58 @@ class Phonons:
         Modes below ``THERMAL_CUTOFF_THZ`` (and the three modes of smallest |nu| at Gamma) are left out, and so are
         modes with Gamma <= 0, whose lifetime is undefined; ``n_zero_linewidth`` [T] counts those.
 
+        Isotope and boundary scattering (DESIGN.md section 12.11) add to Gamma by Matthiessen's rule: with
+        ``mass_variances`` (g per primitive atom, as ``isotope_linewidths``) Gamma^iso, with ``boundary_mfp`` (L, in
+        micrometres) Gamma^bnd = |v| / (4 pi 10^4 L), averaged over degenerate sets.  tau, the kept modes and
+        ``n_zero_linewidth`` then use Gamma + Gamma^iso + Gamma^bnd.
+
         Returns ``temperatures``, ``kappa`` [T, 3, 3], per mode ``frequencies`` [N, 3n] (THz), ``linewidths``
-        [T, N, 3n] (THz), ``group_velocities`` [N, 3n, 3] (THz A) and ``heat_capacity`` [T, N, 3n] (eV/K), and
-        ``n_imaginary`` and ``n_zero_linewidth``.  Needs ``force_constants3``, else ValueError; bad temperatures raise
-        ValueError."""
+        [T, N, 3n] (THz, three-phonon), ``group_velocities`` [N, 3n, 3] (THz A) and ``heat_capacity`` [T, N, 3n]
+        (eV/K), and ``n_imaginary`` and ``n_zero_linewidth``; with the options also ``isotope_linewidths`` and
+        ``boundary_linewidths`` [N, 3n] (THz).  Needs ``force_constants3``, else ValueError; bad temperatures,
+        ``mass_variances`` that are not n_prim finite values >= 0 and a ``boundary_mfp`` that is not finite and > 0
+        raise ValueError."""
         if temperatures is None:
             raise ValueError("thermal_conductivity needs temperatures")
         mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        iso, mfp = self._extra_scattering(mesh, nu, e, tets, mass_variances, boundary_mfp)
         dev = self.device
         t = torch.as_tensor(temps).to(dev)
         gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, i) for i in range(nu.shape[0])], 1)
-        return self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+        return self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary, iso, mfp)[0]
 
-    def _rta_conductivity(self, mesh, nu, gamma, t, temps, n_imaginary) -> dict:
-        """``thermal_conductivity``'s result from the mesh frequencies nu [N, 3n] and the linewidths gamma [T, N, 3n]
-        at the temperatures t (device) and temps (array)."""
+    def _rta_conductivity(self, mesh, nu, gamma, t, temps, n_imaginary, iso=None, boundary_mfp=None):
+        """(``thermal_conductivity``'s result, the total linewidths [T, N, 3n] on the device) from the mesh frequencies
+        nu [N, 3n], the three-phonon linewidths gamma [T, N, 3n] at the temperatures t (device) and temps (array), and
+        the isotope linewidths iso [N, 3n] and boundary mean free path (um) when given."""
         v = torch.as_tensor(self.group_velocities(gamma_mesh(mesh))).to(self.device)  # [N, 3n, 3]
+        extra = {}
+        if iso is not None:
+            extra["isotope_linewidths"] = iso
+        if boundary_mfp is not None:
+            speed = torch.where(nu >= THERMAL_CUTOFF_THZ, torch.linalg.vector_norm(v, dim=-1), 0.0)
+            extra["boundary_linewidths"] = _set_average(speed / (4 * math.pi * 1e4 * boundary_mfp), nu)
+        total = gamma
+        for x in extra.values():
+            total = total + x[None]
         kept = nu >= THERMAL_CUTOFF_THZ
         tt = t[:, None, None]
         x = H_OVER_KB_K_PER_THZ * torch.where(kept, nu, 1.0)[None] / torch.where(tt > 0, tt, 1.0)
         em = torch.exp(-x)
         cv = torch.where(kept[None] & (tt > 0), KB * x * x * em / torch.expm1(-x) ** 2, 0.0)  # [T, N, 3n]
-        use = kept[None] & (gamma > 0)
-        tau = torch.where(use, 1.0 / (4 * math.pi * torch.where(use, gamma, 1.0)), 0.0)
+        use = kept[None] & (total > 0)
+        tau = torch.where(use, 1.0 / (4 * math.pi * torch.where(use, total, 1.0)), 0.0)
         vv = v[:, :, :, None] * v[:, :, None, :]  # [N, 3n, 3, 3]
         vol = abs(float(np.linalg.det(self.cell.prim_lattice)))
         kappa = torch.einsum("tqm,qmab->tab", cv * tau, vv) * (KAPPA_W_PER_MK / (nu.shape[0] * vol))
-        return {"temperatures": temps, "kappa": kappa.cpu().numpy(), "frequencies": nu.cpu().numpy(),
-                "linewidths": gamma.cpu().numpy(), "group_velocities": v.cpu().numpy(),
-                "heat_capacity": cv.cpu().numpy(), "n_imaginary": n_imaginary,
-                "n_zero_linewidth": (kept[None] & ~(gamma > 0)).sum(dim=(1, 2)).cpu().numpy()}
+        res = {"temperatures": temps, "kappa": kappa.cpu().numpy(), "frequencies": nu.cpu().numpy(),
+               "linewidths": gamma.cpu().numpy(), "group_velocities": v.cpu().numpy(),
+               "heat_capacity": cv.cpu().numpy(), "n_imaginary": n_imaginary,
+               "n_zero_linewidth": (kept[None] & ~(total > 0)).sum(dim=(1, 2)).cpu().numpy()}
+        res.update({k: x.cpu().numpy() for k, x in extra.items()})
+        return res, total
 
-    def thermal_conductivity_wigner(self, mesh, temperatures) -> dict:
+    def thermal_conductivity_wigner(self, mesh, temperatures, *, mass_variances=None, boundary_mfp=None) -> dict:
         """Lattice thermal conductivity with the Wigner coherence term (Simoncelli, Marzari and Mauri, Nat. Phys. 15,
         809 (2019)) on the full Gamma-centred ``mesh``, every mesh point a target, in W/(m K) (DESIGN.md section
         12.10): kappa = kappa_P + kappa_C, kappa_P ``thermal_conductivity``'s kappa (bitwise: the same linewidths and
@@ -1157,22 +1258,25 @@ class Phonons:
 
         with V_s,s' = c^2 <e_s| dD/dQ |e_s'> / (|nu_s| + |nu_s'|) the velocity operator (THz A, c =
         ``THZ_PER_SQRT_EV_A2_AMU``; its diagonal is the group velocity of a non-degenerate mode), C and Gamma the heat
-        capacities and degenerate-averaged linewidths of ``thermal_conductivity``.  The pairs are the ordered pairs of
+        capacities and degenerate-averaged linewidths of ``thermal_conductivity`` (with ``mass_variances`` and
+        ``boundary_mfp`` as there, Gamma is the total of section 12.11 in the Lorentzians).  The pairs are the ordered pairs of
         modes that ``thermal_conductivity`` keeps (nu >= ``THERMAL_CUTOFF_THZ``, not the three acoustic modes at Gamma,
         Gamma > 0) and that lie in different degenerate sets (adjacent |d nu| < ``DEGENERACY_THZ``): a pair inside a
         set depends on the basis eigh picks in it, and the set's basis-invariant part is already in kappa_P.
 
-        Returns everything ``thermal_conductivity`` returns, with ``kappa`` = kappa_P + kappa_C, plus ``kappa_p`` and
-        ``kappa_c`` [T, 3, 3].  Needs ``force_constants3``, else ValueError; bad temperatures raise ValueError.  dD/dQ
+        Returns everything ``thermal_conductivity`` returns with the same options, with ``kappa`` = kappa_P + kappa_C,
+        plus ``kappa_p`` and ``kappa_c`` [T, 3, 3].  Needs ``force_constants3``, else ValueError; bad temperatures and
+        options raise ValueError as in ``thermal_conductivity``.  dD/dQ
         (``chg_dynamical_matrix_derivatives``) and the pair sum (``chg_coherence_conductivity``) run on the device per
         chunk of q within ``wigner_chunk_bytes``."""
         if temperatures is None:
             raise ValueError("thermal_conductivity_wigner needs temperatures")
         mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        iso, mfp = self._extra_scattering(mesh, nu, e, tets, mass_variances, boundary_mfp)
         dev = self.device
         t = torch.as_tensor(temps).to(dev)
         gamma = torch.stack([self._target_linewidths(mesh, nu, e, tets, t, i) for i in range(nu.shape[0])], 1)
-        res = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+        res, gamma = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary, iso, mfp)
         cv = torch.as_tensor(res["heat_capacity"]).to(dev)
         sid = _degenerate_set_ids(nu).to(torch.int32)
         q = gamma_mesh(mesh)
@@ -1239,7 +1343,8 @@ class Phonons:
         kept = (nu >= THERMAL_CUTOFF_THZ)[None] & (gamma > 0)
         return s, gamma, kept.reshape(len(temps), -1)
 
-    def thermal_conductivity_lbte(self, mesh, temperatures, *, pinv_cutoff=1e-8) -> dict:
+    def thermal_conductivity_lbte(self, mesh, temperatures, *, pinv_cutoff=1e-8, mass_variances=None,
+                                  boundary_mfp=None) -> dict:
         """Lattice thermal conductivity (W/(m K)) from the direct solution of the linearised phonon Boltzmann equation
         (Chaput, PRL 110, 265506 (2013)) on the full Gamma-centred ``mesh``, every mesh point a target (DESIGN.md
         section 12.8).  The collision matrix, symmetrised and in 1/ps,
@@ -1255,11 +1360,15 @@ class Phonons:
             kappa = 1 / (N V0) sum over eta_k > pinv_cutoff of (U^T X)_k (x) (U^T X)_k / eta_k
 
         which is ``thermal_conductivity``'s kappa when S = 0.  Eigenvalues <= ``pinv_cutoff`` (1/ps; the energy mode
-        near 0 and small negative ones) are left out and counted.  At T = 0 kappa is 0 and no matrix is built.
+        near 0 and small negative ones) are left out and counted.  At T = 0 kappa is 0 and no matrix is built.  With
+        ``mass_variances`` and ``boundary_mfp`` (as ``thermal_conductivity``) Gamma is the total of DESIGN.md section
+        12.11 on the diagonal and in the kept modes; S keeps the three-phonon processes only (as phono3py, the
+        off-diagonal part of elastic isotope scattering is left out).
 
         Returns ``temperatures``, ``kappa`` and ``kappa_rta`` [T, 3, 3] (the latter bitwise ``thermal_conductivity``'s
-        kappa), per mode ``frequencies``, ``linewidths``, ``group_velocities`` and ``heat_capacity`` as
-        ``thermal_conductivity``, ``n_imaginary``, ``n_zero_linewidth``, ``n_dropped`` [T] (eigenvalues <=
+        kappa with the same options), per mode ``frequencies``, ``linewidths``, ``group_velocities`` and ``heat_capacity`` as
+        ``thermal_conductivity`` (and its ``isotope_linewidths`` and ``boundary_linewidths`` with the options),
+        ``n_imaginary``, ``n_zero_linewidth``, ``n_dropped`` [T] (eigenvalues <=
         pinv_cutoff) and ``min_eigenvalue`` [T] (1/ps, NaN where no matrix was built).  The matrices of all
         temperatures above 0 are built in one pass over the targets when n_t M^2 8 bytes fit in ``lbte_matrix_bytes``
         (M: the modes at or above the cutoff), else in groups of temperatures with P remade per group; ValueError
@@ -1271,6 +1380,7 @@ class Phonons:
         if not (math.isfinite(cutoff) and cutoff >= 0):
             raise ValueError(f"pinv_cutoff must be finite and non-negative, got {pinv_cutoff!r}")
         mesh, nu, e, n_imaginary, tets, temps = self._three_phonon_mesh(mesh, temperatures)
+        iso, mfp = self._extra_scattering(mesh, nu, e, tets, mass_variances, boundary_mfp)
         n_mesh, nb = nu.shape
         dev, f64 = self.device, torch.float64
         t = torch.as_tensor(temps).to(dev)
@@ -1290,7 +1400,7 @@ class Phonons:
         kappa = torch.zeros(len(temps), 3, 3, dtype=f64, device=dev)
         n_dropped = np.zeros(len(temps), dtype=np.int64)
         min_eig = np.full(len(temps), np.nan)
-        res = x = s = None
+        res = x = s = total = None
         for group, target, g, rows in self._collision_passes(mesh, nu, e, tets, t, groups):
             if target == 0:
                 s = torch.zeros(len(group), m0, m0, dtype=f64, device=dev)
@@ -1304,11 +1414,11 @@ class Phonons:
             if target < n_mesh - 1:
                 continue
             if res is None:  # the end of the first pass: every Gamma is known
-                res = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary)
+                res, total = self._rta_conductivity(mesh, nu, gamma, t, temps, n_imaginary, iso, mfp)
                 x = (torch.as_tensor(res["heat_capacity"]).to(dev).sqrt()[..., None]
                      * torch.as_tensor(res["group_velocities"]).to(dev)[None]).reshape(len(temps), -1, 3)[:, cols]
             for j, ti in enumerate(group):
-                kappa[ti], n_dropped[ti], min_eig[ti] = self._lbte_solve(s[j], gamma[ti].reshape(-1)[cols], x[ti],
+                kappa[ti], n_dropped[ti], min_eig[ti] = self._lbte_solve(s[j], total[ti].reshape(-1)[cols], x[ti],
                                                                          cutoff)
             s = None
         vol = abs(float(np.linalg.det(self.cell.prim_lattice)))

@@ -695,6 +695,21 @@ int chg_coherence_conductivity(const double* freqs, const double* eigvecs, const
                                const double* heat_capacity, const double* gamma, int32_t n_q, int32_t n_band,
                                int32_t n_t, double cutoff_thz, double* work, int64_t work_doubles, double* kappa,
                                void* stream);
+/* Isotope (mass-disorder) scattering rates of Tamura (DESIGN.md section 12.11), half width in THz, before any
+ * degenerate averaging: for each target t (mesh index targets[t]) and band l at w = omega[t][l],
+ *   gamma [n_target][n_band] = (pi / 4) w^2 (1/N) sum_{q' l'} W_l'(q'; w) sum_k g_k |sum_a conj(e_ka(t, l)) e_ka(q', l')|^2
+ * (overwritten), W the linear-tetrahedron vertex weight of d(w - nu_l'(q')) (1/6 of the sum over the 24 (tetrahedron,
+ * corner) at q', tetrahedra as chg_joint_dos), N = n1 n2 n3; vertex modes with nu_l'(q') < cutoff_thz take no part,
+ * and gamma = 0 where w < cutoff_thz.  freqs [n1 n2 n3][n_band] THz (signed, ascending per q); eigvecs [n1 n2 n3][mode]
+ * [n_band] interleaved complex128, mode-major; mass_variances [n_prim] g_k = sum_i f_i (1 - m_i / m_k)^2; n_band =
+ * 3 n_prim; targets [n_target] int32, n_target <= 65535; omega [n_target][n_band] THz.  work: at least n_target N
+ * n_band^2 + CHG_ISO_MAX_CHUNKS n_target n_band doubles (work_doubles).  Deterministic: per-block partial sums added in
+ * a fixed order, no atomics; a target's result does not depend on the other targets of the call.                   */
+#define CHG_ISO_MAX_CHUNKS 128
+int chg_isotope_scattering(const double* freqs, const double* eigvecs, int32_t n_band, int32_t n1, int32_t n2,
+                           int32_t n3, const int32_t* tetrahedra, const double* mass_variances, int32_t n_prim,
+                           const int32_t* targets, int32_t n_target, const double* omega, double cutoff_thz,
+                           double* gamma, double* work, int64_t work_doubles, void* stream);
 
 #ifdef __cplusplus
 }
