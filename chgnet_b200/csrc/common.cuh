@@ -74,6 +74,17 @@ __device__ __forceinline__ float dsilu_f(float x) {
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void stg4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
+// ldg4 with L2 evict-first priority (createpolicy + .L2::cache_hint), for rows a kernel reads once at random, so that
+// they do not displace lines that other loads of the kernel still use
+__device__ __forceinline__ float4 ldg4_evict_first(const float* p) {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  float4 v;
+  asm("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+      : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+      : "l"(p), "l"(pol));
+  return v;
+}
 __device__ __forceinline__ float4 lds4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void sts4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
 

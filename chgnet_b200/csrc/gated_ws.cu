@@ -72,7 +72,8 @@ struct FusedArgs {
   float* save_p;        // [rows][128] or null
 };
 
-// pull one 128-byte line towards L2 (no register, no dependency): issued one tile ahead of the gathers that read it
+// pull one 128-byte line towards L2 (no register, no dependency): the bond-weight rows of a tile, read after its products.
+// The streamed rows (pa, saved pre / p, the per-bond products) are NOT prefetched a tile ahead: measured slower (DESIGN.md §4)
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // byte offset of 16-byte chunk c (0..15) of row r in a swizzled [128][64] fp32 tile
 __device__ __forceinline__ int swz(int r, int c) { return r * 256 + ((c ^ (r & 7)) << 4); }
@@ -178,17 +179,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_fwd_kernel(const Fused
         gi[2 * TR + gt] = a.idx2[r];
       }
       tc::wg_barrier(1 + half, 128);  // indices visible
-      {
-        // the rows of the NEXT tile that stream from HBM (p_b: per-bond products for AtomConv; p_c: per-angle products for
-        // BondConv): prefetch this group's half (2 lines of 128 B per row) towards L2 while this tile is gathered
-        const int nt = tile + gridDim.x;
-        if (nt < n_tiles) {
-          const int r = min(nt * TR + gt, a.n_rows - 1);
-          const float* row = MODE == BOND ? a.p_c + (size_t)r * 128 + half * 64 : a.p_b + (size_t)__ldg(a.idx2 + r) * 128 + half * 64;
-          prefetch_l2(row);
-          prefetch_l2(row + 32);
-        }
-      }
 #pragma unroll 1
       for (int b = 0; b < 16 / PB; ++b) {
         float4 v[PB];
@@ -490,15 +480,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         if (MODE == ATOM) s_pidx[2 * TR + t] = a.idx2[r];
       }
       tc::wg_barrier(1, 256);  // indices visible
-      {
-        const int nt = tile + gridDim.x;  // next tile of this CTA: its saved p rows stream from HBM (4 lines of 128 B per row)
-        if (nt < n_tiles) {
-          const int r = min(nt * TR + (t & 127), a.n_rows - 1);
-          const float* row = a.save_p + (size_t)r * 128 + (t >> 7) * 64;
-          prefetch_l2(row);
-          prefetch_l2(row + 32);
-        }
-      }
       float4 g1, g2, b1, b2v;
       if (use_ln) {
         g1 = lds4(s_ln + c0);
@@ -600,7 +581,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
     const int t = tid - 256;             // 0..255
     const int tx = t & 15, ty = t >> 4;
     const int c0 = tx * 4;
-    const int crow = t & 127, chalf = t >> 7;
     const int row0 = ((warp - 8) >> 2) * 64;  // this warpgroup's rows of the products
     const uint32_t img = tc::smem_u32(s_img);
     int tl = 0;
@@ -611,13 +591,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1) gated_ws_bwd_kernel(const BwdAr
         s_fidx[t] = a.idx0[r];
         s_fidx[TR + t] = a.idx1[r];
         s_fidx[2 * TR + t] = a.idx2[r];
-      }
-      {
-        // the rows this tile's silu' needs that stream from HBM: per-bond products (AtomConv) / saved pre (BondConv)
-        const int r = min(base + crow, a.n_rows - 1);
-        const float* row = MODE == ATOM ? a.p_b + (size_t)__ldg(a.idx2 + r) * 128 + chalf * 64 : a.save_pre + (size_t)r * 128 + chalf * 64;
-        prefetch_l2(row);
-        prefetch_l2(row + 32);
       }
       tc::mbar_wait(&bars.a_full, tl & 1);
 #pragma unroll 1

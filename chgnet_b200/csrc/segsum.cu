@@ -63,32 +63,32 @@ segment_sum_kernel(const float* __restrict__ data, const int32_t* __restrict__ p
           a0 = a0 + v0; a1 = a1 + v1; a2 = a2 + v2; a3 = a3 + v3;
         }
         for (; k < end; k += S) a0 = a0 + ldg4(base + (size_t)k * W);
-      } else {
+      } else {  // gathered: every input row is read once per call, evict-first (common.cuh)
         if (U == 8) {
           for (; k + 7 * S < end; k += 8 * S) {
             const int i0 = perm[k], i1 = perm[k + S], i2 = perm[k + 2 * S], i3 = perm[k + 3 * S];
             const int i4 = perm[k + 4 * S], i5 = perm[k + 5 * S], i6 = perm[k + 6 * S], i7 = perm[k + 7 * S];
-            const float4 v0 = ldg4(base + (size_t)i0 * W);
-            const float4 v1 = ldg4(base + (size_t)i1 * W);
-            const float4 v2 = ldg4(base + (size_t)i2 * W);
-            const float4 v3 = ldg4(base + (size_t)i3 * W);
-            const float4 v4 = ldg4(base + (size_t)i4 * W);
-            const float4 v5 = ldg4(base + (size_t)i5 * W);
-            const float4 v6 = ldg4(base + (size_t)i6 * W);
-            const float4 v7 = ldg4(base + (size_t)i7 * W);
+            const float4 v0 = ldg4_evict_first(base + (size_t)i0 * W);
+            const float4 v1 = ldg4_evict_first(base + (size_t)i1 * W);
+            const float4 v2 = ldg4_evict_first(base + (size_t)i2 * W);
+            const float4 v3 = ldg4_evict_first(base + (size_t)i3 * W);
+            const float4 v4 = ldg4_evict_first(base + (size_t)i4 * W);
+            const float4 v5 = ldg4_evict_first(base + (size_t)i5 * W);
+            const float4 v6 = ldg4_evict_first(base + (size_t)i6 * W);
+            const float4 v7 = ldg4_evict_first(base + (size_t)i7 * W);
             a0 = a0 + v0; a1 = a1 + v1; a2 = a2 + v2; a3 = a3 + v3;
             a0 = a0 + v4; a1 = a1 + v5; a2 = a2 + v6; a3 = a3 + v7;
           }
         }
         for (; k + 3 * S < end; k += 4 * S) {
           const int i0 = perm[k], i1 = perm[k + S], i2 = perm[k + 2 * S], i3 = perm[k + 3 * S];
-          const float4 v0 = ldg4(base + (size_t)i0 * W);
-          const float4 v1 = ldg4(base + (size_t)i1 * W);
-          const float4 v2 = ldg4(base + (size_t)i2 * W);
-          const float4 v3 = ldg4(base + (size_t)i3 * W);
+          const float4 v0 = ldg4_evict_first(base + (size_t)i0 * W);
+          const float4 v1 = ldg4_evict_first(base + (size_t)i1 * W);
+          const float4 v2 = ldg4_evict_first(base + (size_t)i2 * W);
+          const float4 v3 = ldg4_evict_first(base + (size_t)i3 * W);
           a0 = a0 + v0; a1 = a1 + v1; a2 = a2 + v2; a3 = a3 + v3;
         }
-        for (; k < end; k += S) a0 = a0 + ldg4(base + (size_t)perm[k] * W);
+        for (; k < end; k += S) a0 = a0 + ldg4_evict_first(base + (size_t)perm[k] * W);
       }
     }
     // fixed combination order -> bitwise reproducible
