@@ -80,6 +80,8 @@ SIGNATURES: dict[str, list] = {
     "chg_self_energy_spectrum": [P, I, I, I, I, P, I, P, I, P, I, P, P, I, D, P, I64, P, P],
     "chg_coherence_conductivity": [P, P, P, P, P, P, I, I, I, D, P, I64, P, P],
     "chg_isotope_scattering": [P, P, I, I, I, I, P, P, I, P, I, P, D, P, P, I64, P],
+    "chg_sample_displacements": [P, P, I, P, P, P, P, I64, I64, I64, I, P, I64, P, P, P],
+    "chg_displacement_moments": [P, P, P, P, I, I, I, P, I64, P, P],
 }
 
 # CHG_{DOS,TD,JDOS}_MAX_CHUNKS of include/chgnet_b200.h: the scratch blocks chg_tetrahedron_dos,
@@ -157,6 +159,18 @@ def isotope_scratch_doubles(n_target, n_q, n_band):
     """The scratch of one ``chg_isotope_scattering`` call: the overlaps [n_target, n_q, n_band, n_band] and
     ``ISO_MAX_CHUNKS`` chunks of [n_target, n_band] partial sums."""
     return n_target * n_q * n_band**2 + ISO_MAX_CHUNKS * n_target * n_band
+
+
+def sampler_scratch_doubles(n_samples, n_modes):
+    """The scratch of one ``chg_sample_displacements`` call: the amplitude-scaled normal variates [n_samples,
+    n_modes]."""
+    return n_samples * n_modes
+
+
+def moments_scratch_doubles(n_samples, n_prim, n_atoms):
+    """The scratch of one ``chg_displacement_moments`` call: the running sums and one slot per sample of the
+    18 n_prim n_atoms + 2 folded moments."""
+    return (1 + n_samples) * (18 * n_prim * n_atoms + 2)
 
 _lib = None
 
@@ -720,6 +734,45 @@ class CudaKernels:
         self._call("chg_isotope_scattering", _p(freqs), _p(eigvecs), nb, n1, n2, n3, _p(tetrahedra),
                    _p(mass_variances), nb // 3, _p(targets), n_target, _p(omega), float(cutoff_thz), _p(gamma),
                    _p(work), work.numel())
+
+    def sample_displacements(self, evecs, amp, inv_sqrt_m, frac_ref, lattice, inv_lattice, seed, iteration,
+                             first_sample, frac, u):
+        """frac [M N, 3] fp32 and u [M, N, 3] fp64 (written): the thermal displacement samples first_sample ...
+        first_sample + M - 1 of the supercell (``chg_sample_displacements``, DESIGN.md section 12.12): evecs
+        [3N, 3N] fp64 row lam the unit mode vector, amp [3N], inv_sqrt_m [N], frac_ref [N, 3], lattice and inv_lattice
+        [3, 3] fp64; the variates are a function of (seed, iteration, sample, mode) only."""
+        self._chk(evecs, amp, inv_sqrt_m, frac_ref, lattice, inv_lattice, frac, u)
+        n3 = evecs.shape[0]
+        m = u.shape[0]
+        if (any(t.dtype != torch.float64 for t in (evecs, amp, inv_sqrt_m, frac_ref, lattice, inv_lattice, u))
+                or frac.dtype != torch.float32 or n3 % 3 or tuple(evecs.shape) != (n3, n3) or tuple(amp.shape) != (n3,)
+                or tuple(inv_sqrt_m.shape) != (n3 // 3,) or tuple(frac_ref.shape) != (n3 // 3, 3)
+                or tuple(lattice.shape) != (3, 3) or tuple(inv_lattice.shape) != (3, 3)
+                or tuple(frac.shape) != (m * (n3 // 3), 3) or tuple(u.shape) != (m, n3 // 3, 3)):
+            raise ChgnetB200Error(f"sample_displacements: frac must be float32 [M N, 3] and every other tensor float64: "
+                                  f"evecs [3N, 3N], amp [3N], inv_sqrt_m [N], frac_ref [N, 3], lattice and "
+                                  f"inv_lattice [3, 3], u [M, N, 3]")
+        work = torch.empty(max(1, sampler_scratch_doubles(m, n3)), dtype=torch.float64, device=u.device)
+        self._call("chg_sample_displacements", _p(evecs), _p(amp), n3, _p(inv_sqrt_m), _p(frac_ref), _p(lattice),
+                   _p(inv_lattice), int(seed), int(iteration), int(first_sample), m, _p(work), work.numel(), _p(frac),
+                   _p(u))
+
+    def displacement_moments(self, u, force, f0, perm, acc):
+        """acc [2 n_prim 9 N + 2] fp64 += the folded moments G_c, B, sum |dF|^2 and sum f0 . u of the samples u and
+        force [M, N, 3] fp64 (``chg_displacement_moments``, DESIGN.md section 12.12): f0 [N, 3] fp64, perm [n_cells, N]
+        int32 the supercell translations, n_prim = N / n_cells."""
+        self._chk(u, force, f0, perm, acc)
+        m, n = u.shape[0], u.shape[1]
+        n_cells = perm.shape[0]
+        if (any(t.dtype != torch.float64 for t in (u, force, f0, acc)) or perm.dtype != torch.int32 or n_cells < 1
+                or n % n_cells or tuple(u.shape) != (m, n, 3) or tuple(force.shape) != (m, n, 3)
+                or tuple(f0.shape) != (n, 3) or tuple(perm.shape) != (n_cells, n)
+                or tuple(acc.shape) != (18 * (n // n_cells) * n + 2,)):
+            raise ChgnetB200Error("displacement_moments: u and force must be float64 [M, N, 3], f0 [N, 3], perm int32 "
+                                  "[n_cells, N] with n_cells dividing N, acc float64 [18 n_prim N + 2]")
+        work = torch.empty(max(1, moments_scratch_doubles(m, n // n_cells, n)), dtype=torch.float64, device=u.device)
+        self._call("chg_displacement_moments", _p(u), _p(force), _p(f0), _p(perm), n, n_cells, m, _p(work),
+                   work.numel(), _p(acc))
 
     def atom_conv_tan(self, pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d):
         self._chk(pcn_d, pe_d, wag, wag_d, center, nbr, d2u, save_pre, save_p, w2t, ln, msg_d, pre_d, p_d)

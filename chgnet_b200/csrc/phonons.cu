@@ -1611,6 +1611,177 @@ struct IsotopeStore {  // work[chunk][t][l]: gamma[t][l] = scale * omega[t][l]^2
   }
 };
 
+// ---------------------------------------------------------------------------------------------------------------
+// Effective force constants by stochastic sampling (DESIGN.md section 12.12).
+//
+// chg_sample_displacements, three stages: eff_variates_kernel writes xi[s][lam] = amp[lam] xi(seed, iteration,
+// first_sample + s, lam), the standard normal of a splitmix64 hash of the counter by Box-Muller, so a sample does not
+// depend on how the samples are split over calls; eff_superpose_kernel is the fp64 product d[s][i] = inv_sqrt_m[i / 3]
+// sum_lam xi[s][lam] E[lam][i] (64 x 64 output tiles, lam ascending, one thread 4 x 4 outputs); eff_positions_kernel
+// turns each atom's draw into fp32 fractional coordinates and writes the fp64 displacement the model sees,
+// u = (frac32 - fp32(frac_ref)) L.
+//
+// chg_displacement_moments: eff_moments_kernel, one thread per (sample, primitive atom kappa, supercell atom j), sums
+// over the n_cells translations l in order and writes the sample's partial sums of G_c and B for (kappa, j) to work
+// slot 1 + s; the thread (s, 0, 0) also writes the sample's |dF|^2 and F_0 . u; the threads of sample 0 copy the running
+// sums acc into slot 0.  chunk_reduce_kernel then adds the slots in order, acc = (((acc + p_0) + p_1) + ...): a left fold
+// over the samples in order, so the result is bitwise independent of how the samples are split over calls.  No atomics.
+constexpr int EFF_THREADS = 256;
+constexpr int EFF_TILE = 64;  // output tile of eff_superpose_kernel (samples x coordinates)
+constexpr int EFF_BK = 16;    // modes staged per step
+
+__device__ __forceinline__ uint64_t eff_mix(uint64_t x) {  // splitmix64
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
+__global__ void __launch_bounds__(EFF_THREADS)
+eff_variates_kernel(const double* __restrict__ amp, int n_modes, uint64_t seed, uint64_t iteration,
+                    uint64_t first_sample, int n_samples, double* __restrict__ xi) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_samples * n_modes) return;
+  const uint64_t s = first_sample + (uint64_t)(i / n_modes), lam = (uint64_t)(i % n_modes);
+  const uint64_t r = eff_mix(eff_mix(eff_mix(eff_mix(seed) + iteration) + s) + lam);
+  const double u1 = (double)((r >> 11) + 1) * 0x1.0p-53;  // (0, 1]
+  const double u2 = (double)(eff_mix(r) >> 11) * 0x1.0p-53;  // [0, 1)
+  xi[i] = __ldg(amp + lam) * (sqrt(-2.0 * log(u1)) * cospi(2.0 * u2));
+}
+
+__global__ void __launch_bounds__(EFF_THREADS)
+eff_superpose_kernel(const double* __restrict__ xi, const double* __restrict__ evecs,
+                     const double* __restrict__ inv_sqrt_m, int n_samples, int n_modes, double* __restrict__ d) {
+  __shared__ double sa[EFF_BK][EFF_TILE + 1];  // sa[lam][s]
+  __shared__ double sb[EFF_BK][EFF_TILE];      // sb[lam][i]
+  const int s0 = blockIdx.y * EFF_TILE, i0 = blockIdx.x * EFF_TILE;
+  const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
+  double acc[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
+  for (int k0 = 0; k0 < n_modes; k0 += EFF_BK) {
+    for (int e = threadIdx.x; e < EFF_BK * EFF_TILE; e += EFF_THREADS) {
+      const int r = e / EFF_BK, ka = e % EFF_BK;  // xi read along lam
+      const int s = s0 + r, la = k0 + ka;
+      sa[ka][r] = (s < n_samples && la < n_modes) ? __ldg(xi + (size_t)s * n_modes + la) : 0.0;
+      const int kb = e / EFF_TILE, c = e % EFF_TILE;  // E read along i
+      const int lb = k0 + kb, i = i0 + c;
+      sb[kb][c] = (lb < n_modes && i < n_modes) ? __ldg(evecs + (size_t)lb * n_modes + i) : 0.0;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < EFF_BK; ++k) {
+      double a[4], b[4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) a[r] = sa[k][ty + 16 * r];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) b[c] = sb[k][tx + 16 * c];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[r][c] = fma(a[r], b[c], acc[r][c]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int s = s0 + ty + 16 * r;
+    if (s >= n_samples) continue;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int i = i0 + tx + 16 * c;
+      if (i < n_modes) d[(size_t)s * n_modes + i] = acc[r][c] * __ldg(inv_sqrt_m + i / 3);
+    }
+  }
+}
+
+// u [s][a] holds the fp64 draw d on entry and the displacement the model sees on exit
+__global__ void __launch_bounds__(EFF_THREADS)
+eff_positions_kernel(const double* __restrict__ frac_ref, const double* __restrict__ lattice,
+                     const double* __restrict__ inv_lattice, int n_atoms, int n_samples, float* __restrict__ frac,
+                     double* __restrict__ u) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_samples * n_atoms) return;
+  const int a = (int)(i % n_atoms);
+  double* ui = u + (size_t)i * 3;
+  const double d[3] = {ui[0], ui[1], ui[2]};
+  double du[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const double ref = __ldg(frac_ref + (size_t)a * 3 + c);
+    const double x = ref + (d[0] * __ldg(inv_lattice + c) + d[1] * __ldg(inv_lattice + 3 + c) +
+                            d[2] * __ldg(inv_lattice + 6 + c));
+    const float x32 = __double2float_rn(x);
+    frac[(size_t)i * 3 + c] = x32;
+    du[c] = (double)x32 - (double)__double2float_rn(ref);
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+    ui[c] = du[0] * __ldg(lattice + c) + du[1] * __ldg(lattice + 3 + c) + du[2] * __ldg(lattice + 6 + c);
+}
+
+__global__ void __launch_bounds__(EFF_THREADS)
+eff_moments_kernel(const double* __restrict__ u, const double* __restrict__ force, const double* __restrict__ f0,
+                   const int32_t* __restrict__ perm, int n_atoms, int n_cells, int n_prim,
+                   const double* __restrict__ acc, double* __restrict__ work) {
+  const int64_t n_g = (int64_t)n_prim * 9 * n_atoms, n_out = 2 * n_g + 2;
+  const int s = blockIdx.y;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;  // kappa n_atoms + j
+  const double* us = u + (size_t)s * n_atoms * 3;
+  const double* fs = force + (size_t)s * n_atoms * 3;
+  double* w = work + (size_t)(s + 1) * n_out;
+  if (t < n_prim * n_atoms) {
+    const int k = t / n_atoms, j = t % n_atoms;
+    double g[9], b[9];
+#pragma unroll
+    for (int x = 0; x < 9; ++x) g[x] = b[x] = 0.0;
+    for (int l = 0; l < n_cells; ++l) {
+      const int a = __ldg(perm + (size_t)l * n_atoms + k * n_cells), c = __ldg(perm + (size_t)l * n_atoms + j);
+      double ua[3], df[3], uc[3];
+#pragma unroll
+      for (int x = 0; x < 3; ++x) {
+        ua[x] = __ldg(us + a * 3 + x);
+        df[x] = __ldg(fs + a * 3 + x) - __ldg(f0 + a * 3 + x);
+        uc[x] = __ldg(us + c * 3 + x);
+      }
+#pragma unroll
+      for (int x = 0; x < 3; ++x)
+#pragma unroll
+        for (int y = 0; y < 3; ++y) {
+          g[3 * x + y] = fma(ua[x], uc[y], g[3 * x + y]);
+          b[3 * x + y] = fma(df[x], uc[y], b[3 * x + y]);
+        }
+    }
+#pragma unroll
+    for (int x = 0; x < 3; ++x)
+#pragma unroll
+      for (int y = 0; y < 3; ++y) {
+        const int64_t o = ((int64_t)(k * 3 + x) * n_atoms + j) * 3 + y;
+        w[o] = g[3 * x + y];
+        w[n_g + o] = b[3 * x + y];
+        if (s == 0) work[o] = acc[o], work[n_g + o] = acc[n_g + o];
+      }
+  }
+  if (t == 0) {
+    double ss = 0.0, wf = 0.0;
+    for (int i = 0; i < 3 * n_atoms; ++i) {
+      const double f = __ldg(f0 + i), df = __ldg(fs + i) - f;
+      ss = fma(df, df, ss);
+      wf = fma(f, __ldg(us + i), wf);
+    }
+    w[2 * n_g] = ss;
+    w[2 * n_g + 1] = wf;
+    if (s == 0) work[2 * n_g] = acc[2 * n_g], work[2 * n_g + 1] = acc[2 * n_g + 1];
+  }
+}
+
+struct CopyStore {  // out[o] = the sum
+  double* out;
+  __device__ void operator()(int64_t o, double s) const { out[o] = s; }
+};
+
 }  // namespace
 }  // namespace chg
 
@@ -1968,5 +2139,52 @@ extern "C" int chg_isotope_scattering(const double* freqs, const double* eigvecs
       freqs, n_band, n1, n2, n3, tetrahedra, omega, work, n_target, l_tile, cutoff_thz, partial);
   const double scale = 3.141592653589793 / (4.0 * 6.0 * (double)n_q);
   CHG_CUDA(reduce_chunks(partial, chunks, (int64_t)n_target * n_band, IsotopeStore{gamma, omega, scale}, st));
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_sample_displacements(const double* evecs, const double* amp, int32_t n_modes,
+                                        const double* inv_sqrt_m, const double* frac_ref, const double* lattice,
+                                        const double* inv_lattice, int64_t seed, int64_t iteration,
+                                        int64_t first_sample, int32_t n_samples, double* work, int64_t work_doubles,
+                                        float* frac, double* u, void* stream) {
+  CHG_CHECK_ARG(n_modes >= 0 && n_modes % 3 == 0 && n_samples >= 0, "bad size (n_modes must be 3 n_atoms)");
+  CHG_CHECK_ARG(seed >= 0 && iteration >= 0 && first_sample >= 0, "seed, iteration and first_sample must be >= 0");
+  if (n_modes == 0 || n_samples == 0) return CHG_OK;
+  CHG_CHECK_ARG(evecs && amp && inv_sqrt_m && frac_ref && lattice && inv_lattice && work && frac && u, "null pointer");
+  const int64_t tiles_s = ((int64_t)n_samples + EFF_TILE - 1) / EFF_TILE;
+  CHG_CHECK_ARG(tiles_s <= 65535, "too many samples in one call (at most 65535 * 64)");
+  const int64_t n_xi = (int64_t)n_samples * n_modes;
+  CHG_CHECK_ARG(work_doubles >= n_xi, "work holds less than n_samples n_modes doubles");
+  cudaStream_t st = as_stream(stream);
+  eff_variates_kernel<<<(unsigned)((n_xi + EFF_THREADS - 1) / EFF_THREADS), EFF_THREADS, 0, st>>>(
+      amp, n_modes, (uint64_t)seed, (uint64_t)iteration, (uint64_t)first_sample, n_samples, work);
+  count_launch();
+  const dim3 grid((unsigned)((n_modes + EFF_TILE - 1) / EFF_TILE), (unsigned)tiles_s);
+  eff_superpose_kernel<<<grid, EFF_THREADS, 0, st>>>(work, evecs, inv_sqrt_m, n_samples, n_modes, u);
+  count_launch();
+  const int64_t n_items = (int64_t)n_samples * (n_modes / 3);
+  eff_positions_kernel<<<(unsigned)((n_items + EFF_THREADS - 1) / EFF_THREADS), EFF_THREADS, 0, st>>>(
+      frac_ref, lattice, inv_lattice, n_modes / 3, n_samples, frac, u);
+  CHG_LAUNCH_END();
+}
+
+extern "C" int chg_displacement_moments(const double* u, const double* force, const double* f0, const int32_t* perm,
+                                        int32_t n_atoms, int32_t n_cells, int32_t n_samples, double* work,
+                                        int64_t work_doubles, double* acc, void* stream) {
+  CHG_CHECK_ARG(n_atoms >= 0 && n_cells > 0 && n_samples >= 0 && n_atoms % n_cells == 0,
+                "bad size (n_atoms must be a multiple of n_cells)");
+  CHG_CHECK_ARG(n_samples <= 65535, "too many samples in one call (at most 65535)");
+  if (n_atoms == 0 || n_samples == 0) return CHG_OK;
+  CHG_CHECK_ARG(u && force && f0 && perm && work && acc, "null pointer");
+  const int n_prim = n_atoms / n_cells;
+  const int64_t n_out = 18 * (int64_t)n_prim * n_atoms + 2;
+  CHG_CHECK_ARG(n_out < (1ll << 31), "supercell too large");
+  CHG_CHECK_ARG(work_doubles >= (1 + (int64_t)n_samples) * n_out,
+                "work holds less than (1 + n_samples) (18 n_prim n_atoms + 2) doubles");
+  cudaStream_t st = as_stream(stream);
+  const int64_t pairs = (int64_t)n_prim * n_atoms;
+  const dim3 grid((unsigned)((pairs + EFF_THREADS - 1) / EFF_THREADS), (unsigned)n_samples);
+  eff_moments_kernel<<<grid, EFF_THREADS, 0, st>>>(u, force, f0, perm, n_atoms, n_cells, n_prim, acc, work);
+  CHG_CUDA(reduce_chunks(work, 1 + n_samples, n_out, CopyStore{acc}, st));
   CHG_LAUNCH_END();
 }

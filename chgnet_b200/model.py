@@ -341,6 +341,25 @@ class StaticGraphEvaluator:
         return preds[0] if self.single else preds
 
 
+class _ReplicaForces:
+    """forces(frac [M, N, 3] fp64) -> (F [M, N, 3] fp64, E [M] fp64) of displaced copies of the supercell ``sc``
+    (``CHGNet.effective_phonons``): each copy gets its own exact graph (``structures_to_batch``, built by the
+    library's worker threads), and the M copies go through one ``chg_forward``.  A shared graph of the reference
+    positions with cutoffs widened by a skin would avoid the builds, but soft and imaginary modes sampled at the
+    frequency floor move atoms by an angstrom or more, and the skin's angles grow like ((3 + skin) / 3)^6
+    (DESIGN.md section 12.12)."""
+
+    def __init__(self, model, sc) -> None:
+        self.model, self.sc = model.eval(), sc
+
+    def __call__(self, frac):
+        m, n = frac.shape[0], frac.shape[1]
+        x = frac.detach().cpu().numpy()
+        b = self.model.structures_to_batch([(self.sc.z, x[s], self.sc.lattice) for s in range(m)])
+        res = self.model._get_native()(b, need_grad=True)
+        return res["force"].view(m, n, 3), res["energy"] + res["e_ref"]
+
+
 class CHGNet(nn.Module):
     """Crystal Hamiltonian Graph neural Network — H100 kernel path."""
 
@@ -940,6 +959,49 @@ class CHGNet(nn.Module):
             fc3 = third_order_force_constants(
                 lambda frac, v: self._hvp_replicas(self.graph_converter((sc.z, frac, sc.lattice)), v, batch_size), sc, h)
         return Phonons(fc, sc, fc3=fc3, device=self.device)
+
+    def effective_phonons(self, structure, supercell_matrix, temperature, *, n_samples: int = 256,
+                          n_iterations: int = 5, mixing: float = 0.5, quantum: bool = True,
+                          frequency_floor: float = 0.5, seed: int = 0, batch_size: int = 16):
+        """Phonons of temperature-dependent effective force constants, fitted to the model's forces on thermally
+        displaced supercells and iterated until the fit reproduces the distribution it was sampled from (stochastic
+        TDEP / self-consistent phonons; ``chgnet_b200.phonons.effective_force_constants``, DESIGN.md section 12.12).
+
+        ``structure`` and ``supercell_matrix`` are what ``phonons`` accepts; ``temperature`` is one value in K.  The
+        start is ``phonons(structure, supercell_matrix)``; each of the ``n_iterations`` iterations samples
+        ``n_samples`` supercells (``quantum`` or classical amplitudes, modes below ``frequency_floor`` THz sampled at
+        the floor, normal variates a function of ``seed``, iteration, sample and mode only), evaluates them
+        ``batch_size`` at a time as copies of one graph, fits force constants to the forces and mixes them in with
+        ``mixing``.  Returns a ``chgnet_b200.phonons.Phonons`` of the effective force constants, so every method of it
+        gives finite-temperature results, with one more attribute, ``effective``: a dict of ``temperature``,
+        ``quantum``, ``harmonic_force_constants`` (the start), ``history`` (per iteration ``max_change``,
+        ``n_imaginary``, ``sigma_a``, ``u0``) and the last ``sigma_a`` and ``u0`` (eV per primitive cell; the free
+        energy is F(T) ~ ``thermal_properties(mesh, T)["free_energy"] + u0``).
+
+        For the thermal conductivity of the effective fc2 with the harmonic fc3:
+        ``Phonons(ph.force_constants, ph.cell, fc3=model.phonons(..., third_order=True).force_constants3)``.
+
+        Each sample gets an exact graph of its own, built on the host by the library's worker threads
+        (``structures_to_batch``); the sampled positions, forces and moments stay on the device.  ValueError for a negative
+        or non-finite temperature, ``quantum=False`` at T = 0, ``n_iterations < 1``, ``mixing`` outside (0, 1],
+        ``frequency_floor <= 0``, ``batch_size < 1``, a negative seed, or n_samples n_cells < 3N - 3 (raised before
+        any model call)."""
+        from chgnet_b200.phonons import (Phonons, check_effective_arguments, effective_force_constants,
+                                         make_supercell)
+
+        if self.graph_converter is None:
+            raise ValueError("graph_converter cannot be None!")
+        sc = make_supercell(*self._structure_arrays(structure), supercell_matrix)
+        kw = dict(n_samples=n_samples, n_iterations=n_iterations, mixing=mixing, quantum=quantum,
+                  frequency_floor=frequency_floor, seed=seed, batch_size=batch_size)
+        check_effective_arguments(temperature, len(sc.z), len(sc.points), **kw)
+        harmonic = self.phonons(structure, supercell_matrix, batch_size=batch_size)
+        forces = _ReplicaForces(self, sc)
+        fc, info = effective_force_constants(forces, sc, harmonic.force_constants, temperature, device=self.device,
+                                             **kw)
+        ph = Phonons(fc, sc, device=self.device)
+        ph.effective = info
+        return ph
 
     def static_evaluator(self, graph, *, task: PredTask = "efsm"):
         """Evaluator for graph(s) whose TOPOLOGY stays fixed while coordinates / cells change (finite differences,

@@ -19,7 +19,9 @@
   linewidths (``chg_imag_self_energy``) and the lattice thermal conductivity in the relaxation-time approximation;
   frequency-resolved self-energies (``chg_self_energy_spectrum``) and anharmonic phonon spectral functions; the Wigner
   coherence term of the thermal conductivity (``chg_coherence_conductivity``); isotope scattering rates
-  (``chg_isotope_scattering``, no fc3 needed) and isotope and boundary scattering in every thermal conductivity.
+  (``chg_isotope_scattering``, no fc3 needed) and isotope and boundary scattering in every thermal conductivity;
+  temperature-dependent effective force constants fitted to the forces of thermally displaced supercells
+  (``effective_force_constants``, with ``chg_sample_displacements`` and ``chg_displacement_moments``).
 
 Units: eV/A^2 for force constants, amu for masses, THz for frequencies (imaginary modes as negative numbers),
 eV and eV/K per primitive cell for the thermodynamic functions, THz*A (100 m/s) for group velocities, states/THz per
@@ -409,6 +411,194 @@ def fibonacci_directions(n: int) -> np.ndarray:
     r = np.sqrt(1.0 - z * z)
     phi = i * (math.pi * (3.0 - math.sqrt(5.0)))
     return np.stack([r * np.cos(phi), r * np.sin(phi), z], axis=1)
+
+
+def translation_table(sc: Supercell) -> np.ndarray:
+    """[n_cells, N] int32 ``perm[l, j]``: the supercell atom that the lattice translation R_l (``sc.points[l]``) moves
+    atom j to.  Atom j = k n_cells + l' goes to k n_cells + (the point R_l + R_l' reduced modulo the supercell lattice),
+    found by integer arithmetic in primitive fractional coordinates, so any integer M works."""
+    m = np.asarray(sc.matrix, dtype=np.int64)
+    det = int(round(np.linalg.det(m)))
+    adj = np.round(np.linalg.inv(m) * det).astype(np.int64)  # det M^-1, integral
+
+    def code(n):  # the point n modulo the supercell lattice, as one integer
+        x = (n @ adj) % det
+        return (x[..., 0] * det + x[..., 1]) * det + x[..., 2]
+
+    pts = np.asarray(sc.points, dtype=np.int64)
+    n_cells = len(pts)
+    keys = code(pts)
+    order = np.argsort(keys)
+    cell = order[np.searchsorted(keys[order], code(pts[:, None, :] + pts[None, :, :]))]  # [l, l']
+    n_prim = len(sc.p2s)
+    perm = (np.arange(n_prim)[None, :, None] * n_cells + cell[:, None, :]).reshape(n_cells, n_prim * n_cells)
+    return np.ascontiguousarray(perm, dtype=np.int32)
+
+
+def _expand_compact(x: torch.Tensor, perm_inv: torch.Tensor) -> torch.Tensor:
+    """[3N, 3N] supercell matrix X_sc[(T_l(p2s k), a), (T_l(j), b)] = x[k, j, a, b] of the compact x [n_prim, N, 3, 3],
+    atom-major (T_l(p2s k) = k n_cells + l); perm_inv [n_cells, N] long, perm_inv[l, perm[l, j]] = j."""
+    n = x.shape[1]
+    return x[:, perm_inv].reshape(n, n, 3, 3).permute(0, 2, 1, 3).reshape(3 * n, 3 * n)
+
+
+def sampling_modes(phi_sc: torch.Tensor, masses: np.ndarray, temperature: float, *, quantum: bool,
+                   frequency_floor: float):
+    """The modes of the supercell force constants ``phi_sc`` [3N, 3N] (eV/A^2, on the device) and the sampling
+    amplitudes of ``effective_force_constants`` (DESIGN.md section 12.12), for the atom ``masses`` [N] (amu).
+
+    D_sc = phi_sc / sqrt(m m'), made symmetric as (D + D^T) / 2, is diagonalised by ``torch.linalg.eigh`` in fp64.
+    Mode lam (signed THz, as ``Phonons.frequencies``) is sampled at nu~ = max(|nu|, ``frequency_floor``) with the
+    amplitude A (amu^1/2 A), A^2 = C / nu~ coth(h nu~ / 2 k T) (``quantum``, C = ``DISPLACEMENT_A2_AMU_THZ``) or
+    k T (``THZ_PER_SQRT_EV_A2_AMU`` / nu~)^2 (classical); the three modes of smallest |nu| (the translations) get 0.
+    Returns ``(nu [3N], evecs [3N, 3N] row lam the unit mode vector, amp [3N], n_imaginary)``, ``n_imaginary`` the
+    number of modes below -``THERMAL_CUTOFF_THZ``.  The displacement covariance of the samples is
+    sum_lam A_lam^2 (e_lam / sqrt m)(e_lam / sqrt m)^T."""
+    inv = torch.as_tensor(np.repeat(1.0 / np.sqrt(np.asarray(masses, dtype=np.float64)), 3)).to(phi_sc.device)
+    d = phi_sc * inv[:, None] * inv[None, :]
+    lam, e = torch.linalg.eigh(0.5 * (d + d.T))
+    nu = _signed_thz(lam)
+    nt = nu.abs().clamp_min(frequency_floor)
+    t = float(temperature)
+    if quantum:
+        occ = 1.0 / torch.tanh(H_OVER_KB_K_PER_THZ * nt / (2.0 * t)) if t > 0 else torch.ones_like(nt)
+        a2 = DISPLACEMENT_A2_AMU_THZ / nt * occ
+    else:
+        a2 = KB * t * (THZ_PER_SQRT_EV_A2_AMU / nt) ** 2
+    a2[torch.argsort(nu.abs(), stable=True)[:3]] = 0.0
+    return nu, e.T.contiguous(), torch.sqrt(a2), int((nu < -THERMAL_CUTOFF_THZ).sum())
+
+
+def check_effective_arguments(temperature, n_atoms: int, n_cells: int, *, n_samples, n_iterations, mixing, quantum,
+                              frequency_floor, seed, batch_size) -> float:
+    """The temperature (K) as a float; ValueError for any argument ``effective_force_constants`` rejects."""
+    t = float(temperature)
+    if not (math.isfinite(t) and t >= 0):
+        raise ValueError(f"temperature must be finite and non-negative, got {temperature!r}")
+    if not quantum and t == 0:
+        raise ValueError("a classical distribution at T = 0 has zero amplitude: use quantum=True or T > 0")
+    if int(n_iterations) != n_iterations or n_iterations < 1:
+        raise ValueError(f"n_iterations must be an integer >= 1, got {n_iterations!r}")
+    if not (0 < float(mixing) <= 1):
+        raise ValueError(f"mixing must lie in (0, 1], got {mixing!r}")
+    if not (math.isfinite(float(frequency_floor)) and frequency_floor > 0):
+        raise ValueError(f"frequency_floor must be finite and positive, got {frequency_floor!r}")
+    if int(batch_size) != batch_size or batch_size < 1:
+        raise ValueError(f"batch_size must be an integer >= 1, got {batch_size!r}")
+    if int(seed) != seed or seed < 0 or seed >= 2**63:
+        raise ValueError(f"seed must be an integer in [0, 2^63), got {seed!r}")
+    if int(n_samples) != n_samples or n_samples * n_cells < 3 * n_atoms - 3:
+        raise ValueError(f"n_samples * n_cells = {n_samples} * {n_cells} must be at least 3N - 3 = {3 * n_atoms - 3}: "
+                         "fewer samples leave the fit underdetermined")
+    return t
+
+
+def effective_force_constants(forces, sc: Supercell, fc0, temperature, *, kernels=None, device="cuda",
+                              n_samples: int = 256, n_iterations: int = 5, mixing: float = 0.5, quantum: bool = True,
+                              frequency_floor: float = 0.5, seed: int = 0, batch_size: int = 16):
+    """Temperature-dependent effective harmonic force constants by stochastic sampling (sTDEP / self-consistent
+    phonons; DESIGN.md section 12.12).  Returns ``(fc [n_prim, N, 3, 3], info)``.
+
+    ``forces(frac [M, N, 3] torch fp64) -> (F [M, N, 3] fp64, E [M] fp64)`` gives the forces (eV/A) and total energies
+    (eV) of M copies of the supercell ``sc`` with the fractional coordinates ``frac`` (same lattice, not wrapped);
+    it is called with at most ``batch_size`` copies, first once with the reference positions.  ``fc0`` are the
+    starting compact force constants (``CHGNet.phonons``); the self-term acoustic-sum-rule correction of ``Phonons``
+    is applied to them first.  Iteration i:
+
+    1. the supercell modes of Phi_i and their amplitudes at ``temperature`` (K), ``quantum`` or classical
+       (``sampling_modes``);
+    2. ``n_samples`` displacement samples u_s = M^-1/2 sum_lam e_lam A_lam xi_s,lam with normal variates that are a
+       function of (``seed``, i, s, lam) only, as fp32 fractional coordinates, u_s being the displacement those
+       coordinates carry (``chg_sample_displacements``);
+    3. their forces, and the moments G_c, B and S folded over the supercell translations
+       (``chg_displacement_moments``), dF = F - F_0 with F_0 the forces of the reference positions;
+    4. the fit Phi_fit = -B G+: G is the full Gram matrix of the displacements, projected on the complement of the
+       rigid translations, and G+ inverts it by ``eigh`` treating eigenvalues <= 1e-10 max as zero.  The samples hold
+       no mass-weighted translation, so the fit is undetermined along three directions; the projection fixes them by
+       the acoustic sum rule (sum_j Phi[k, j] = 0), and for harmonic forces the fit is exact.  Returned as computed
+       (not symmetrised); Phi_i+1 = Phi_i + ``mixing`` (Phi_fit - Phi_i).
+
+    ``info``: ``temperature``, ``quantum``, ``harmonic_force_constants`` (``fc0``) and ``history``, one dict per
+    iteration with ``max_change`` max |Phi_fit - Phi_i| (eV/A^2), ``n_imaginary`` (modes of Phi_i below
+    -``THERMAL_CUTOFF_THZ`` in the supercell), ``sigma_a`` and ``u0``; and the last iteration's ``sigma_a`` and ``u0``:
+
+    * ``sigma_a``: Knoop's anharmonicity measure of Phi_fit, sqrt(sum_s |dF_s + Phi_sc u_s|^2 / S), S = sum_s |dF_s|^2,
+      from the moments (S + 2 <Phi_fit, B> + <Phi_fit, G Phi_fit>).  The sum cancels in fp64, so values below ~1e-7
+      are rounding;
+    * ``u0`` (eV per primitive cell): the TDEP free-energy correction < E_s - E_0 + F_0 . u_s - u_s Phi_sc u_s / 2 >
+      / n_cells with Phi_fit.  F(T) ~ ``Phonons(fc, sc).thermal_properties(mesh, T)["free_energy"] + u0``.
+
+    ``kernels`` holds ``sample_displacements`` and ``displacement_moments`` (default: the CUDA kernels on ``device``).
+    ValueError for the arguments ``check_effective_arguments`` rejects."""
+    n_prim, n = len(sc.p2s), len(sc.s2p)
+    n_cells = len(sc.points)
+    t = check_effective_arguments(temperature, n, n_cells, n_samples=n_samples, n_iterations=n_iterations,
+                                  mixing=mixing, quantum=quantum, frequency_floor=frequency_floor, seed=seed,
+                                  batch_size=batch_size)
+    fc0 = np.asarray(fc0, dtype=np.float64)
+    if fc0.shape != (n_prim, n, 3, 3):
+        raise ValueError(f"force constants must have shape {[n_prim, n, 3, 3]}, got {list(fc0.shape)}")
+    if kernels is None:
+        from chgnet_b200._lib import CudaKernels
+
+        kernels = CudaKernels(device)
+    dev, f64 = torch.device(device), torch.float64
+    perm = translation_table(sc)
+    perm_inv = np.empty_like(perm)
+    np.put_along_axis(perm_inv, perm, np.arange(n)[None, :].repeat(n_cells, 0), axis=1)
+    perm_t = torch.as_tensor(perm).to(dev)
+    perm_inv_t = torch.as_tensor(perm_inv.astype(np.int64)).to(dev)
+    masses = ATOMIC_MASSES[np.asarray(sc.z) - 1]
+    inv_sqrt_m = torch.as_tensor(1.0 / np.sqrt(masses)).to(dev)
+    frac_ref = torch.as_tensor(np.ascontiguousarray(sc.frac, dtype=np.float64)).to(dev)
+    lat = np.ascontiguousarray(sc.lattice, dtype=np.float64)
+    lat_t, inv_lat_t = torch.as_tensor(lat).to(dev), torch.as_tensor(np.linalg.inv(lat)).to(dev)
+    n3, n_g = 3 * n, 9 * n_prim * n
+    # the rigid translations t_a[j, b] = delta_ab / sqrt N and the projector on their complement
+    trans = torch.zeros(3, n3, dtype=f64, device=dev)
+    for a in range(3):
+        trans[a, a::3] = 1.0 / math.sqrt(n)
+    proj = torch.eye(n3, dtype=f64, device=dev) - trans.T @ trans
+
+    bs = min(int(batch_size), int(n_samples))
+    frac = torch.empty(bs * n, 3, dtype=torch.float32, device=dev)
+    u = torch.empty(bs, n, 3, dtype=f64, device=dev)
+    f0, e0 = forces(frac_ref.to(torch.float32).to(f64).view(1, n, 3))
+    f0 = f0.reshape(n, 3).to(dev, f64).contiguous()
+    e0 = e0.reshape(-1)[:1].to(dev, f64)
+    acc = torch.empty(2 * n_g + 2, dtype=f64, device=dev)
+    energies = torch.empty(int(n_samples), dtype=f64, device=dev)
+    phi = torch.as_tensor(acoustic_sum_rule(fc0, sc.p2s)[0]).to(dev)
+    history = []
+    for it in range(int(n_iterations)):
+        _, evecs, amp, n_imag = sampling_modes(_expand_compact(phi, perm_inv_t), masses, t, quantum=quantum,
+                                               frequency_floor=frequency_floor)
+        acc.zero_()
+        for s0 in range(0, int(n_samples), bs):
+            m = min(bs, int(n_samples) - s0)
+            kernels.sample_displacements(evecs, amp, inv_sqrt_m, frac_ref, lat_t, inv_lat_t, seed, it, s0,
+                                         frac[: m * n], u[:m])
+            f, e = forces(frac[: m * n].view(m, n, 3).to(f64))
+            kernels.displacement_moments(u[:m], f.reshape(m, n, 3).to(dev, f64).contiguous(), f0, perm_t, acc)
+            energies[s0 : s0 + m] = e.reshape(-1).to(dev, f64)
+        g_c, b = acc[:n_g].view(n_prim * 3, n3), acc[n_g : 2 * n_g].view(n_prim * 3, n3)
+        ss, wf = acc[2 * n_g], acc[2 * n_g + 1]
+        g = _expand_compact(g_c.view(n_prim, 3, n, 3).permute(0, 2, 1, 3), perm_inv_t)
+        gp = proj @ g @ proj
+        lam, v = torch.linalg.eigh(0.5 * (gp + gp.T))
+        keep = lam > 1e-10 * lam.max()
+        vk = v[:, keep]
+        fit_rows = -((b @ vk) / lam[keep]) @ vk.T  # [3 n_prim, 3N], rows (k, a), columns (j, b)
+        fit = fit_rows.view(n_prim, 3, n, 3).permute(0, 2, 1, 3)
+        res2 = ss + 2.0 * (fit_rows * b).sum() + ((fit_rows @ g) * fit_rows).sum()
+        sigma = float(torch.sqrt(res2.clamp_min(0.0) / ss)) if float(ss) > 0 else 0.0
+        u0 = float(((energies - e0).sum() + wf - 0.5 * (fit_rows * g_c).sum()) / (n_samples * n_cells))
+        history.append({"max_change": float((fit - phi).abs().max()), "n_imaginary": n_imag, "sigma_a": sigma,
+                        "u0": u0})
+        phi = phi + float(mixing) * (fit - phi)
+    info = {"temperature": t, "quantum": bool(quantum), "harmonic_force_constants": fc0, "history": history,
+            "sigma_a": history[-1]["sigma_a"], "u0": history[-1]["u0"]}
+    return np.ascontiguousarray(phi.cpu().numpy()), info
 
 
 class Phonons:

@@ -710,6 +710,34 @@ int chg_isotope_scattering(const double* freqs, const double* eigvecs, int32_t n
                            int32_t n3, const int32_t* tetrahedra, const double* mass_variances, int32_t n_prim,
                            const int32_t* targets, int32_t n_target, const double* omega, double cutoff_thz,
                            double* gamma, double* work, int64_t work_doubles, void* stream);
+/* Thermal displacement samples of a supercell (DESIGN.md section 12.12).  For samples s = first_sample ...
+ * first_sample + n_samples - 1 and the N = n_modes / 3 atoms:
+ *   d[s][i] = inv_sqrt_m[i / 3] sum_lam E[lam][i] amp[lam] xi(seed, iteration, s, lam)   (fp64, lam ascending),
+ *   frac[s][a] = fp32(frac_ref[a] + d[s][a] inv_lattice)   (not wrapped),
+ *   u[s][a] = ((double)frac[s][a] - (double)fp32(frac_ref[a])) lattice   (A, the displacement the model sees),
+ * xi the standard normal of Box-Muller on r = h(h(h(h(seed) + iteration) + s) + lam), h = splitmix64, with
+ * u1 = ((r >> 11) + 1) 2^-53 and u2 = (h(r) >> 11) 2^-53: xi = sqrt(-2 ln u1) cos(2 pi u2).  evecs [n_modes][n_modes]
+ * row lam the unit mode vector; amp [n_modes] (amu^1/2 A); inv_sqrt_m [N]; frac_ref [N][3]; lattice and inv_lattice
+ * [3][3] (rows are lattice vectors); frac [n_samples N][3] fp32 and u [n_samples][N][3] fp64 (written).  seed,
+ * iteration, first_sample >= 0.  work: at least n_samples n_modes doubles (work_doubles).  A sample does not depend on
+ * the other samples of the call.                                                                                   */
+int chg_sample_displacements(const double* evecs, const double* amp, int32_t n_modes, const double* inv_sqrt_m,
+                             const double* frac_ref, const double* lattice, const double* inv_lattice, int64_t seed,
+                             int64_t iteration, int64_t first_sample, int32_t n_samples, double* work,
+                             int64_t work_doubles, float* frac, double* u, void* stream);
+/* Displacement-force moments folded over the supercell translations (DESIGN.md section 12.12), accumulated into
+ * acc [2 n_prim 9 N + 2] (n_prim = N / n_cells, atom-major supercell: atom kappa n_cells is primitive atom kappa at
+ * the origin cell):
+ *   acc[G_c[kappa][b][j][b']] += sum_s sum_l u[s][T_l(kappa n_cells)][b] u[s][T_l(j)][b'],
+ *   acc[n_prim 9 N + B[kappa][a][j][b]] += sum_s sum_l dF[s][T_l(kappa n_cells)][a] u[s][T_l(j)][b],
+ *   acc[2 n_prim 9 N] += sum_s |dF[s]|^2,   acc[2 n_prim 9 N + 1] += sum_s f0 . u[s],
+ * dF = force - f0, T_l(j) = perm[l][j].  u and force [n_samples][N][3] fp64, f0 [N][3], perm [n_cells][N] int32;
+ * n_samples <= 65535.  work: at least (1 + n_samples) (18 n_prim N + 2) doubles (work_doubles).  Deterministic: each
+ * sample's sums run in a fixed order and are added to acc one sample after the other, no atomics, so the result does
+ * not depend on how the samples are split over calls.                                                              */
+int chg_displacement_moments(const double* u, const double* force, const double* f0, const int32_t* perm,
+                             int32_t n_atoms, int32_t n_cells, int32_t n_samples, double* work, int64_t work_doubles,
+                             double* acc, void* stream);
 
 #ifdef __cplusplus
 }
